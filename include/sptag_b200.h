@@ -27,7 +27,9 @@ extern "C" {
 #define SPTAG_B200_FAILED_PARSE_VALUE 0x0011
 #define SPTAG_B200_MEMORY_OVERFLOW 0x0012
 #define SPTAG_B200_LACK_OF_INPUTS 0x0013
+#define SPTAG_B200_VECTOR_NOT_FOUND 0x0014
 #define SPTAG_B200_EMPTY_INDEX 0x0015
+#define SPTAG_B200_EMPTY_DATA 0x0016
 #define SPTAG_B200_DIMENSION_MISMATCH 0x0017
 
 /* enum orders follow inc/Core/DefinitionList.h:6-9 (VectorValueType), :36-38 (DistCalcMethod),
@@ -112,7 +114,8 @@ void sptag_b200_destroy(sptag_b200_handle h);
 /* Replaces: VectorIndex::SetParameter / GetParameter (BKTIndex.cpp:980-1025) for the search-time
  * parameters, same names as the ini file: MaxCheck, MaxCheckForRefineGraph,
  * NumberOfInitialDynamicPivots, NumberOfOtherDynamicPivots,
- * ThresholdOfNumberOfContinuousNoBetterPropagation; "EnableADC" = VectorIndex::SetQuantizerADC
+ * ThresholdOfNumberOfContinuousNoBetterPropagation; the update parameters AddCEF (500), CEF (1000) and RNGFactor (1.0,
+ * a float) used by sptag_b200_add / sptag_b200_delete_vectors; "EnableADC" = VectorIndex::SetQuantizerADC
  * (VectorIndex.h:136-138) for quantized indexes; "SearchDeleted" (0/1) = the handle-wide DEFAULT of the
  * p_searchDeleted argument (the per-call value is sptag_b200_search_options.search_deleted /
  * sptag_b200_iterator_open_ex); the refine pass always runs with 0 like NeighborhoodGraph::RefineNode.  Additional B200 tuning knobs (not in the
@@ -292,6 +295,55 @@ int sptag_b200_group_create(const sptag_b200_handle* shards, int32_t num_shards,
 int sptag_b200_group_search(sptag_b200_group g, const void* queries, int32_t num_queries, int32_t k, int32_t* out_ids,
                             float* out_dists);
 void sptag_b200_group_destroy(sptag_b200_group g);
+
+/* ---- Index mutation ----
+ * Every call below takes the handle's lock and runs after every kernel already launched on the handle, so a concurrent
+ * search sees all of a mutation or none of it.  add / delete / delete_vectors return Fail while an iterator of the handle
+ * is open (its per-query visited sets are sized to the vector count).  A handle in a shard group may be mutated between
+ * group searches: the group reads each shard's current size on every search.  Quantized indexes: add, delete_vectors
+ * and save return LackOfInputs; delete by id works on them (it only sets tombstone bytes).
+ *
+ * Replaces: VectorIndex::DeleteIndex(const SizeType& id) per id, in array order (BKTIndex.cpp:893-899, KDTIndex.cpp:619-625,
+ * Labelset::Insert, Labelset.h:59-76).  ids are the ids search returns (id_offset is subtracted).  out_codes (HOST, nullable)
+ * [num]: Success, or VectorNotFound for an id that is already deleted or repeated earlier in the array.  An id outside
+ * the index gets VectorNotFound; the reference tombstones nothing for it either, but answers Success for ids >= R
+ * (InvalidIDBehavior::AlwaysContains, Labelset.h:43-57) and is undefined for negative ids.  The tombstone map is created on the
+ * first deletion and the searches test it from then on (Labelset::Count() > 0, BKTIndex.cpp:473). */
+int sptag_b200_delete(sptag_b200_handle h, const int32_t* ids, int32_t num, int32_t* out_codes);
+
+/* Replaces: VectorIndex::DeleteIndex(const void* p_vectors, SizeType num) (BKTIndex.cpp:876-890, KDTIndex.cpp:602-616):
+ * for every vector SearchIndex (the index's MaxCheck, searchDeleted = false, K = CEF), then DeleteIndex of every result
+ * with Dist < 1e-6.  The reference runs the vectors under OpenMP, where one deletion can change a later search; this
+ * call computes its single-thread order (vector 0, 1, ...).  vectors: HOST, num x dim of the index value type. */
+int sptag_b200_delete_vectors(sptag_b200_handle h, const void* vectors, int32_t num);
+
+/* Replaces: VectorIndex::AddIndex(p_data, p_vectorNum, p_dimension, nullptr, false, p_normalized) (BKTIndex.cpp:902-970,
+ * KDTIndex.cpp:628-696): appends the rows (graph rows -1, tombstone bytes 0; Dataset.h:127-144), normalises them for
+ * Cosine unless `normalized` (Utils::Normalize, CommonUtils.h:62-76), then for node = first .. last in order runs
+ * RefineNode(node, updateNeighbors = true, searchDeleted = true, AddCEF) (NeighborhoodGraph.h:535-561): the refine search
+ * with the node's row (MaxCheckForRefineGraph, K = AddCEF + 1), RebuildNeighbors into the node's row with the graph's
+ * degree as NeighborhoodSize and RNGFactor, and InsertNeighbors (RelativeNeighborhoodGraph.h:40-82) of the node into the
+ * row of every other result.  The reference's loop is sequential too, so the graph equals its graph bit for bit.
+ * The tree is not changed.  Once AddCountForRebuild vectors (default 1000) were added since the tree was built, the
+ * reference starts an asynchronous tree rebuild (RebuildJob) whose result and timing are not reproducible: results equal
+ * the reference's as long as that job has not replaced its tree.
+ * vectors: HOST, num x dim.  out_first_id (nullable): the first new id, id_offset included.
+ * EmptyData for null / num <= 0 / dim <= 0, DimensionSizeMismatch for a wrong dim.  Buffers grow geometrically.
+ * If a step of the chain fails, the call returns its error and the index keeps the rows that were linked in before the
+ * failing one (sptag_b200_num_vectors tells how many); the later rows are dropped. */
+int sptag_b200_add(sptag_b200_handle h, const void* vectors, int32_t num, int32_t dim, int32_t normalized,
+                   int32_t* out_first_id);
+
+/* Replaces: VectorIndex::SaveIndex(folder) (VectorIndex.cpp:197-222 SaveIndexConfig): writes indexloader.ini (algorithm,
+ * value type, metric, NeighborhoodSize, the search and update parameters) and vectors.bin / graph.bin / tree.bin /
+ * deletes.bin in the formats sptag_b200_load parses (Dataset.h:146-180, NeighborhoodGraph.h:606-615, BKTree.h:635-645 /
+ * KDTree.h:123-133, Labelset.h:78-83).  The reference's VectorIndex::LoadIndex reads the folder too.  Live rows' tombstone
+ * bytes are 0 (the reference's own save has 0xff for rows added since load, Dataset.h:127-144; both mean "live").  Creates the folder
+ * if needed.  Quantized handles: LackOfInputs (the quantizer blob is not kept). */
+int sptag_b200_save(sptag_b200_handle h, const char* folder);
+
+/* Labelset::Count(): tombstones set so far. */
+int32_t sptag_b200_num_deleted(sptag_b200_handle h);
 
 /* Device time in milliseconds of the search kernel(s) of the most recent sptag_b200_search*
  * call on this handle, measured with CUDA events on the launching stream (synchronises). */

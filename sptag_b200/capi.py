@@ -29,7 +29,8 @@ EXPORTS = [
     "sptag_b200_graph_degree", "sptag_b200_iterator_open", "sptag_b200_iterator_next", "sptag_b200_iterator_close",
     "sptag_b200_iterator_next_from_nearest", "sptag_b200_search_ex", "sptag_b200_iterator_open_ex",
     "sptag_b200_refine_search", "sptag_b200_refine_schedule", "sptag_b200_rebuild_graph", "sptag_b200_group_create", "sptag_b200_group_search",
-    "sptag_b200_group_destroy",
+    "sptag_b200_group_destroy", "sptag_b200_add", "sptag_b200_delete", "sptag_b200_delete_vectors", "sptag_b200_save",
+    "sptag_b200_num_deleted",
 ]
 
 
@@ -99,6 +100,11 @@ def lib():
         L.sptag_b200_iterator_next_from_nearest.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.sptag_b200_iterator_close.argtypes = [C.c_void_p]
         L.sptag_b200_iterator_close.restype = None
+        L.sptag_b200_add.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32)]
+        L.sptag_b200_delete.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+        L.sptag_b200_delete_vectors.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
+        L.sptag_b200_save.argtypes = [C.c_void_p, C.c_char_p]
+        L.sptag_b200_num_deleted.argtypes = [C.c_void_p]
         L.sptag_b200_last_kernel_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
         L.sptag_b200_launch_count.restype = C.c_int64
         for f in ("num_vectors", "dim", "value_type", "metric", "algo"):
@@ -299,6 +305,35 @@ class B200Index:
             np.array([g.shape[0], g.shape[1]], np.int32).tofile(f)
             g.tofile(f)
         return g
+
+    # -- mutation -------------------------------------------------------------------------------
+    def add(self, vectors, normalized=False):
+        """VectorIndex::AddIndex: appends the rows and links them into the graph on the device -> the first new id."""
+        vectors = np.ascontiguousarray(vectors)
+        first = C.c_int32()
+        _check(lib().sptag_b200_add(self._h, vectors.ctypes.data, vectors.shape[0], vectors.shape[1],
+                                    1 if normalized else 0, C.byref(first)))
+        return first.value
+
+    def delete(self, ids):
+        """VectorIndex::DeleteIndex(id) per id -> int32 ErrorCodes (0 Success, 0x14 VectorNotFound)."""
+        ids = np.ascontiguousarray(ids, dtype=np.int32).reshape(-1)
+        codes = np.empty(ids.shape[0], np.int32)
+        _check(lib().sptag_b200_delete(self._h, ids.ctypes.data, ids.shape[0], codes.ctypes.data))
+        return codes
+
+    def delete_vectors(self, vectors):
+        """VectorIndex::DeleteIndex(vectors, num) in its single-thread order."""
+        vectors = np.ascontiguousarray(vectors)
+        _check(lib().sptag_b200_delete_vectors(self._h, vectors.ctypes.data, vectors.shape[0]))
+
+    def save(self, folder):
+        """VectorIndex::SaveIndex(folder): a folder both the reference's LoadIndex and B200Index.load read."""
+        _check(lib().sptag_b200_save(self._h, os.fsencode(folder)))
+
+    @property
+    def num_deleted(self):
+        return lib().sptag_b200_num_deleted(self._h)
 
     def distance_batch(self, queries, ids):
         queries = np.ascontiguousarray(queries, dtype=np.float32)

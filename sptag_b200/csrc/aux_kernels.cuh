@@ -114,6 +114,153 @@ __global__ void carry_backpointers_kernel(const int* __restrict__ old_graph, int
 }
 
 // ------------------------------------------------------------------------------------------
+// Index mutation (AddIndex / DeleteIndex, BKTIndex.cpp:876-970, KDTIndex.cpp:602-696)
+// ------------------------------------------------------------------------------------------
+
+// COMMON::Utils::Normalize (CommonUtils.h:62-76) on rows [first, first + num), one thread per row: a double accumulator in
+// element order (a product of two values of T is exact in double, so contracting it into an FMA changes nothing), then
+// (T)(x / len * base).  The integer casts truncate toward zero like the reference's cvttsd2si.
+template <typename T>
+__device__ __forceinline__ T cast_from_double(double v) {
+    if (sizeof(T) == 4) return (T)__double2float_rn(v);
+    return (T)__double2int_rz(v);
+}
+template <typename T>
+__global__ void normalize_rows_kernel(unsigned char* vectors, unsigned long long row_stride_bytes, int first, int num, int dim,
+                                      int base) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= num) return;
+    T* a = reinterpret_cast<T*>(vectors + (size_t)(first + r) * row_stride_bytes);
+    double len = 0.0;
+    for (int j = 0; j < dim; ++j) {
+        const double v = (double)a[j];
+        len = __dadd_rn(len, __dmul_rn(v, v));
+    }
+    len = __dsqrt_rn(len);
+    if (len < 1e-6) {
+        const T val = cast_from_double<T>(__dmul_rn(__ddiv_rn(1.0, __dsqrt_rn((double)dim)), (double)base));
+        for (int j = 0; j < dim; ++j) a[j] = val;
+    } else {
+        for (int j = 0; j < dim; ++j) a[j] = cast_from_double<T>(__dmul_rn(__ddiv_rn((double)a[j], len), (double)base));
+    }
+}
+
+// DeleteIndex(id) for a batch (Labelset::Insert, Labelset.h:59-76) in call order: an id that is out of range, already
+// tombstoned, or repeated earlier in the same batch gets VectorNotFound; the first occurrence of a live id tombstones it.
+// Three launches: first[id] = INT_MAX, first[id] = min(batch position), then the winners flip the byte and count.
+// Only a byte of 1 is a tombstone (Labelset::Contains / Insert test == 1): rows the reference added and saved carry 0xff.
+__global__ void tombstone_reset_kernel(const int* __restrict__ ids, int num, int n, int* __restrict__ first) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < num && ids[i] >= 0 && ids[i] < n) first[ids[i]] = 0x7fffffff;
+}
+__global__ void tombstone_order_kernel(const int* __restrict__ ids, int num, int n, int* __restrict__ first) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < num && ids[i] >= 0 && ids[i] < n) atomicMin(&first[ids[i]], i);
+}
+__global__ void tombstone_apply_kernel(const int* __restrict__ ids, int num, int n, const int* __restrict__ first,
+                                       signed char* __restrict__ deleted, int* __restrict__ codes, int* __restrict__ count) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= num) return;
+    const int id = ids[i];
+    int code = 0x14;  // VectorNotFound
+    if (id >= 0 && id < n && first[id] == i && deleted[id] != 1) {
+        deleted[id] = 1;
+        atomicAdd(count, 1);
+        code = 0;
+    }
+    codes[i] = code;
+}
+
+// DeleteIndex(vectors) step for one query (BKTIndex.cpp:882-887): every result with Dist < 1e-6 is tombstoned.  The search
+// returned ids plus the shard offset.  One warp.
+__global__ void tombstone_close_kernel(const int* __restrict__ ids, const float* __restrict__ dists, int k, int id_offset,
+                                       signed char* __restrict__ deleted, int* __restrict__ count) {
+    for (int j = threadIdx.x; j < k; j += 32) {
+        const int id = ids[j] < 0 ? -1 : ids[j] - id_offset;
+        if (id >= 0 && (double)dists[j] < 1e-6 && deleted[id] != 1) {
+            deleted[id] = 1;
+            atomicAdd(count, 1);
+        }
+    }
+}
+
+// ComputeDistance(a, b) by one half-warp, the summation trees of rebuild_neighbors_kernel (both distances are symmetric
+// bit for bit: (a - b)^2 = (b - a)^2 and a * b = b * a exactly)
+template <bool COSINE, int ELEM>
+__device__ __forceinline__ float row_distance(const unsigned char* a, const unsigned char* b, int dim, int j, int simd_width) {
+    if (ELEM == 0) {
+        QueryRegs<0> qr;
+        if (simd_width != 16)
+            return half_warp_distance_w<COSINE>(reinterpret_cast<const float*>(a), reinterpret_cast<const float*>(b), dim, j,
+                                                simd_width);
+        return half_warp_distance<0, COSINE>(reinterpret_cast<const float*>(a), qr, reinterpret_cast<const float*>(b), dim, j);
+    }
+    return half_warp_distance_elem_w<COSINE, ELEM>(a, b, dim, j, simd_width);
+}
+
+// RelativeNeighborhoodGraph::InsertNeighbors (RelativeNeighborhoodGraph.h:40-82) as RefineNode(updateNeighbors = true) runs
+// it (NeighborhoodGraph.h:549-559): for every item of the added node's refine-search list, in list order until the first
+// VID < 0 and skipping the node itself, insert the node into the item's row.  The items' rows are distinct and no call
+// reads another item's row, so one warp per item computes exactly the sequential loop.  Per row: walk the slots (the last
+// one excluded when it holds a duplicate back-pointer); the first slot that is empty, or farther from the row's owner than
+// the node (ties: the smaller id first), takes the node and the displaced entries shift right while each is no farther
+// from the owner than from the node; a slot whose entry is closer to the node than the node is to the owner ends the walk.
+// The two distances of a step are computed at once, one per half-warp.
+template <bool COSINE, int ELEM>
+__global__ void __launch_bounds__(128) insert_neighbors_kernel(const unsigned char* __restrict__ vectors,
+                                                               unsigned long long row_stride_bytes, int dim, int node,
+                                                               const int* __restrict__ res_ids,
+                                                               const float* __restrict__ res_dists, int num_results,
+                                                               int* __restrict__ graph, int degree, int simd_width) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, j = lane & 15, half = lane >> 4;
+    const int w = blockIdx.x * (blockDim.x >> 5) + warp;
+    if (w >= num_results) return;
+    // RefineNode stops at the first VID < 0
+    for (int t0 = 0; t0 <= w; t0 += 32) {
+        const int t = t0 + lane;
+        if (__any_sync(kFull, t <= w && res_ids[t] < 0)) return;
+    }
+    const int target = res_ids[w];
+    if (target == node) return;
+    const float insert_dist = res_dists[w];
+    int* row = graph + (size_t)target * degree;
+    const unsigned char* node_vec = vectors + (size_t)target * row_stride_bytes;   // the row's owner
+    const unsigned char* insert_vec = vectors + (size_t)node * row_stride_bytes;   // the node being added
+    const int check = (row[degree - 1] < -1) ? degree - 1 : degree;
+    for (int k = 0; k < check; ++k) {
+        int tmp = row[k];
+        __syncwarp();
+        if (tmp < 0) {
+            if (lane == 0) row[k] = node;
+            return;
+        }
+        const unsigned char* tmp_vec = vectors + (size_t)tmp * row_stride_bytes;
+        // half 0: d(tmp, owner); half 1: d(tmp, inserted)
+        float d = row_distance<COSINE, ELEM>(tmp_vec, half ? insert_vec : node_vec, dim, j, simd_width);
+        float d_owner = __shfl_sync(kFull, d, 0), d_ins = __shfl_sync(kFull, d, 16);
+        if (d_owner > insert_dist || (insert_dist == d_owner && node < tmp)) {
+            if (lane == 0) row[k] = node;
+            __syncwarp();
+            while (++k < check && d_owner <= d_ins) {
+                const int next = row[k];
+                __syncwarp();
+                if (lane == 0) row[k] = tmp;
+                __syncwarp();
+                tmp = next;
+                if (tmp < 0) return;
+                tmp_vec = vectors + (size_t)tmp * row_stride_bytes;
+                d = row_distance<COSINE, ELEM>(tmp_vec, half ? insert_vec : node_vec, dim, j, simd_width);
+                d_owner = __shfl_sync(kFull, d, 0);
+                d_ins = __shfl_sync(kFull, d, 16);
+            }
+            return;
+        } else if (d_ins < insert_dist) {
+            return;
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------
 // NeighborhoodGraph::RebuildGraph (NeighborhoodGraph.h:404-456): EnableRebuild's in-degree repair.  Rows hold 2 x ns
 // candidates; the first ns/2 stay; the other ns - ns/2 slots are refilled from entries [ns/2, 2 ns): the ones whose target's
 // in-degree is below ns/2 first, then the earliest others, in index order; the in-degree array follows every change.

@@ -20,6 +20,7 @@
 #include <fstream>
 #include <map>
 #include <mutex>
+#include <sys/stat.h>
 #include <sstream>
 #include <string>
 #include <vector>
@@ -94,6 +95,12 @@ struct sptag_b200_index {
     int search_deleted = 0;   // handle-wide default of p_searchDeleted (parameter "SearchDeleted"); per-call value: sptag_b200_search_ex
     // search parameters (reference names)
     int max_check = 8192, max_check_refine = 8192, initial_pivots = 50, other_pivots = 4, no_better_threshold = 3;
+    // graph-update parameters (reference names, BKT/ParameterDefinitionList.h:28-31): AddIndex's refine budget, the
+    // result count of DeleteIndex(vectors), RebuildNeighbors' factor
+    int add_cef = 500, cef = 1000;
+    float rng_factor = 1.0f;
+    int open_iterators = 0;  // their per-query bitmaps are sized to n: mutations are refused while any is open
+    DeviceBuffer d_mut, d_first;  // mutation scratch: ids / codes / counter, and the per-id first batch position
     // B200 tuning knobs
     int queries_per_sm = 0;  // 0 = auto
     int stage_rows = 0;      // 0 = auto
@@ -200,6 +207,9 @@ struct CallOpts {
     int search_deleted = -1;    // -1 = the handle's "SearchDeleted" default, else 0 / 1
     const unsigned char* d_filter = nullptr;  // device byte map (0 = never added to the results) or nullptr
     size_t refine_query_stride = 0;  // refine flavour: bytes between queries (index rows: the padded row stride)
+    // test the tombstone map even while the host's count is 0: DeleteIndex(vectors) tombstones on the device between two
+    // of its searches (an all-zero map rejects nothing, so this equals the reference's Count() == 0 dispatch)
+    bool tombstones_live = false;
 };
 
 // Fill SearchParams + launch geometry for this handle.  Allocates per-slot scratch.  Caller holds h->mu.
@@ -247,7 +257,8 @@ int configure(sptag_b200_index* h, int k, SearchParams& p, int& grid, size_t& sm
     p.tree_num = h->tree_num;
     p.node_count = h->node_count;
     // flags += (m_deletedID.Count() == 0 || p_searchDeleted) << 2  (BKTIndex.cpp:473, KDTIndex.cpp:260)
-    p.deleted = (h->num_deleted > 0 && !eff_search_deleted) ? (const signed char*)h->d_deleted.ptr : nullptr;
+    p.deleted = ((h->num_deleted > 0 || opts.tombstones_live) && !eff_search_deleted) ? (const signed char*)h->d_deleted.ptr
+                                                                                       : nullptr;
     p.filter = opts.d_filter;
     p.k = k;
     p.id_offset = h->id_offset;
@@ -792,6 +803,8 @@ void sptag_b200_destroy(sptag_b200_handle h) {
     h->d_tree_starts.release();
     h->d_deleted.release();
     h->d_graph_new.release();
+    h->d_mut.release();
+    h->d_first.release();
     h->d_codebooks.release();
     h->d_rotation_t.release();
     h->d_rotation.release();
@@ -958,7 +971,8 @@ int sptag_b200_load(const char* folder, int32_t device, int32_t id_offset, sptag
         }
     }
     static const char* names[] = {"MaxCheck", "MaxCheckForRefineGraph", "NumberOfInitialDynamicPivots",
-                                  "NumberOfOtherDynamicPivots", "ThresholdOfNumberOfContinuousNoBetterPropagation"};
+                                  "NumberOfOtherDynamicPivots", "ThresholdOfNumberOfContinuousNoBetterPropagation",
+                                  "AddCEF", "CEF", "RNGFactor"};
     for (const char* nm : names) {
         auto it = kv.find(nm);
         if (it != kv.end()) sptag_b200_set_param(h, nm, it->second.c_str());
@@ -1046,6 +1060,9 @@ int sptag_b200_set_param(sptag_b200_handle h, const char* name, const char* valu
     const std::string n(name);
     if (n == "MaxCheck") h->max_check = (int)v;
     else if (n == "MaxCheckForRefineGraph") h->max_check_refine = (int)v;
+    else if (n == "AddCEF") h->add_cef = (int)v;
+    else if (n == "CEF") h->cef = (int)v;
+    else if (n == "RNGFactor") h->rng_factor = strtof(value, nullptr);
     else if (n == "SearchDeleted") h->search_deleted = (v != 0) ? 1 : 0;
     else if (n == "NumberOfInitialDynamicPivots") h->initial_pivots = (int)v;
     else if (n == "NumberOfOtherDynamicPivots") h->other_pivots = (int)v;
@@ -1069,8 +1086,14 @@ int sptag_b200_get_param(sptag_b200_handle h, const char* name, char* value_out,
     std::lock_guard<std::mutex> lock(h->mu);
     const std::string n(name);
     long v;
+    if (n == "RNGFactor") {  // float, printed like the reference's ini (ConvertToString)
+        snprintf(value_out, (size_t)capacity, "%f", h->rng_factor);
+        return SPTAG_B200_SUCCESS;
+    }
     if (n == "MaxCheck") v = h->max_check;
     else if (n == "MaxCheckForRefineGraph") v = h->max_check_refine;
+    else if (n == "AddCEF") v = h->add_cef;
+    else if (n == "CEF") v = h->cef;
     else if (n == "SearchDeleted") v = h->search_deleted;
     else if (n == "NumberOfInitialDynamicPivots") v = h->initial_pivots;
     else if (n == "NumberOfOtherDynamicPivots") v = h->other_pivots;
@@ -1133,14 +1156,23 @@ int search_host_impl(sptag_b200_handle h, const void* queries, int32_t num_queri
         if (int rc = st->d_stats.ensure((size_t)num_queries * kStatsPerQuery * 4)) return rc;
     cudaStream_t stream = st->stream;
     CUDA_OK(cudaMemcpyAsync(st->d_queries.ptr, queries, qbytes, cudaMemcpyHostToDevice, stream));
+    int map_n = 0;
     if (allowed) {
         // SearchIndexWithFilter: the caller evaluated filterFunc once per vector; the map is this call's own copy
-        if (int rc = st->d_filter.ensure((size_t)h->n)) return rc;
-        CUDA_OK(cudaMemcpyAsync(st->d_filter.ptr, allowed, (size_t)h->n, cudaMemcpyHostToDevice, stream));
+        {
+            std::lock_guard<std::mutex> lock(h->mu);
+            map_n = h->n;
+        }
+        if (int rc = st->d_filter.ensure((size_t)map_n)) return rc;
+        CUDA_OK(cudaMemcpyAsync(st->d_filter.ptr, allowed, (size_t)map_n, cudaMemcpyHostToDevice, stream));
         opts.d_filter = (const unsigned char*)st->d_filter.ptr;
     }
     {
         std::lock_guard<std::mutex> lock(h->mu);  // configure + enqueue only; the copies above / below overlap other callers' kernels
+        if (allowed && h->n != map_n) {  // an add ran in between: the map no longer covers every vector
+            cudaStreamSynchronize(stream);
+            return fail(SPTAG_B200_FAIL, "the index grew from %d to %d vectors during the filtered search", map_n, h->n);
+        }
         if (int rc = search_device_impl(h, st->d_queries.ptr, num_queries, k, (int*)st->d_ids.ptr, (float*)st->d_dists.ptr,
                                         out_stats ? (int*)st->d_stats.ptr : nullptr, stream, refine, opts)) {
             cudaStreamSynchronize(stream);
@@ -1460,6 +1492,7 @@ int sptag_b200_iterator_open_ex(sptag_b200_handle h, const void* queries, int32_
         delete it;
         return fail(SPTAG_B200_FAIL, "iterator set-up failed: %s", cudaGetErrorString(e));
     }
+    h->open_iterators++;  // sptag_b200_iterator_close gives it back
     *out = it;
     return SPTAG_B200_SUCCESS;
 }
@@ -1639,6 +1672,7 @@ void sptag_b200_iterator_close(sptag_b200_iter it) {
         std::lock_guard<std::mutex> lock(it->h->mu);
         DeviceGuard guard(it->h->device);
         it->release();
+        it->h->open_iterators--;
     }
     delete it;
 }
@@ -1860,5 +1894,335 @@ int32_t sptag_b200_dim(sptag_b200_handle h) { return h ? h->dim : 0; }
 int32_t sptag_b200_value_type(sptag_b200_handle h) { return h ? h->value_type : -1; }
 int32_t sptag_b200_metric(sptag_b200_handle h) { return h ? h->metric : -1; }
 int32_t sptag_b200_algo(sptag_b200_handle h) { return h ? h->algo : -1; }
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------
+// Index mutation: AddIndex / DeleteIndex / SaveIndex (BKTIndex.cpp:876-970, KDTIndex.cpp:602-696, VectorIndex.cpp)
+// ---------------------------------------------------------------------------------------------------------------
+namespace {
+
+// Grow `b` to at least `need` bytes keeping its first `keep` bytes; capacity grows by half at least, so a stream of
+// small adds reallocates O(log n) times.  The caller has waited for every launch that reads the buffer.
+int grow_keep(DeviceBuffer& b, size_t need, size_t keep) {
+    if (need <= b.bytes) return 0;
+    size_t cap = std::max(need, b.bytes + b.bytes / 2);
+    void* p = nullptr;
+    if (cudaMalloc(&p, cap) != cudaSuccess) {
+        cudaGetLastError();
+        cap = need;
+        cudaError_t e = cudaMalloc(&p, cap);
+        if (e != cudaSuccess) return fail(SPTAG_B200_MEMORY_OVERFLOW, "cudaMalloc(%zu) failed: %s", cap, cudaGetErrorString(e));
+    }
+    if (keep && b.ptr) {
+        cudaError_t e = cudaMemcpy(p, b.ptr, std::min(keep, b.bytes), cudaMemcpyDeviceToDevice);
+        if (e != cudaSuccess) {
+            cudaFree(p);
+            return fail(SPTAG_B200_FAIL, "device copy on growth failed: %s", cudaGetErrorString(e));
+        }
+    }
+    b.release();
+    b.ptr = p;
+    b.bytes = cap;
+    return 0;
+}
+
+// A mutation runs under h->mu after every kernel already enqueued on the handle (searches of other threads hold the
+// lock only while they enqueue; each records its scratch set's ev_done), so a concurrent search sees all of it or none.
+int quiesce(sptag_b200_index* h) {
+    for (auto& sc : h->scratch)
+        if (sc.used) CUDA_OK(cudaEventSynchronize(sc.ev_done));
+    return 0;
+}
+
+int check_mutable(const sptag_b200_index* h) {
+    if (h->open_iterators > 0)
+        return fail(SPTAG_B200_FAIL, "%d iterator(s) of this index are open: their per-query visited sets are sized to the "
+                                     "current vector count; close them before changing the index", h->open_iterators);
+    return 0;
+}
+
+// The tombstone map exists from the first deletion on (sptag_b200_load / _create allocate it only for a non-empty one)
+// (sptag_b200_add grows an existing map with the vectors)
+int ensure_deleted_map(sptag_b200_index* h) {
+    if (h->d_deleted.ptr) return 0;
+    if (int rc = h->d_deleted.ensure((size_t)h->n)) return rc;
+    CUDA_OK(cudaMemset(h->d_deleted.ptr, 0, (size_t)h->n));
+    return 0;
+}
+
+int value_base(int vt) {  // COMMON::Utils::GetBase<T> (CommonUtils.h:54-59)
+    switch (vt) {
+    case SPTAG_B200_VT_INT8: return 127;
+    case SPTAG_B200_VT_UINT8: return 255;
+    case SPTAG_B200_VT_INT16: return 32767;
+    }
+    return 1;
+}
+
+bool write_all(FILE* f, const void* p, size_t bytes) { return bytes == 0 || std::fwrite(p, 1, bytes, f) == bytes; }
+
+const char* value_type_name(int vt) {
+    switch (vt) {
+    case SPTAG_B200_VT_INT8: return "Int8";
+    case SPTAG_B200_VT_UINT8: return "UInt8";
+    case SPTAG_B200_VT_INT16: return "Int16";
+    }
+    return "Float";
+}
+
+}  // namespace
+
+extern "C" {
+
+int sptag_b200_delete(sptag_b200_handle h, const int32_t* ids, int32_t num, int32_t* out_codes) {
+    if (!h) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (num < 0 || (num > 0 && !ids)) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    if (num == 0) return SPTAG_B200_SUCCESS;
+    std::lock_guard<std::mutex> lock(h->mu);
+    DeviceGuard guard(h->device);
+    if (int rc = check_mutable(h)) return rc;
+    if (int rc = quiesce(h)) return rc;
+    if (int rc = ensure_deleted_map(h)) return rc;
+    // ids as search returns them: the shard offset comes off first
+    std::vector<int32_t> local((size_t)num);
+    for (int i = 0; i < num; ++i) {
+        const long long v = (long long)ids[i] - h->id_offset;
+        local[(size_t)i] = (v < 0 || v >= h->n) ? -1 : (int32_t)v;  // out of range: VectorNotFound
+    }
+    if (int rc = h->d_mut.ensure((size_t)num * 8 + 16)) return rc;
+    if (int rc = h->d_first.ensure((size_t)h->n * 4)) return rc;
+    int* d_ids = (int*)h->d_mut.ptr;
+    int* d_codes = d_ids + num;
+    int* d_count = d_codes + num;
+    cudaStream_t stream = nullptr;
+    CUDA_OK(cudaMemcpyAsync(d_ids, local.data(), (size_t)num * 4, cudaMemcpyHostToDevice, stream));
+    CUDA_OK(cudaMemsetAsync(d_count, 0, 4, stream));
+    const unsigned blocks = (unsigned)((num + 255) / 256);
+    tombstone_reset_kernel<<<blocks, 256, 0, stream>>>(d_ids, num, h->n, (int*)h->d_first.ptr);
+    tombstone_order_kernel<<<blocks, 256, 0, stream>>>(d_ids, num, h->n, (int*)h->d_first.ptr);
+    tombstone_apply_kernel<<<blocks, 256, 0, stream>>>(d_ids, num, h->n, (const int*)h->d_first.ptr,
+                                                       (signed char*)h->d_deleted.ptr, d_codes, d_count);
+    g_launches += 3;
+    CUDA_OK(cudaGetLastError());
+    int added = 0;
+    CUDA_OK(cudaMemcpyAsync(&added, d_count, 4, cudaMemcpyDeviceToHost, stream));
+    if (out_codes) CUDA_OK(cudaMemcpyAsync(out_codes, d_codes, (size_t)num * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    h->num_deleted += added;
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_delete_vectors(sptag_b200_handle h, const void* vectors, int32_t num) {
+    if (!h) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (num < 0 || (num > 0 && !vectors)) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    if (h->q_type != 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "DeleteIndex(vectors) on a quantized index is not built");
+    if (num == 0) return SPTAG_B200_SUCCESS;
+    std::lock_guard<std::mutex> lock(h->mu);
+    DeviceGuard guard(h->device);
+    if (int rc = check_mutable(h)) return rc;
+    const int k = h->cef;
+    if (k < 1 || k > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "CEF = %d outside [1, 2048]", k);
+    if (int rc = quiesce(h)) return rc;
+    if (int rc = ensure_deleted_map(h)) return rc;
+    const size_t qb = query_bytes(h);
+    const size_t qoff = round_up((size_t)k * 8 + 16, 256);
+    if (int rc = h->d_mut.ensure(qoff + (size_t)num * qb)) return rc;
+    int* d_ids = (int*)h->d_mut.ptr;
+    float* d_dists = (float*)(d_ids + k);
+    int* d_count = (int*)(d_dists + k);
+    unsigned char* d_q = (unsigned char*)h->d_mut.ptr + qoff;
+    cudaStream_t stream = nullptr;
+    CUDA_OK(cudaMemcpyAsync(d_q, vectors, (size_t)num * qb, cudaMemcpyHostToDevice, stream));
+    CUDA_OK(cudaMemsetAsync(d_count, 0, 4, stream));
+    // SearchIndex(query) per vector (the index's MaxCheck, searchDeleted = false, K = CEF), then DeleteIndex of every
+    // result closer than 1e-6 -- in vector order, each search seeing the tombstones of the ones before it
+    CallOpts opts;
+    opts.search_deleted = 0;
+    opts.tombstones_live = true;
+    for (int i = 0; i < num; ++i) {
+        if (int rc = search_device_impl(h, d_q + (size_t)i * qb, 1, k, d_ids, d_dists, nullptr, stream, false, opts)) {
+            cudaStreamSynchronize(stream);
+            return rc;
+        }
+        tombstone_close_kernel<<<1, 32, 0, stream>>>(d_ids, d_dists, k, h->id_offset, (signed char*)h->d_deleted.ptr, d_count);
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+    }
+    int added = 0;
+    CUDA_OK(cudaMemcpyAsync(&added, d_count, 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    h->num_deleted += added;
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_add(sptag_b200_handle h, const void* vectors, int32_t num, int32_t dim, int32_t normalized,
+                   int32_t* out_first_id) {
+    if (!h) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (!vectors || num <= 0 || dim <= 0) return fail(SPTAG_B200_EMPTY_DATA, "no vectors to add");
+    if (dim != h->dim) return fail(SPTAG_B200_DIMENSION_MISMATCH, "vectors have %d dimensions, the index %d", dim, h->dim);
+    if (h->q_type != 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "AddIndex on a quantized index is not built");
+    std::lock_guard<std::mutex> lock(h->mu);
+    DeviceGuard guard(h->device);
+    if (int rc = check_mutable(h)) return rc;
+    const int k = h->add_cef + 1;
+    if (k < 1 || k > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "AddCEF = %d outside [0, 2047]", h->add_cef);
+    if ((long long)h->n + num > 0x7fffffffLL - 1) return fail(SPTAG_B200_MEMORY_OVERFLOW, "more than 2^31 - 2 vectors");
+    if (int rc = quiesce(h)) return rc;
+    cudaStream_t stream = nullptr;
+    const int old_n = h->n, new_n = h->n + num;
+    const size_t rs = h->row_stride, row_bytes = (size_t)h->dim * value_size(h->value_type);
+    // Dataset::AddBatch (Dataset.h:127-144): append the rows (plus the spare padded row), new graph rows all -1, new
+    // tombstone bytes 0
+    if (int rc = grow_keep(h->d_vectors, ((size_t)new_n + 1) * rs, (size_t)old_n * rs)) return rc;
+    CUDA_OK(cudaMemsetAsync((unsigned char*)h->d_vectors.ptr + (size_t)old_n * rs, 0, ((size_t)num + 1) * rs, stream));
+    CUDA_OK(cudaMemcpy2DAsync((unsigned char*)h->d_vectors.ptr + (size_t)old_n * rs, rs, vectors, row_bytes, row_bytes,
+                              (size_t)num, cudaMemcpyHostToDevice, stream));
+    const size_t grow_row = (size_t)h->degree * 4;
+    if (int rc = grow_keep(h->d_graph, (size_t)new_n * grow_row, (size_t)old_n * grow_row)) return rc;
+    CUDA_OK(cudaMemsetAsync((unsigned char*)h->d_graph.ptr + (size_t)old_n * grow_row, 0xff, (size_t)num * grow_row, stream));
+    if (h->d_deleted.ptr) {
+        if (int rc = grow_keep(h->d_deleted, (size_t)new_n, (size_t)old_n)) return rc;
+        CUDA_OK(cudaMemsetAsync((unsigned char*)h->d_deleted.ptr + old_n, 0, (size_t)num, stream));
+    }
+    unsigned char* dv = (unsigned char*)h->d_vectors.ptr;
+    if (h->metric == SPTAG_B200_METRIC_COSINE && !normalized) {
+        const unsigned blocks = (unsigned)((num + 127) / 128);
+        const int base = value_base(h->value_type);
+        switch (h->value_type) {
+        case SPTAG_B200_VT_INT8: normalize_rows_kernel<int8_t><<<blocks, 128, 0, stream>>>(dv, rs, old_n, num, h->dim, base); break;
+        case SPTAG_B200_VT_UINT8: normalize_rows_kernel<uint8_t><<<blocks, 128, 0, stream>>>(dv, rs, old_n, num, h->dim, base); break;
+        case SPTAG_B200_VT_INT16: normalize_rows_kernel<int16_t><<<blocks, 128, 0, stream>>>(dv, rs, old_n, num, h->dim, base); break;
+        default: normalize_rows_kernel<float><<<blocks, 128, 0, stream>>>(dv, rs, old_n, num, h->dim, base); break;
+        }
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+    }
+    h->n = new_n;
+    // RefineNode(node, updateNeighbors = true, searchDeleted = true, AddCEF) for node = old_n .. new_n - 1, in order
+    // (NeighborhoodGraph.h:535-561): each node's search sees the rows the nodes before it rebuilt and inserted into
+    if (int rc = h->d_ids.ensure((size_t)k * 4)) return rc;
+    if (int rc = h->d_dists.ensure((size_t)k * 4)) return rc;
+    int* d_ids = (int*)h->d_ids.ptr;
+    float* d_dists = (float*)h->d_dists.ptr;
+    int* graph = (int*)h->d_graph.ptr;
+    CallOpts ropts;
+    ropts.max_check = h->max_check_refine;  // RefineSearchIndex: workSpace->Reset(MaxCheckForRefineGraph, AddCEF + 1)
+    ropts.search_deleted = 1;
+    ropts.refine_query_stride = rs;
+    const bool l2 = (h->metric == SPTAG_B200_METRIC_L2);
+    const int deg = h->degree;
+    const unsigned ins_blocks = (unsigned)((k + 3) / 4);
+    for (int node = old_n; node < new_n; ++node) {
+        if (int rc = search_device_impl(h, dv + (size_t)node * rs, 1, k, d_ids, d_dists, nullptr, stream, /*refine=*/true, ropts)) {
+            cudaStreamSynchronize(stream);
+            h->n = node;  // keep the rows that are linked in (no row points to a node that was not inserted)
+            return rc;
+        }
+        int* row = graph + (size_t)node * deg;
+#define SPTAG_B200_ADD(COS, EL)                                                                                            \
+    do {                                                                                                                   \
+        rebuild_neighbors_kernel<COS, EL><<<1, 32, (size_t)deg * 4, stream>>>(dv, rs, h->dim, node, 1, d_ids, d_dists, k,  \
+                                                                             deg, h->rng_factor, row, h->simd_width);      \
+        insert_neighbors_kernel<COS, EL><<<ins_blocks, 128, 0, stream>>>(dv, rs, h->dim, node, d_ids, d_dists, k, graph,  \
+                                                                         deg, h->simd_width);                              \
+    } while (0)
+        if (h->value_type == SPTAG_B200_VT_FLOAT) {
+            if (l2) SPTAG_B200_ADD(false, 0); else SPTAG_B200_ADD(true, 0);
+        } else if (h->value_type == SPTAG_B200_VT_INT8) {
+            if (l2) SPTAG_B200_ADD(false, 1); else SPTAG_B200_ADD(true, 1);
+        } else if (h->value_type == SPTAG_B200_VT_UINT8) {
+            if (l2) SPTAG_B200_ADD(false, 2); else SPTAG_B200_ADD(true, 2);
+        } else {
+            if (l2) SPTAG_B200_ADD(false, 3); else SPTAG_B200_ADD(true, 3);
+        }
+#undef SPTAG_B200_ADD
+        g_launches += 2;
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) {
+            cudaStreamSynchronize(stream);
+            h->n = node;
+            return fail(SPTAG_B200_FAIL, "AddIndex step of node %d failed: %s", node, cudaGetErrorString(e));
+        }
+    }
+    CUDA_OK(cudaStreamSynchronize(stream));
+    if (out_first_id) *out_first_id = old_n + h->id_offset;
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_save(sptag_b200_handle h, const char* folder) {
+    if (!h) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (!folder) return fail(SPTAG_B200_LACK_OF_INPUTS, "null folder");
+    if (h->q_type != 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "saving a quantized index is not built (the quantizer blob is not kept)");
+    std::lock_guard<std::mutex> lock(h->mu);
+    DeviceGuard guard(h->device);
+    if (int rc = quiesce(h)) return rc;
+    const std::string dir(folder);
+    mkdir(dir.c_str(), 0777);  // like SaveIndex, which creates the folder; an existing one is reused
+    const size_t n = (size_t)h->n, rs = h->row_stride, row_bytes = (size_t)h->dim * value_size(h->value_type);
+    const bool bkt = (h->algo == SPTAG_B200_ALGO_BKT);
+    const size_t node_sz = bkt ? 12 : 16;
+    std::vector<unsigned char> vec(n * row_bytes), nodes(((size_t)h->node_count + 1) * node_sz), del(n, 0);
+    std::vector<int32_t> graph(n * (size_t)h->degree), starts((size_t)h->tree_num);
+    CUDA_OK(cudaMemcpy2D(vec.data(), row_bytes, h->d_vectors.ptr, rs, row_bytes, n, cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(graph.data(), h->d_graph.ptr, graph.size() * 4, cudaMemcpyDeviceToHost));
+    // the node array on the device ends with the (-1, -1, -1) sentinel LoadTrees appends (BKTree.h:662); the reference
+    // saves its loaded array, sentinel included
+    CUDA_OK(cudaMemcpy(nodes.data(), h->d_nodes.ptr, nodes.size(), cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(starts.data(), h->d_tree_starts.ptr, starts.size() * 4, cudaMemcpyDeviceToHost));
+    if (h->d_deleted.ptr) CUDA_OK(cudaMemcpy(del.data(), h->d_deleted.ptr, n, cudaMemcpyDeviceToHost));
+    int32_t node_count = h->node_count;
+    if (bkt) {
+        int32_t last;
+        memcpy(&last, nodes.data() + (size_t)(node_count - 1) * node_sz, 4);
+        if (last != -1) node_count++;
+    }
+    auto open_w = [&](const char* name) { return std::fopen((dir + "/" + name).c_str(), "wb"); };
+    bool ok = true;
+    // vectors.bin (Dataset.h:146-180), graph.bin (NeighborhoodGraph.h:606-615), tree.bin (BKTree.h:635-645 /
+    // KDTree.h:123-133), deletes.bin (Labelset.h:78-83: count, then Dataset<int8> n x 1)
+    if (FILE* f = open_w("vectors.bin")) {
+        const int32_t hdr[2] = {h->n, h->dim};
+        ok = write_all(f, hdr, 8) && write_all(f, vec.data(), vec.size()) && ok;
+        ok = std::fclose(f) == 0 && ok;
+    } else ok = false;
+    if (FILE* f = open_w("graph.bin")) {
+        const int32_t hdr[2] = {h->n, h->degree};
+        ok = write_all(f, hdr, 8) && write_all(f, graph.data(), graph.size() * 4) && ok;
+        ok = std::fclose(f) == 0 && ok;
+    } else ok = false;
+    if (FILE* f = open_w("tree.bin")) {
+        ok = write_all(f, &h->tree_num, 4) && write_all(f, starts.data(), starts.size() * 4) && write_all(f, &node_count, 4) &&
+             write_all(f, nodes.data(), (size_t)node_count * node_sz) && ok;
+        ok = std::fclose(f) == 0 && ok;
+    } else ok = false;
+    if (FILE* f = open_w("deletes.bin")) {
+        const int32_t hdr[3] = {h->num_deleted, h->n, 1};
+        ok = write_all(f, hdr, 12) && write_all(f, del.data(), del.size()) && ok;
+        ok = std::fclose(f) == 0 && ok;
+    } else ok = false;
+    // indexloader.ini as VectorIndex::SaveIndexConfig writes it (VectorIndex.cpp:197-222): [Index] with the algorithm and
+    // value type, then the parameters; the reference's LoadIndex and sptag_b200_load both read it
+    if (FILE* f = open_w("indexloader.ini")) {
+        const char* metric = h->metric == SPTAG_B200_METRIC_L2 ? "L2" : (h->metric == SPTAG_B200_METRIC_COSINE ? "Cosine" : "InnerProduct");
+        const int w = std::fprintf(
+            f,
+            "[Index]\nIndexAlgoType=%s\nValueType=%s\n\nTreeFilePath=tree.bin\nGraphFilePath=graph.bin\nVectorFilePath=vectors.bin\n"
+            "DeleteVectorFilePath=deletes.bin\nNeighborhoodSize=%d\nCEF=%d\nAddCEF=%d\nMaxCheckForRefineGraph=%d\nRNGFactor=%f\n"
+            "DistCalcMethod=%s\nMaxCheck=%d\nThresholdOfNumberOfContinuousNoBetterPropagation=%d\nNumberOfInitialDynamicPivots=%d\n"
+            "NumberOfOtherDynamicPivots=%d\n",
+            bkt ? "BKT" : "KDT", value_type_name(h->value_type), h->degree, h->cef, h->add_cef, h->max_check_refine,
+            h->rng_factor, metric, h->max_check, h->no_better_threshold, h->initial_pivots, h->other_pivots);
+        ok = w > 0 && std::fclose(f) == 0 && ok;
+    } else ok = false;
+    if (!ok) return fail(SPTAG_B200_FAIL, "cannot write the index files in %s", folder);
+    return SPTAG_B200_SUCCESS;
+}
+
+int32_t sptag_b200_num_deleted(sptag_b200_handle h) {
+    if (!h) return 0;
+    std::lock_guard<std::mutex> lock(h->mu);  // written by the delete calls under the same lock
+    return h->num_deleted;
+}
 
 }  // extern "C"

@@ -39,7 +39,9 @@ enum class ErrorCode : std::uint16_t {
     FailedParseValue = 0x0011,
     MemoryOverFlow = 0x0012,
     LackOfInputs = 0x0013,
+    VectorNotFound = 0x0014,
     EmptyIndex = 0x0015,
+    EmptyData = 0x0016,
     DimensionSizeMismatch = 0x0017,
 };
 
@@ -226,6 +228,32 @@ public:
                   std::fwrite(g.data(), 4, g.size(), f) == g.size();
         ok = (std::fclose(f) == 0) && ok;
         return ok ? ErrorCode::Success : ErrorCode::Fail;
+    }
+
+    // VectorIndex::AddIndex (VectorIndex.h:37, BKTIndex.cpp:902-970) without metadata: sptag_b200_add
+    ErrorCode AddIndex(const void* p_data, SizeType p_vectorNum, DimensionType p_dimension, bool p_normalized = false) {
+        if (!m_handle) return ErrorCode::EmptyIndex;
+        return static_cast<ErrorCode>(sptag_b200_add(m_handle, p_data, p_vectorNum, p_dimension, p_normalized ? 1 : 0, nullptr));
+    }
+
+    // VectorIndex::DeleteIndex(const SizeType&) (VectorIndex.h:181, BKTIndex.cpp:893-899): Success or VectorNotFound
+    ErrorCode DeleteIndex(const SizeType& p_id) {
+        if (!m_handle) return ErrorCode::EmptyIndex;
+        std::int32_t code = 0;
+        const int rc = sptag_b200_delete(m_handle, &p_id, 1, &code);
+        return static_cast<ErrorCode>(rc != 0 ? rc : code);
+    }
+
+    // VectorIndex::DeleteIndex(const void*, SizeType) (VectorIndex.h:39, BKTIndex.cpp:876-890), single-thread order
+    ErrorCode DeleteIndex(const void* p_vectors, SizeType p_vectorNum) {
+        if (!m_handle) return ErrorCode::EmptyIndex;
+        return static_cast<ErrorCode>(sptag_b200_delete_vectors(m_handle, p_vectors, p_vectorNum));
+    }
+
+    // VectorIndex::SaveIndex(folder) (VectorIndex.h:87): a folder the reference's LoadIndex and this LoadIndex read
+    ErrorCode SaveIndex(const std::string& p_folderPath) const {
+        if (!m_handle) return ErrorCode::EmptyIndex;
+        return static_cast<ErrorCode>(sptag_b200_save(m_handle, p_folderPath.c_str()));
     }
 
     // VectorIndex::GetIterator (VectorIndex.h:43, BKTIndex.cpp:650-657); nullptr where the reference returns nullptr
