@@ -127,7 +127,14 @@ void sptag_b200_destroy(sptag_b200_handle h);
  * kernels), 8 = AVX / AVX2, 4 = SSE; 8 and 4 are built for float, int8 and uint8 rows and run the generic-dimension
  * kernels; int16 rows and quantized indexes exist in the AVX-512 form only and return LackOfInputs otherwise), B200.VisitedLog (-1 auto, 0 clear the
  * visited bitmap per query, 1 log the touched words and clear only those: for indexes of tens of millions
- * of vectors), B200.VisitedLogEntries. */
+ * of vectors), B200.VisitedLogEntries, B200.VisitedSet (-1 auto: the per-slot visited bitmap unless its allocation fails
+ * for lack of device memory, then the hashed set; a bitmap size that failed is not tried again until a launch needs a
+ * smaller one or B200.VisitedSet is set; 0 bitmap; 1 hashed set: one table of 2^(bits(max(MaxCheck,
+ * MaxCheckForRefineGraph)) + 2) entries per query slot, at least 64, independent of the number of vectors; a query that fills half of
+ * it is searched again on a bitmap by a second launch on the same stream; results are identical in every mode),
+ * B200.VisitedHashEntries (table entries per slot: 0 = the default above, otherwise a power of two in [64, 2^30]).
+ * Read-only: B200.LastVisitedOverflows (queries the hashed set handed to the bitmap re-run in the last blocking search
+ * call of this handle; 0 on the bitmap), B200.ScratchBytes (device bytes held by the handle's search scratch sets). */
 int sptag_b200_set_param(sptag_b200_handle h, const char* name, const char* value);
 int sptag_b200_get_param(sptag_b200_handle h, const char* name, char* value_out, int32_t capacity);
 

@@ -74,6 +74,14 @@ struct SearchParams {
     // large N: instead of clearing the whole bitmap per query, log the words that were set and clear only those
     unsigned int* vlog;                    // per slot, vlog_entries words; nullptr = clear the bitmap per query
     unsigned long long vlog_entries;
+    // hashed visited set (search_kernel only): per slot an open-addressed table of keys id + 1 (0 = empty), linear probing
+    // from a multiplicative hash; `vlog` then logs the table positions a query filled.  nullptr = the bitmap above.
+    unsigned int* vhash;
+    unsigned vhash_mask;                   // table entries per slot - 1 (a power of two)
+    int vhash_shift;                       // 32 - log2(entries): the home position is the top bits of id * 2654435769
+    int vhash_limit;                       // distinct ids a query may insert before it is abandoned; INT_MAX without a table
+    unsigned int* overflow;                // {count, query indices}: the queries abandoned at the limit
+    const unsigned int* rerun;             // re-run launch: the same list; the kernel searches only the queries listed there
     // shared-memory layout (bytes from the dynamic smem base)
     int stage_rows, stages, slot_stride;
     int slot_stagger;  // 1: odd ring slots start 64 B later (stride is a multiple of 128); 0: stride = 64 mod 128
@@ -526,6 +534,39 @@ static __device__ __noinline__ int heap_full_slot(const int2* hs, const int2* hg
     return (d > best) ? -1 : besti;
 }
 
+// Hashed visited set (open addressing, keys id + 1, 0 = empty, linear probing).  The per-lane probe past the home position
+// is rare and kept out of line like heap_full_slot, so that it adds nothing to the kernels' register allocation; the
+// warp-uniform insert has an out-of-line copy too (which one costs fewer registers depends on the kernel).
+constexpr unsigned kVhashFound = 0x80000000u;  // table positions stay below 2^30
+// One lane's probe for `key` after position `pos`, which holds another id (other lanes of the warp insert other keys
+// concurrently): the position where the key was inserted, or its position | kVhashFound when it was there already.
+static __device__ __noinline__ unsigned vhash_probe(unsigned* table, unsigned pos, unsigned key, unsigned mask) {
+    for (;;) {
+        pos = (pos + 1u) & mask;
+        const unsigned old = atomicCAS(&table[pos], 0u, key);
+        if (old == 0u) return pos;
+        if (old == key) return pos | kVhashFound;
+    }
+}
+// CheckAndSet for a warp-uniform key: every lane walks the same probe sequence from `pos`; lane 0 inserts the key and
+// logs its position at *log_at.  True if the key was present.
+static __device__ __forceinline__ bool vhash_insert_uniform(unsigned* table, unsigned* log_at, unsigned pos, unsigned key,
+                                                            unsigned mask, int lane) {
+    unsigned cur;
+    while ((cur = __ldcg(&table[pos])) != 0u && cur != key) pos = (pos + 1u) & mask;
+    const bool was = cur == key;
+    if (!was && lane == 0) {
+        table[pos] = key;
+        *log_at = pos;
+    }
+    __syncwarp();
+    return was;
+}
+static __device__ __noinline__ bool vhash_insert_uniform_call(unsigned* table, unsigned* log_at, unsigned pos, unsigned key,
+                                                              unsigned mask, int lane) {
+    return vhash_insert_uniform(table, log_at, pos, key, mask, lane);
+}
+
 // Heap::insert (Heap.h:39-62).  The sift-up path (the ancestors loc>>1, loc>>2, ...) is loaded by
 // one lane per level, the stop level is found with a ballot, and the shifted parents plus the new
 // value are stored in one step -- the resulting array is identical to the sequential loop's.
@@ -785,7 +826,8 @@ struct BktNodeDev {
     int centerid, childStart, childEnd;
 };
 
-template <int DIM, bool COSINE, int RPL, bool PQ, int ELEM>
+// HASH: the hashed visited set can be bound (search_kernel); the iterator kernels keep their per-query bitmaps
+template <int DIM, bool COSINE, int RPL, bool PQ, int ELEM, bool HASH = false>
 struct WarpSearch {
     const SearchParams& p;
     const int lane, half, j;
@@ -796,7 +838,7 @@ struct WarpSearch {
     uint64_t* bars;
     float* qs;
     // HBM scratch of this slot
-    unsigned int* visited;
+    unsigned int* visited;  // the bitmap, or the hash table when p.vhash is set
     unsigned int* vlog;  // nullptr when the bitmap is cleared wholesale
     int vlog_count;
     // queues
@@ -840,8 +882,27 @@ struct WarpSearch {
         return ring + (size_t)s * p.slot_stride + (p.slot_stagger ? ((s & 1) << 6) : 0);
     }
 
-    // OptHashPosVector::CheckAndSet for a warp-uniform id: true if already present
+    // the hashed visited set is bound to this launch
+    __device__ __forceinline__ bool hashed() const { return HASH && p.vhash != nullptr; }
+    // hashed visited set: home position of an id in this slot's table
+    __device__ __forceinline__ unsigned vhash_home(int id) const { return ((unsigned)id * 2654435769u) >> p.vhash_shift; }
+    // the query has filled its table to the load limit: it is abandoned (nothing counts as new any more, the search loops
+    // stop) and search_kernel re-runs it on the bitmap.  Never true on the bitmap.
+    __device__ __forceinline__ bool vset_full() const { return HASH && vlog_count >= p.vhash_limit; }
+
+    // OptHashPosVector::CheckAndSet for a warp-uniform id: true if already present.  OUTLINE: the hashed insert is a call
+    // (BKT tree seeding; the KD-tree leaves inline it)
+    template <bool OUTLINE = true>
     __device__ __forceinline__ bool check_and_set_uniform(int id) {
+        if (hashed()) {
+            if (vset_full()) return true;
+            const bool was = OUTLINE ? vhash_insert_uniform_call(visited, vlog + vlog_count, vhash_home(id), (unsigned)id + 1u,
+                                                                 p.vhash_mask, lane)
+                                     : vhash_insert_uniform(visited, vlog + vlog_count, vhash_home(id), (unsigned)id + 1u,
+                                                            p.vhash_mask, lane);
+            if (!was) vlog_count++;
+            return was;
+        }
         const unsigned w = __ldcg(&visited[id >> 5]);
         const unsigned bit = 1u << (id & 31);
         const bool was = (w & bit) != 0;
@@ -1215,7 +1276,7 @@ struct WarpSearch {
 
     // BKTree::SearchTrees (BKTree.h:771-799)
     __device__ __forceinline__ void search_trees(int limit) {
-        while (spt.count != 0) {
+        while (spt.count != 0 && !vset_full()) {
             const int2 bcell = hpop(spt);
             const int centerid = p.nodes[3 * bcell.x], cs = p.nodes[3 * bcell.x + 1], ce = p.nodes[3 * bcell.x + 2];
             ntree++;
@@ -1238,6 +1299,8 @@ struct WarpSearch {
     // "visited" by the time its second copy is reached, so only the first occurrence (the leader) touches the bitmap.
     // issue_mark starts the atomics and returns without reading their result; the caller overlaps other work with the
     // round trip and asks for the verdict later.
+    // Hashed set: the first probe is an atomicCAS at the home position (leaders hold distinct ids and the table is this
+    // warp's own, so only lanes of this warp race); `bit` holds the position and `old` what the CAS found.
     struct RowMark {
         int first_neg;
         bool leader;
@@ -1250,14 +1313,34 @@ struct WarpSearch {
         const bool active = lane < m.first_neg;
         const unsigned same = __match_any_sync(kFull, active ? nn : (-1 - lane));
         m.leader = active && ((__ffs(same) - 1) == lane);
-        m.bit = 1u << (nn & 31);
         m.old = 0xffffffffu;
-        if (m.leader) m.old = atomicOr(&visited[nn >> 5], m.bit);
+        if (hashed()) {
+            m.leader = m.leader && !vset_full();
+            m.bit = vhash_home(nn);
+            if (m.leader) m.old = atomicCAS(&visited[m.bit], 0u, (unsigned)nn + 1u);
+        } else {
+            m.bit = 1u << (nn & 31);
+            if (m.leader) m.old = atomicOr(&visited[nn >> 5], m.bit);
+        }
         return m;
     }
-    // L2 prefetch of the bitmap words the next step will update (no data returns to the SM)
+    // the verdict of issue_mark: this lane's id was not visited before.  Hashed set: the probe continues past positions
+    // that hold other ids (another lane's id may have just taken the home position); `bit` ends at the id's position.
+    __device__ __forceinline__ bool mark_fresh(RowMark& m, int nn) {
+        if (!hashed()) return m.leader && (m.old & m.bit) == 0;
+        if (!m.leader || m.old == (unsigned)nn + 1u) return false;
+        if (m.old == 0u) return true;
+        const unsigned r = vhash_probe(visited, m.bit, (unsigned)nn + 1u, p.vhash_mask);
+        m.bit = r & ~kVhashFound;
+        return (r & kVhashFound) == 0;
+    }
+    // what the clear log records for a fresh id: its bitmap word, or its table position
+    __device__ __forceinline__ unsigned mark_word(const RowMark& m, int nn) const {
+        return hashed() ? m.bit : (unsigned)(nn >> 5);
+    }
+    // L2 prefetch of the bitmap words (table home positions) the next step will update (no data returns to the SM)
     __device__ __forceinline__ void prefetch_marks(int nn) {
-        if (nn >= 0) asm volatile("prefetch.global.L2 [%0];" ::"l"(visited + (nn >> 5)));
+        if (nn >= 0) asm volatile("prefetch.global.L2 [%0];" ::"l"(visited + (hashed() ? vhash_home(nn) : (unsigned)(nn >> 5))));
     }
 
     // BKT::Index<T>::Search<notDeleted, CheckDup, AlwaysTrue> (BKTIndex.cpp:268-352).
@@ -1278,7 +1361,7 @@ struct WarpSearch {
         for (;;) {
             if (reseed) search_trees(tree_limit);
             if (pre_id >= 0 && ng.count != 0 && ng.s[1].x == pre_id) prefetch_marks(pre_nn);
-            if (ng.count == 0) break;
+            if (ng.count == 0 || vset_full()) break;
             const int2 gnode = ng.s[1];  // what Heap::pop will return
             int tmpNode = gnode.x;
             const float gdist = pair_dist(gnode);
@@ -1332,14 +1415,14 @@ struct WarpSearch {
                     nn = (cbase + lane <= checkPos) ? node[cbase + lane] : -1;
                     mark = issue_mark(nn, cbase + lane <= checkPos);
                 }
-                const bool fresh = mark.leader && (mark.old & mark.bit) == 0;
+                const bool fresh = mark_fresh(mark, nn);
                 const unsigned freshmask = __ballot_sync(kFull, fresh);
                 const int cnt = __popc(freshmask);
                 __syncwarp();
                 if (fresh) {
                     const int rank = __popc(freshmask & ((1u << lane) - 1u));
                     cand_id[rank] = nn;
-                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = (unsigned)(nn >> 5);
+                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = mark_word(mark, nn);
                 }
                 vlog_count += cnt;
                 compute_dists(cnt);
@@ -1373,7 +1456,7 @@ struct WarpSearch {
         int tree_limit = p.initial_pivots;
         for (;;) {
             if (reseed) search_trees(tree_limit);
-            if (ng.count == 0) break;
+            if (ng.count == 0 || vset_full()) break;
             const int2 gnode = hpop(ng);
             int tmpNode = gnode.x;
             const float gdist = pair_dist(gnode);
@@ -1409,27 +1492,17 @@ struct WarpSearch {
 
             for (int cbase = 0; cbase <= checkPos; cbase += 32) {
                 if (cbase > 0) nn = (cbase + lane <= checkPos) ? node[cbase + lane] : -1;
-                const bool in_row = (cbase + lane <= checkPos);
-                // the scan stops at the first negative entry (BKTIndex.cpp:333-336)
-                const unsigned negmask = __ballot_sync(kFull, in_row && nn < 0) | ~__ballot_sync(kFull, in_row);
-                const int first_neg = negmask ? (__ffs(negmask) - 1) : 32;
-                const bool active = lane < first_neg;
-                // a repeated id inside the row is "visited" by the time its second copy is reached
-                const unsigned same = __match_any_sync(kFull, active ? nn : (-1 - lane));
-                const bool leader = active && ((__ffs(same) - 1) == lane);
-                bool fresh = false;
-                if (leader) {
-                    const unsigned bit = 1u << (nn & 31);
-                    const unsigned old = atomicOr(&visited[nn >> 5], bit);
-                    fresh = (old & bit) == 0;
-                }
+                // the scan stops at the first negative entry (BKTIndex.cpp:333-336); a repeated id inside the row is
+                // "visited" by the time its second copy is reached
+                RowMark mark = issue_mark(nn, cbase + lane <= checkPos);
+                const bool fresh = mark_fresh(mark, nn);
                 const unsigned freshmask = __ballot_sync(kFull, fresh);
                 const int cnt = __popc(freshmask);
                 __syncwarp();
                 if (fresh) {
                     const int rank = __popc(freshmask & ((1u << lane) - 1u));
                     cand_id[rank] = nn;
-                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = (unsigned)(nn >> 5);
+                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = mark_word(mark, nn);
                 }
                 vlog_count += cnt;
                 compute_dists(cnt);
@@ -1446,7 +1519,7 @@ struct WarpSearch {
                     const int id = __shfl_sync(kFull, myid, r);
                     if (mres.insert(d, lane)) hins(ng, id, d);
                 }
-                if (first_neg < 32) break;
+                if (mark.first_neg < 32) break;
             }
             reseed = heap_top_dist(ng) > heap_top_dist(spt);
             tree_limit = p.other_pivots + checked;
@@ -1590,7 +1663,7 @@ struct WarpSearch {
             if (node < 0) {
                 const int index = -node - 1;
                 if (index >= p.n) return;
-                if (check_and_set_uniform(index)) return;
+                if (check_and_set_uniform<false>(index)) return;
                 ++tree_checked;
                 ++checked;
                 __syncwarp();
@@ -1624,7 +1697,7 @@ struct WarpSearch {
     }
 
     __device__ __forceinline__ void kdt_search_trees(int limit) {
-        while (spt.count != 0 && checked < limit) {
+        while (spt.count != 0 && checked < limit && !vset_full()) {
             const int2 tcell = hpop_k(spt);
             kdt_search_node(tcell.x, pair_dist(tcell));
         }
@@ -1634,7 +1707,7 @@ struct WarpSearch {
         for (int t = 0; t < p.tree_num; ++t) kdt_search_node(p.tree_starts[t], 0.0f);
         kdt_search_trees(p.initial_pivots);
         int pre_id = -1, pre_nn = -1;  // graph row of NGQueue's new top, fetched one step ahead (see bkt_search)
-        while (ng.count != 0) {
+        while (ng.count != 0 && !vset_full()) {
             const int2 gnode = ng.s[1];  // what Heap::pop will return
             const float gdist = pair_dist(gnode);
             const int* node = p.graph + (size_t)gnode.x * p.degree;
@@ -1661,14 +1734,14 @@ struct WarpSearch {
                     nn = (cbase + lane < p.degree) ? node[cbase + lane] : -1;
                     mark = issue_mark(nn, cbase + lane < p.degree);
                 }
-                const bool fresh = mark.leader && (mark.old & mark.bit) == 0;
+                const bool fresh = mark_fresh(mark, nn);
                 const unsigned freshmask = __ballot_sync(kFull, fresh);
                 const int cnt = __popc(freshmask);
                 __syncwarp();
                 if (fresh) {
                     const int rank = __popc(freshmask & ((1u << lane) - 1u));
                     cand_id[rank] = nn;
-                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = (unsigned)(nn >> 5);
+                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = mark_word(mark, nn);
                 }
                 vlog_count += cnt;
                 compute_dists(cnt);
@@ -1698,7 +1771,7 @@ struct WarpSearch {
     __device__ __forceinline__ void kdt_search_legacy() {
         for (int t = 0; t < p.tree_num; ++t) kdt_search_node(p.tree_starts[t], 0.0f);
         kdt_search_trees(p.initial_pivots);
-        while (ng.count != 0) {
+        while (ng.count != 0 && !vset_full()) {
             const int2 gnode = hpop(ng);
             const float gdist = pair_dist(gnode);
             const int* node = p.graph + (size_t)gnode.x * p.degree;
@@ -1711,25 +1784,15 @@ struct WarpSearch {
             bool bLocalOpt = true;
             for (int cbase = 0; cbase < p.degree; cbase += 32) {
                 if (cbase > 0) nn = (cbase + lane < p.degree) ? node[cbase + lane] : -1;
-                const bool in_row = (cbase + lane < p.degree);
-                const unsigned negmask = __ballot_sync(kFull, in_row && nn < 0) | ~__ballot_sync(kFull, in_row);
-                const int first_neg = negmask ? (__ffs(negmask) - 1) : 32;
-                const bool active = lane < first_neg;
-                const unsigned same = __match_any_sync(kFull, active ? nn : (-1 - lane));
-                const bool leader = active && ((__ffs(same) - 1) == lane);
-                bool fresh = false;
-                if (leader) {
-                    const unsigned bit = 1u << (nn & 31);
-                    const unsigned old = atomicOr(&visited[nn >> 5], bit);
-                    fresh = (old & bit) == 0;
-                }
+                RowMark mark = issue_mark(nn, cbase + lane < p.degree);
+                const bool fresh = mark_fresh(mark, nn);
                 const unsigned freshmask = __ballot_sync(kFull, fresh);
                 const int cnt = __popc(freshmask);
                 __syncwarp();
                 if (fresh) {
                     const int rank = __popc(freshmask & ((1u << lane) - 1u));
                     cand_id[rank] = nn;
-                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = (unsigned)(nn >> 5);
+                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = mark_word(mark, nn);
                 }
                 vlog_count += cnt;
                 compute_dists(cnt);
@@ -1739,7 +1802,7 @@ struct WarpSearch {
                     checked++;
                     hins(ng, cand_id[r], d);
                 }
-                if (first_neg < 32) break;
+                if (mark.first_neg < 32) break;
             }
             if (bLocalOpt)
                 no_better++;
@@ -1765,13 +1828,13 @@ template <int DIM, bool COSINE, int RPL, bool KDT, bool PQ = false, int ELEM = 0
 __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) {
     extern __shared__ __align__(128) unsigned char smem[];
     const int lane = threadIdx.x;
-    WarpSearch<DIM, COSINE, RPL, PQ, ELEM> w(p, lane);
+    WarpSearch<DIM, COSINE, RPL, PQ, ELEM, true> w(p, lane);
     w.ring = smem;
     w.cand_id = reinterpret_cast<int*>(smem + p.off_cand);
     w.cand_dist = reinterpret_cast<float*>(smem + p.off_cand + 128);
     w.bars = reinterpret_cast<uint64_t*>(smem + p.off_bar);
     w.qs = reinterpret_cast<float*>(smem + p.off_query);
-    w.visited = p.visited + (size_t)blockIdx.x * p.visited_words;
+    w.visited = p.vhash ? p.vhash + (size_t)blockIdx.x * (p.vhash_mask + 1ull) : p.visited + (size_t)blockIdx.x * p.visited_words;
     w.vlog = p.vlog ? p.vlog + (size_t)blockIdx.x * p.vlog_entries : nullptr;
     w.tk = p.topk ? p.topk + (size_t)blockIdx.x * p.topk_pad : nullptr;
     w.ng.s = reinterpret_cast<int2*>(smem + p.off_ng);
@@ -1795,10 +1858,17 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
     __syncwarp();
 
     for (;;) {
-        int q = 0;
-        if (lane == 0) q = (int)atomicAdd(p.work_counter, 1u);
+        // unsigned: the output offsets below zero-extend it, so nothing about it has to be kept live across the search
+        unsigned q = 0;
+        if (lane == 0) q = atomicAdd(p.work_counter, 1u);
         q = __shfl_sync(kFull, q, 0);
-        if (q >= p.nq) break;
+        // the re-run launch after a hashed-set launch searches the queries on the overflow list that launch left behind
+        if (p.rerun) {
+            if (q >= p.rerun[0]) break;
+            q = p.rerun[1 + q];
+        } else if (q >= (unsigned)p.nq) {
+            break;
+        }
 
         // ---- WorkSpace::Reset (WorkSpace.h:265-278) ----
         if (w.vlog == nullptr) {
@@ -1866,7 +1936,8 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
         else
             w.bkt_search();
 
-        // log mode: leave the bitmap clean for the next query of this slot
+        // log mode and hashed set: leave the bitmap / table clean for the next query of this slot (the table's log never
+        // overflows: it holds the load limit plus one row chunk)
         if (w.vlog != nullptr) {
             __syncwarp();
             if (w.vlog_count <= (int)p.vlog_entries) {
@@ -1877,6 +1948,13 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
                 for (size_t i = lane; i < n4; i += 32) v4[i] = make_uint4(0, 0, 0, 0);
             }
             __syncwarp();
+        }
+        // hashed set filled to its limit: the result is incomplete; the re-run launch searches the query again and writes
+        // all of its outputs
+        if (w.vset_full()) {
+            if (lane == 0) p.overflow[1 + atomicAdd(p.overflow, 1u)] = q;
+            __syncwarp();
+            continue;
         }
         // ---- QueryResultSet::SortResult: the register list is already ascending by (dist, id) ----
         if (w.tk != nullptr) {

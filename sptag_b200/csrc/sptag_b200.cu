@@ -12,6 +12,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cfloat>
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -130,6 +131,10 @@ struct sptag_b200_index {
     int slot_scheme = 0;          // 0 auto, 1 = 128-multiple stride + staggered odd slots, 2 = stride 64 mod 128
     int visited_log = -1;         // -1 auto (bitmap > 256 KB per slot), 0 clear per query, 1 log + selective clear
     int visited_log_entries = 0;  // 0 = auto
+    // -1 auto (the bitmap unless its per-slot allocation fails), 0 bitmap, 1 hashed set per slot
+    int visited_set = -1;
+    int visited_hash_entries = 0;  // table entries per slot, 0 = 2^(bits(max(MaxCheck, MaxCheckForRefineGraph)) + 2)
+    std::atomic<int> last_visited_overflows{0};  // queries the hashed set handed to the re-run, last blocking search
     // PQ / OPQ quantizer (null when q_type == 0)
     int q_type = 0, q_rtype = SPTAG_B200_VT_FLOAT, q_m = 0, q_ks = 0, q_dsub = 0;
     int q_adc = 0;  // IQuantizer::SetEnableADC (not serialized by the reference either)
@@ -140,15 +145,25 @@ struct sptag_b200_index {
     // still busy with a launch from ANOTHER stream the new launch takes set 1 (allocated on first use), so two batches
     // can be in flight -- the second kernel's CTAs take over SM by SM as the first kernel's persistent warps run out of
     // queries, which hides the tail of a batch.
+    // Hashed visited set: d_vhash holds the per-slot tables, d_vlog their clear logs, d_overflow the abandoned queries, and
+    // d_visited only the bitmaps of the re-run grid.
     struct Scratch {
-        DeviceBuffer d_visited, d_ng_spill, d_spt_spill, d_counter, d_vlog, d_topk, d_codes, d_adc;
+        DeviceBuffer d_visited, d_ng_spill, d_spt_spill, d_counter, d_vlog, d_topk, d_codes, d_adc, d_vhash, d_overflow;
         bool visited_clean = false;   // the whole d_visited buffer is known to be zero
+        // auto visited set: the size of a per-slot bitmap allocation that failed for lack of memory (0 = none).  Launches
+        // that need at least as much skip the attempt (set 0 binds the hashed set, set 1 defers to set 0), so the failed
+        // cudaMalloc and the free that precedes it are not repeated per call.  Cleared by setting B200.VisitedSet.
+        size_t bitmap_unfit = 0;
         cudaEvent_t ev_done = nullptr;  // recorded after every kernel that uses this set; the next launch on it waits
         cudaStream_t last_stream = nullptr;
         bool used = false;
         void release() {  // early free: set 1 did not fit in HBM and the launch falls back to set 0
             d_visited.release(); d_ng_spill.release(); d_spt_spill.release(); d_counter.release(); d_vlog.release();
-            d_topk.release(); d_codes.release(); d_adc.release();
+            d_topk.release(); d_codes.release(); d_adc.release(); d_vhash.release(); d_overflow.release();
+        }
+        size_t bytes() const {
+            return d_visited.bytes + d_ng_spill.bytes + d_spt_spill.bytes + d_counter.bytes + d_vlog.bytes + d_topk.bytes +
+                   d_codes.bytes + d_adc.bytes + d_vhash.bytes + d_overflow.bytes;
         }
     } scratch[2];
     DeviceBuffer d_ids, d_dists;                      // refine pass: per-batch result lists
@@ -157,7 +172,7 @@ struct sptag_b200_index {
     struct Staging {
         std::mutex mu;
         cudaStream_t stream = nullptr;
-        DeviceBuffer d_queries, d_ids, d_dists, d_stats, d_filter;
+        DeviceBuffer d_queries, d_ids, d_dists, d_stats, d_filter, d_overflows;
     } staging[2];
     std::atomic<unsigned> staging_rr{0};
     DeviceBuffer d_graph_new;                         // sptag_b200_refine_graph: the pass's output rows
@@ -215,6 +230,7 @@ struct CallOpts {
     // test the tombstone map even while the host's count is 0: DeleteIndex(vectors) tombstones on the device between two
     // of its searches (an all-zero map rejects nothing, so this equals the reference's Count() == 0 dispatch)
     bool tombstones_live = false;
+    int* d_overflows = nullptr;  // device int: receives how many queries the hashed set handed to the re-run (bitmap: 0)
 };
 
 // Slots of a result heap kept in HBM for k results: a power of two (the final sort is bitonic), at least 64
@@ -318,6 +334,20 @@ void fill_params(const sptag_b200_index* h, int k, const CallOpts& opts, SearchP
                                                           : (size_t)std::max(65536, 8 * alloc_check);
         p.vlog_entries = std::min(entries, (size_t)h->n + 2);
     }
+    // hashed visited set, bound only by bind_scratch: the reference's first-block size 2^(bits(max(MaxCheck,
+    // MaxCheckForRefineGraph)) + HashTableExponent 2) (WorkSpace.h:83-93) unless B200.VisitedHashEntries sets it
+    // At least 64 entries: a query stops inserting at half the capacity, and the last row chunk may add up to 31 ids past
+    // that, which must still find an empty position (the probes end only at one).
+    int log2_entries = 0;
+    if (h->visited_hash_entries > 0) {
+        while ((1 << log2_entries) < h->visited_hash_entries) ++log2_entries;
+    } else {
+        for (unsigned s = (unsigned)std::max(alloc_check, 1); s != 0; s >>= 1) ++log2_entries;
+        log2_entries = std::min(std::max(log2_entries + 2, 6), 30);
+    }
+    p.vhash_mask = (1u << log2_entries) - 1u;
+    p.vhash_shift = 32 - log2_entries;
+    p.vhash_limit = INT_MAX;
     if (k > 32) p.topk_pad = topk_pad_for(k);  // result heap of the reference in HBM, one arena per slot
 }
 
@@ -441,20 +471,54 @@ int lay_out(const sptag_b200_index* h, int nq, SearchLaunch& L) {
 int plan_search(const sptag_b200_index* h, int k, int nq, const CallOpts& opts, SearchLaunch& L) {
     if (int rc = check_supported(h, k)) return rc;
     fill_params(h, k, opts, L.p);
+    L.p.nq = nq;
     return lay_out(h, nq, L);
 }
 
-// Point the launch at scratch set `set`, allocated for every resident slot (grown, never shrunk).  Caller holds h->mu.
+// Grid of the launch that re-runs, on the bitmap, the queries a hashed-set launch abandoned: one slot per SM
+int rerun_grid(const sptag_b200_index* h, int nq) { return std::max(1, std::min(nq, h->num_sms)); }
+constexpr int kRerunCounter = 32;  // the re-run's work counter: word 32 of the set's 256-byte counter block
+
+// Point the launch at scratch set `set`, allocated for every resident slot (grown, never shrunk).  The visited set is
+// the bitmap per slot, or the hashed set (B200.VisitedSet = 1, or auto when the bitmaps do not fit in HBM).  L.p is
+// changed only on success.  Caller holds h->mu.
 int bind_scratch(sptag_b200_index* h, SearchLaunch& L, int set) {
     sptag_b200_index::Scratch& sc = h->scratch[set];
-    SearchParams& p = L.p;
+    SearchParams p = L.p;
     const size_t alloc_slots = (size_t)h->num_sms * L.per_sm;
-    {
+    const size_t bitmap_bytes = alloc_slots * p.visited_words * 4;
+    bool hashed = h->visited_set == 1;
+    if (!hashed && h->visited_set < 0 && sc.bitmap_unfit != 0 && bitmap_bytes >= sc.bitmap_unfit) {
+        // auto, and a bitmap this large did not fit before: set 1 defers to set 0 (search_device_impl), set 0 is hashed
+        if (set != 0) return fail(SPTAG_B200_MEMORY_OVERFLOW, "visited bitmaps of %zu bytes do not fit", bitmap_bytes);
+        hashed = true;
+    } else if (!hashed) {
         const size_t before = sc.d_visited.bytes;
-        if (int rc = sc.d_visited.ensure(alloc_slots * p.visited_words * 4)) return rc;
+        if (int rc = sc.d_visited.ensure(bitmap_bytes)) {
+            if (h->visited_set == 0 || cudaGetLastError() != cudaErrorMemoryAllocation) return rc;
+            // auto: the per-slot bitmaps do not fit (the failed cudaMalloc's error is cleared above).  Set 1 lets the launch
+            // run behind set 0 as before; set 0 binds the hashed set.
+            sc.bitmap_unfit = bitmap_bytes;
+            if (set != 0) return rc;
+            hashed = true;
+        }
         if (sc.d_visited.bytes != before) sc.visited_clean = false;
     }
-    if (p.vlog_entries) {
+    if (hashed) {
+        const size_t entries = (size_t)p.vhash_mask + 1;
+        p.vhash_limit = (int)(entries / 2);
+        p.vlog_entries = (size_t)p.vhash_limit + 32;  // a query stops inserting at the limit; one row chunk may cross it
+        const size_t before = sc.d_vhash.bytes;
+        if (int rc = sc.d_vhash.ensure(alloc_slots * entries * 4)) return rc;
+        if (sc.d_vhash.bytes != before) CUDA_OK(cudaMemset(sc.d_vhash.ptr, 0, sc.d_vhash.bytes));  // queries leave it empty
+        if (int rc = sc.d_vlog.ensure(alloc_slots * p.vlog_entries * 4)) return rc;
+        if (int rc = sc.d_overflow.ensure(((size_t)p.nq + 1) * 4)) return rc;
+        if (int rc = sc.d_visited.ensure((size_t)rerun_grid(h, p.nq) * p.visited_words * 4)) return rc;
+        sc.visited_clean = false;  // the re-run clears its bitmap per query
+        p.vhash = (unsigned int*)sc.d_vhash.ptr;
+        p.vlog = (unsigned int*)sc.d_vlog.ptr;
+        p.overflow = (unsigned int*)sc.d_overflow.ptr;
+    } else if (p.vlog_entries) {
         if (int rc = sc.d_vlog.ensure(alloc_slots * p.vlog_entries * 4)) return rc;
         p.vlog = (unsigned int*)sc.d_vlog.ptr;
         if (!sc.visited_clean) {  // log mode relies on every query leaving its bitmap zeroed
@@ -479,6 +543,7 @@ int bind_scratch(sptag_b200_index* h, SearchLaunch& L, int set) {
     p.ng_spill = (int2*)sc.d_ng_spill.ptr;
     p.spt_spill = (int2*)sc.d_spt_spill.ptr;
     p.work_counter = (unsigned int*)sc.d_counter.ptr;
+    L.p = p;
     return 0;
 }
 
@@ -572,11 +637,36 @@ int search_device_impl(sptag_b200_index* h, const void* d_queries, int nq, int k
     p.out_dists = d_dists;
     p.out_stats = d_stats;
     CUDA_OK(cudaMemsetAsync(p.work_counter, 0, 4, stream));
+    if (p.vhash) {
+        CUDA_OK(cudaMemsetAsync(p.work_counter + kRerunCounter, 0, 4, stream));
+        CUDA_OK(cudaMemsetAsync(p.overflow, 0, 4, stream));
+    }
     CUDA_OK(cudaEventRecord(h->ev_start, stream));
     L.kern<<<L.grid, 32, L.smem, stream>>>(p);
     g_launches++;
     CUDA_OK(cudaGetLastError());
+    if (p.vhash) {
+        // the queries that filled their table run again on the bitmap: same stream, no host synchronisation; the count
+        // is read on the device, so an empty list costs one near-empty launch
+        SearchParams r = p;
+        r.vhash = nullptr;
+        r.vhash_limit = INT_MAX;
+        r.vlog = nullptr;  // clear the bitmap per query
+        r.vlog_entries = 0;
+        r.overflow = nullptr;
+        r.rerun = p.overflow;
+        r.work_counter = p.work_counter + kRerunCounter;
+        L.kern<<<rerun_grid(h, nq), 32, L.smem, stream>>>(r);
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+    }
     CUDA_OK(cudaEventRecord(h->ev_stop, stream));
+    if (opts.d_overflows) {
+        if (p.vhash)
+            CUDA_OK(cudaMemcpyAsync(opts.d_overflows, p.overflow, 4, cudaMemcpyDeviceToDevice, stream));
+        else
+            CUDA_OK(cudaMemsetAsync(opts.d_overflows, 0, 4, stream));
+    }
     h->timed = true;
     return scratch_release(h, stream, set);
 }
@@ -1203,6 +1293,15 @@ int sptag_b200_set_param(sptag_b200_handle h, const char* name, const char* valu
     else if (n == "B200.SimdWidth") h->simd_width = (int)v;
     else if (n == "B200.VisitedLog") h->visited_log = (int)v;
     else if (n == "B200.VisitedLogEntries") h->visited_log_entries = (int)v;
+    else if (n == "B200.VisitedSet") {
+        if (v < -1 || v > 1) return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.VisitedSet %ld: -1 (auto), 0 (bitmap) or 1 (hashed)", v);
+        h->visited_set = (int)v;
+        for (auto& sc : h->scratch) sc.bitmap_unfit = 0;  // auto tries the bitmap again
+    } else if (n == "B200.VisitedHashEntries") {
+        if (v != 0 && (v < 64 || v > (1l << 30) || (v & (v - 1)) != 0))
+            return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.VisitedHashEntries %ld: 0 (default) or a power of two in [64, 2^30]", v);
+        h->visited_hash_entries = (int)v;
+    }
     else if (n == "B200.SlotScheme") h->slot_scheme = (int)v;
     else if (n == "EnableADC") h->q_adc = (v != 0);  // VectorIndex::SetQuantizerADC (VectorIndex.h:136-138)
     else return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
@@ -1234,6 +1333,10 @@ int sptag_b200_get_param(sptag_b200_handle h, const char* name, char* value_out,
     else if (n == "B200.SimdWidth") v = h->simd_width;
     else if (n == "B200.VisitedLog") v = h->visited_log;
     else if (n == "B200.VisitedLogEntries") v = h->visited_log_entries;
+    else if (n == "B200.VisitedSet") v = h->visited_set;
+    else if (n == "B200.VisitedHashEntries") v = h->visited_hash_entries;
+    else if (n == "B200.LastVisitedOverflows") v = h->last_visited_overflows;       // read-only
+    else if (n == "B200.ScratchBytes") v = (long)(h->scratch[0].bytes() + h->scratch[1].bytes());  // read-only
     else if (n == "B200.SlotScheme") v = h->slot_scheme;
     else if (n == "EnableADC") v = h->q_adc;
     else if (n == "B200.LastRefineSearchUs") v = (long)(h->refine_search_ms * 1000.0);    // read-only: device time
@@ -1282,6 +1385,8 @@ int search_host_impl(sptag_b200_handle h, const void* queries, int32_t num_queri
     if (int rc = st->d_dists.ensure(rn * 4)) return rc;
     if (out_stats)
         if (int rc = st->d_stats.ensure((size_t)num_queries * kStatsPerQuery * 4)) return rc;
+    if (int rc = st->d_overflows.ensure(4)) return rc;
+    opts.d_overflows = (int*)st->d_overflows.ptr;
     cudaStream_t stream = st->stream;
     CUDA_OK(cudaMemcpyAsync(st->d_queries.ptr, queries, qbytes, cudaMemcpyHostToDevice, stream));
     int map_n = 0;
@@ -1312,7 +1417,10 @@ int search_host_impl(sptag_b200_handle h, const void* queries, int32_t num_queri
     if (out_stats)
         CUDA_OK(cudaMemcpyAsync(out_stats, st->d_stats.ptr, (size_t)num_queries * kStatsPerQuery * 4,
                                 cudaMemcpyDeviceToHost, stream));
+    int overflows = 0;
+    CUDA_OK(cudaMemcpyAsync(&overflows, st->d_overflows.ptr, 4, cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaStreamSynchronize(stream));
+    h->last_visited_overflows = overflows;
     return SPTAG_B200_SUCCESS;
 }
 }  // namespace
