@@ -576,4 +576,49 @@ __global__ void merge_topk_peer_kernel(const ShardLists lists, int num_lists, in
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// Iterators on hashed visited sets
+// ------------------------------------------------------------------------------------------
+// The largest duplicate group of a BKT tree (a node with childStart < -1 lists its members at [-childStart, childEnd)):
+// with the graph degree it bounds how many ids one step of SearchIterative inserts into the visited set
+__global__ void max_dup_group_kernel(const int* __restrict__ nodes, int node_count, int* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= node_count) return;
+    const int cs = nodes[3 * i + 1], ce = nodes[3 * i + 2];
+    if (cs < -1 && ce + cs > 0) atomicMax(out, ce + cs);
+}
+
+// One query's visited set moving to a new, zeroed allocation: a table of 2^new_bits entries, or a bitmap (new_bits = 0)
+struct IterGrowJob {
+    const unsigned int* old_set;
+    unsigned int* new_set;
+    int q, old_bits, new_bits;
+    int keep;  // carry the ids over; 0: the query's call runs again from the start
+};
+// One warp per job: the keys (id + 1) of the old table into the new table (linear probing from the same multiplicative
+// hash as the kernels; the keys are distinct, so each lane only looks for an empty position) or into the new bitmap; then
+// the query's set pointer and capacity switch over
+__global__ void iter_grow_kernel(const IterGrowJob* __restrict__ jobs, unsigned int** tables, int* __restrict__ state) {
+    const IterGrowJob j = jobs[blockIdx.x];
+    const int lane = threadIdx.x;
+    if (j.keep && j.old_bits) {
+        const unsigned n = 1u << j.old_bits;
+        const unsigned mask = j.new_bits ? (1u << j.new_bits) - 1u : 0u;
+        for (unsigned i = lane; i < n; i += 32) {
+            const unsigned key = j.old_set[i];
+            if (key == 0u) continue;
+            if (j.new_bits) {
+                unsigned pos = ((key - 1u) * 2654435769u) >> (32 - j.new_bits);
+                while (atomicCAS(&j.new_set[pos], 0u, key) != 0u) pos = (pos + 1u) & mask;
+            } else {
+                atomicOr(&j.new_set[(key - 1u) >> 5], 1u << ((key - 1u) & 31));
+            }
+        }
+    }
+    if (lane == 0) {
+        tables[j.q] = j.new_set;
+        state[(size_t)j.q * kIterStateInts + 5] = j.new_bits;
+    }
+}
+
 }  // namespace sptag_b200

@@ -8,9 +8,10 @@
 namespace sptag_b200 {
 
 struct SearchParams;
+struct IterVisited;
 typedef void (*SearchKernelFn)(const SearchParams);
-typedef void (*IterateKernelFn)(const SearchParams, int*, int*, unsigned char*);
-typedef void (*NearestFirstKernelFn)(const SearchParams, int*);
+typedef void (*IterateKernelFn)(const SearchParams, int*, int*, unsigned char*, const IterVisited);
+typedef void (*NearestFirstKernelFn)(const SearchParams, int*, const IterVisited);
 
 // float rows; dim 128 / 768 select the register-resident query variants
 // slots: query slots per SM the host aims at (512-byte rows: register-capped variants above 16)

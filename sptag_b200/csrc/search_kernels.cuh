@@ -38,6 +38,23 @@ namespace sptag_b200 {
 constexpr unsigned kFull = 0xffffffffu;
 constexpr int kStatsPerQuery = 8;
 
+// Where an iterator call starts or resumes (state word 7 of a suspended query holds the resume point; 0: none)
+constexpr int kIterDone = 0, kIterStep = 1, kIterInitTrees = 2, kIterStepTrees = 3, kIterFirst = 4;
+// Per-query HBM area of a suspended iterator call: the m_Results multiset (32 x RPL <= 1024 floats), then resultCount,
+// the checked count and the pending SearchTrees limit
+constexpr int kIterResumeWords = 32 * 32 + 4;
+// Suspension list header: {queries listed, step suspensions, tree suspensions, pad}, then the query indices
+constexpr int kIterListHeader = 4;
+
+// The iterator kernels' visited sets (the per-launch part; the per-query part is in the iterator state)
+struct IterVisited {
+    unsigned int* const* tables;  // per query: its hash table, or its bitmap (state word 5 = 0); nullptr: p.visited bitmaps
+    float* resume;                // per query kIterResumeWords
+    unsigned int* suspended;      // the queries that stopped at their table's limit (kIterListHeader + nq words)
+    const unsigned int* list;     // resume launch: run only the queries listed here (same layout); nullptr = all nq
+    int margin;                   // degree + largest duplicate group + 1: more than one NGQueue step can insert
+};
+
 struct SearchParams {
     // index (device resident)
     const unsigned char* vectors;          // rows padded to a 16-byte multiple
@@ -548,8 +565,9 @@ static __device__ __noinline__ unsigned vhash_probe(unsigned* table, unsigned po
         if (old == key) return pos | kVhashFound;
     }
 }
-// CheckAndSet for a warp-uniform key: every lane walks the same probe sequence from `pos`; lane 0 inserts the key and
-// logs its position at *log_at.  True if the key was present.
+// CheckAndSet for a warp-uniform key: every lane walks the same probe sequence from `pos`; lane 0 inserts the key and,
+// with LOG, logs its position at *log_at.  True if the key was present.
+template <bool LOG = true>
 static __device__ __forceinline__ bool vhash_insert_uniform(unsigned* table, unsigned* log_at, unsigned pos, unsigned key,
                                                             unsigned mask, int lane) {
     unsigned cur;
@@ -557,7 +575,7 @@ static __device__ __forceinline__ bool vhash_insert_uniform(unsigned* table, uns
     const bool was = cur == key;
     if (!was && lane == 0) {
         table[pos] = key;
-        *log_at = pos;
+        if (LOG) *log_at = pos;
     }
     __syncwarp();
     return was;
@@ -817,6 +835,24 @@ struct MResults {
         worst = key_float(__reduce_max_sync(kFull, float_key(lmax)));
         return true;
     }
+    // a suspended iterator call keeps its multiset in HBM (32 * RPL floats) until it resumes
+    __device__ __forceinline__ void save(float* dst, int lane) const {
+#pragma unroll
+        for (int r = 0; r < RPL; ++r) dst[r * 32 + lane] = m[r];
+    }
+    __device__ __forceinline__ void load(const float* src, int lane) {
+#pragma unroll
+        for (int r = 0; r < RPL; ++r) m[r] = src[r * 32 + lane];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            float v = -INFINITY;
+#pragma unroll
+            for (int r = 0; r < G; ++r) v = fmaxf(v, m[k * G + r]);
+            g[k] = v;
+        }
+        lmax = fmaxf(fmaxf(g[0], g[1]), fmaxf(g[2], g[3]));
+        worst = key_float(__reduce_max_sync(kFull, float_key(lmax)));
+    }
 };
 
 // ------------------------------------------------------------------------------------------
@@ -826,8 +862,9 @@ struct BktNodeDev {
     int centerid, childStart, childEnd;
 };
 
-// HASH: the hashed visited set can be bound (search_kernel); the iterator kernels keep their per-query bitmaps
-template <int DIM, bool COSINE, int RPL, bool PQ, int ELEM, bool HASH = false>
+// HASH: the hashed visited set can be bound (search_kernel).  QHASH: the visited set is chosen per query (the iterator
+// kernels): a hash table whose capacity the query carries in qmask / qshift / qlimit, or a bitmap (qmask = 0).
+template <int DIM, bool COSINE, int RPL, bool PQ, int ELEM, bool HASH = false, bool QHASH = false>
 struct WarpSearch {
     const SearchParams& p;
     const int lane, half, j;
@@ -840,7 +877,11 @@ struct WarpSearch {
     // HBM scratch of this slot
     unsigned int* visited;  // the bitmap, or the hash table when p.vhash is set
     unsigned int* vlog;  // nullptr when the bitmap is cleared wholesale
-    int vlog_count;
+    int vlog_count;      // ids inserted (QHASH: the fill of the query's set, kept across calls)
+    // QHASH: this query's table entries - 1 (0: its bitmap), 32 - log2(entries), and the fill at which it stops inserting
+    unsigned qmask;
+    int qshift, qlimit;
+    bool trees_cut;      // QHASH: search_trees stopped before a pop because the table was at its limit
     // queues
     WarpHeap ng, spt;
     MResults<RPL> mres;
@@ -882,13 +923,19 @@ struct WarpSearch {
         return ring + (size_t)s * p.slot_stride + (p.slot_stagger ? ((s & 1) << 6) : 0);
     }
 
-    // the hashed visited set is bound to this launch
-    __device__ __forceinline__ bool hashed() const { return HASH && p.vhash != nullptr; }
+    // the hashed visited set is bound to this launch (QHASH: to this query)
+    __device__ __forceinline__ bool hashed() const { return (HASH && p.vhash != nullptr) || (QHASH && qmask != 0u); }
+    __device__ __forceinline__ unsigned vhash_mask() const { return QHASH ? qmask : p.vhash_mask; }
     // hashed visited set: home position of an id in this slot's table
-    __device__ __forceinline__ unsigned vhash_home(int id) const { return ((unsigned)id * 2654435769u) >> p.vhash_shift; }
+    __device__ __forceinline__ unsigned vhash_home(int id) const {
+        return ((unsigned)id * 2654435769u) >> (QHASH ? qshift : p.vhash_shift);
+    }
     // the query has filled its table to the load limit: it is abandoned (nothing counts as new any more, the search loops
-    // stop) and search_kernel re-runs it on the bitmap.  Never true on the bitmap.
-    __device__ __forceinline__ bool vset_full() const { return HASH && vlog_count >= p.vhash_limit; }
+    // stop) and search_kernel re-runs it on the bitmap.  Never true on the bitmap.  QHASH: the iterator kernels suspend
+    // or restart the query on a larger table (iterate_kernel never reaches the limit inside a step).
+    __device__ __forceinline__ bool vset_full() const {
+        return (HASH && vlog_count >= p.vhash_limit) || (QHASH && vlog_count >= qlimit);
+    }
 
     // OptHashPosVector::CheckAndSet for a warp-uniform id: true if already present.  OUTLINE: the hashed insert is a call
     // (BKT tree seeding; the KD-tree leaves inline it)
@@ -896,10 +943,12 @@ struct WarpSearch {
     __device__ __forceinline__ bool check_and_set_uniform(int id) {
         if (hashed()) {
             if (vset_full()) return true;
-            const bool was = OUTLINE ? vhash_insert_uniform_call(visited, vlog + vlog_count, vhash_home(id), (unsigned)id + 1u,
-                                                                 p.vhash_mask, lane)
-                                     : vhash_insert_uniform(visited, vlog + vlog_count, vhash_home(id), (unsigned)id + 1u,
-                                                            p.vhash_mask, lane);
+            // (the iterators' tables keep no clear log)
+            const bool was = QHASH     ? vhash_insert_uniform<false>(visited, nullptr, vhash_home(id), (unsigned)id + 1u, qmask, lane)
+                             : OUTLINE ? vhash_insert_uniform_call(visited, vlog + vlog_count, vhash_home(id), (unsigned)id + 1u,
+                                                                   p.vhash_mask, lane)
+                                       : vhash_insert_uniform(visited, vlog + vlog_count, vhash_home(id), (unsigned)id + 1u,
+                                                              p.vhash_mask, lane);
             if (!was) vlog_count++;
             return was;
         }
@@ -1274,9 +1323,17 @@ struct WarpSearch {
         }
     }
 
+    // the table is at its limit before a SearchTrees pop (each pop inserts at most one centre): QHASH records the cut, at
+    // which an iterator call suspends
+    __device__ __forceinline__ bool trees_full() {
+        if (!vset_full()) return false;
+        if (QHASH) trees_cut = true;
+        return true;
+    }
+
     // BKTree::SearchTrees (BKTree.h:771-799)
     __device__ __forceinline__ void search_trees(int limit) {
-        while (spt.count != 0 && !vset_full()) {
+        while (spt.count != 0 && !trees_full()) {
             const int2 bcell = hpop(spt);
             const int centerid = p.nodes[3 * bcell.x], cs = p.nodes[3 * bcell.x + 1], ce = p.nodes[3 * bcell.x + 2];
             ntree++;
@@ -1330,7 +1387,7 @@ struct WarpSearch {
         if (!hashed()) return m.leader && (m.old & m.bit) == 0;
         if (!m.leader || m.old == (unsigned)nn + 1u) return false;
         if (m.old == 0u) return true;
-        const unsigned r = vhash_probe(visited, m.bit, (unsigned)nn + 1u, p.vhash_mask);
+        const unsigned r = vhash_probe(visited, m.bit, (unsigned)nn + 1u, vhash_mask());
         m.bit = r & ~kVhashFound;
         return (r & kVhashFound) == 0;
     }
@@ -1544,16 +1601,34 @@ struct WarpSearch {
     // ResultIterator::Next.  Differences from Search: every popped live node is a result (at most `batch` per call),
     // neighbours enter NGQueue unconditionally (m_Results only feeds the relaxed-monotonicity flag), duplicate-group
     // members get their own distance and enter NGQueue, and there is no stop rule besides `count >= batch`.
-    // Results are appended to this query's arena `tk` (sorted afterwards); returns resultCount.
+    // Results are appended to this query's arena `tk` (sorted afterwards); `count` is resultCount.
+    // A query on a hash table (QHASH) suspends where its state can be saved instead of losing an insert: at the top of a
+    // step that could take the fill past the limit (`margin` = degree + largest duplicate group + 1 bounds what one step
+    // inserts), and before a SearchTrees pop at the limit.  `at` enters as where the call starts (kIterFirst, kIterStep) or
+    // resumes, and leaves as kIterDone or the resume point; `limit` is the pending SearchTrees limit.
     // ------------------------------------------------------------------------------------
-    __device__ __forceinline__ int bkt_search_iterative(bool is_first, int batch, int& relaxed) {
-        if (is_first) {
+    __device__ __forceinline__ void bkt_search_iterative(int& at, int batch, int& relaxed, int& count, int& limit,
+                                                         int margin) {
+        if (at == kIterFirst) {
             init_search_trees();
-            search_trees(p.initial_pivots);
+            at = kIterInitTrees;
+            limit = p.initial_pivots;
         }
-        int count = 0;
+        if (at != kIterStep) {  // the first call's trees, or a resumed in-step SearchTrees
+            trees_cut = false;
+            search_trees(limit);
+            if (QHASH && trees_cut) return;
+            if (at == kIterStepTrees && count >= batch) {
+                at = kIterDone;
+                return;
+            }
+        }
         const int checkPos = p.degree - 1;
         while (ng.count != 0) {
+            if (QHASH && vlog_count + margin > qlimit) {
+                at = kIterStep;
+                return;
+            }
             const int2 gnode = hpop(ng);
             const int popped = gnode.x;
             const float gdist = pair_dist(gnode);
@@ -1589,22 +1664,13 @@ struct WarpSearch {
             }
             for (int cbase = 0; cbase <= checkPos; cbase += 32) {
                 if (cbase > 0) nn = (cbase + lane <= checkPos) ? node[cbase + lane] : -1;
-                const bool in_row = (cbase + lane <= checkPos);
-                const unsigned negmask = __ballot_sync(kFull, in_row && nn < 0) | ~__ballot_sync(kFull, in_row);
-                const int first_neg = negmask ? (__ffs(negmask) - 1) : 32;
-                const bool active = lane < first_neg;
-                const unsigned same = __match_any_sync(kFull, active ? nn : (-1 - lane));
-                const bool leader = active && ((__ffs(same) - 1) == lane);
-                bool fresh = false;
-                if (leader) {
-                    const unsigned bit = 1u << (nn & 31);
-                    const unsigned old = atomicOr(&visited[nn >> 5], bit);
-                    fresh = (old & bit) == 0;
-                }
+                RowMark mark = issue_mark(nn, cbase + lane <= checkPos);
+                const bool fresh = mark_fresh(mark, nn);
                 const unsigned freshmask = __ballot_sync(kFull, fresh);
                 const int cnt = __popc(freshmask);
                 __syncwarp();
                 if (fresh) cand_id[__popc(freshmask & ((1u << lane) - 1u))] = nn;
+                vlog_count += cnt;
                 compute_dists(cnt);
                 checked += cnt;
                 for (int r = 0; r < cnt; ++r) {
@@ -1614,12 +1680,20 @@ struct WarpSearch {
                     mres.insert(d, lane);
                 }
                 __syncwarp();
-                if (first_neg < 32) break;
+                if (mark.first_neg < 32) break;
             }
-            if (heap_top_dist(ng) > heap_top_dist(spt)) search_trees(p.other_pivots + checked);
+            if (heap_top_dist(ng) > heap_top_dist(spt)) {
+                limit = p.other_pivots + checked;
+                trees_cut = false;
+                search_trees(limit);
+                if (QHASH && trees_cut) {
+                    at = kIterStepTrees;
+                    return;
+                }
+            }
             if (count >= batch) break;
         }
-        return count;
+        at = kIterDone;
     }
 
     // SearchIndexIterativeFromNeareast, first call (BKTIndex.cpp:549-572): one result of the finished search is marked
@@ -1632,25 +1706,17 @@ struct WarpSearch {
         for (int cbase = 0; cbase <= checkPos; cbase += 32) {
             const bool in_row = (cbase + lane <= checkPos);
             const int nn = in_row ? node[cbase + lane] : -1;
-            const unsigned negmask = __ballot_sync(kFull, in_row && nn < 0) | ~__ballot_sync(kFull, in_row);
-            const int first_neg = negmask ? (__ffs(negmask) - 1) : 32;
-            const bool active = lane < first_neg;
-            const unsigned same = __match_any_sync(kFull, active ? nn : (-1 - lane));
-            const bool leader = active && ((__ffs(same) - 1) == lane);
-            bool fresh = false;
-            if (leader) {
-                const unsigned bit = 1u << (nn & 31);
-                const unsigned old = atomicOr(&visited[nn >> 5], bit);
-                fresh = (old & bit) == 0;
-            }
+            RowMark mark = issue_mark(nn, in_row);
+            const bool fresh = mark_fresh(mark, nn);
             const unsigned freshmask = __ballot_sync(kFull, fresh);
             const int cnt = __popc(freshmask);
             __syncwarp();
             if (fresh) cand_id[__popc(freshmask & ((1u << lane) - 1u))] = nn;
+            vlog_count += cnt;
             compute_dists(cnt);
             for (int r = 0; r < cnt; ++r) hins(ng, cand_id[r], cand_dist[r]);
             __syncwarp();
-            if (first_neg < 32) break;
+            if (mark.first_neg < 32) break;
         }
     }
 
@@ -1988,19 +2054,48 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
 // ResultIterator::Next for a batch of open iterators (ResultIterator.cpp:31-55 -> SearchIndexIterativeNext,
 // BKTIndex.cpp:659-675).  Every query owns persistent arenas in HBM -- visited bitmap, NGQueue, SPTQueue (the
 // reference's rented WorkSpace) -- indexed by query, not by slot; the shared-memory queue heads are restored from and
-// flushed to those arenas around each call.  state[q] = {ng count, spt count, first call, relaxedMono, result slots}.
+// flushed to those arenas around each call.  state[q] = {ng count, spt count, first call, relaxedMono, result slots,
+// log2 of the visited table's entries (0: a bitmap), the visited set's fill, resume point}.
 // p.k = the batch the caller asked for; the effective batch of a query is capped by the result count of its previous
 // call (QueryResult::SetResultNum(resultCount), ResultIterator.cpp:36-41, :52).
+// A query on a hash table that reaches the table's limit suspends (bkt_search_iterative): it saves what the call has
+// built so far, writes no outputs and joins iv.suspended; the host grows its table and launches the kernel again over
+// that list (iv.list), where the query continues from the saved state.  The visited set has exact set semantics in
+// both forms, so the results do not depend on where, or how often, a query was suspended.
 // ------------------------------------------------------------------------------------------
 constexpr int kIterStateInts = 8;
+
+// The per-query visited set of an iterator kernel: its table or bitmap, and the table's capacity
+template <typename W>
+__device__ __forceinline__ void bind_iter_visited(W& w, const SearchParams& p, const IterVisited& iv, int q, int bits) {
+    w.visited = iv.tables ? iv.tables[q] : p.visited + (size_t)q * p.visited_words;
+    w.qmask = bits ? (1u << bits) - 1u : 0u;
+    w.qshift = 32 - bits;
+    w.qlimit = bits ? 1 << (bits - 1) : INT_MAX;
+}
+// The next query of an iterator launch: every query, or those on the resume list; -1 when none is left
+__device__ __forceinline__ int next_iter_query(const SearchParams& p, const IterVisited& iv, int lane) {
+    unsigned i = 0;
+    if (lane == 0) i = atomicAdd(p.work_counter, 1u);
+    i = __shfl_sync(kFull, i, 0);
+    if (iv.list) return i < iv.list[0] ? (int)iv.list[kIterListHeader + i] : -1;
+    return i < (unsigned)p.nq ? (int)i : -1;
+}
+// Append q to the suspension list; `kind` (1 or 2) counts it as a step or a tree suspension, 0 not at all
+__device__ __forceinline__ void suspend_iter_query(const IterVisited& iv, int q, int kind, int lane) {
+    if (lane == 0) {
+        iv.suspended[kIterListHeader + atomicAdd(iv.suspended, 1u)] = (unsigned)q;
+        if (kind) atomicAdd(iv.suspended + kind, 1u);
+    }
+}
 
 template <bool COSINE, int RPL, int ELEM>
 __global__ void __launch_bounds__(32, 12) iterate_kernel(const SearchParams p, int* __restrict__ state,
                                                          int* __restrict__ out_counts,
-                                                         unsigned char* __restrict__ out_relaxed) {
+                                                         unsigned char* __restrict__ out_relaxed, const IterVisited iv) {
     extern __shared__ __align__(128) unsigned char smem[];
     const int lane = threadIdx.x;
-    WarpSearch<0, COSINE, RPL, false, ELEM> w(p, lane);
+    WarpSearch<0, COSINE, RPL, false, ELEM, false, true> w(p, lane);
     w.ring = smem;
     w.cand_id = reinterpret_cast<int*>(smem + p.off_cand);
     w.cand_dist = reinterpret_cast<float*>(smem + p.off_cand + 128);
@@ -2025,31 +2120,41 @@ __global__ void __launch_bounds__(32, 12) iterate_kernel(const SearchParams p, i
     __syncwarp();
 
     for (;;) {
-        int q = 0;
-        if (lane == 0) q = (int)atomicAdd(p.work_counter, 1u);
-        q = __shfl_sync(kFull, q, 0);
-        if (q >= p.nq) break;
+        const int q = next_iter_query(p, iv, lane);
+        if (q < 0) break;
         int* st = state + (size_t)q * kIterStateInts;
-        w.visited = p.visited + (size_t)q * p.visited_words;
+        bind_iter_visited(w, p, iv, q, st[5]);
         w.ng.g = p.ng_spill + (size_t)q * p.ng_spill_entries;
         w.spt.g = p.spt_spill + (size_t)q * p.spt_spill_entries;
         w.tk = p.topk + (size_t)q * p.topk_pad;
         w.ng.count = st[0];
         w.spt.count = st[1];
         w.ng.tail_idx = w.spt.tail_idx = -1;
-        const bool is_first = st[2] != 0;
+        const int resumed = st[7];
+        int at = resumed ? resumed : (st[2] != 0 ? kIterFirst : kIterStep);
         int relaxed = st[3];
         const int slots = st[4];
         const int batch = (slots < 0) ? p.k : min(p.k, slots);
         // queue heads back into shared memory
         for (int i = 1 + lane; i <= min(w.ng.count, w.ng.H); i += 32) w.ng.s[i] = w.ng.g[i];
         for (int i = 1 + lane; i <= min(w.spt.count, w.spt.H); i += 32) w.spt.s[i] = w.spt.g[i];
-        // WorkSpace::ResetResult(m_iMaxCheck, batch) (WorkSpace.h:280-286)
-        w.mres.reset(max(p.max_check / 16, batch), lane);
-        w.checked = w.ndist = w.nexpand = w.ntree = 0;
+        w.ndist = w.nexpand = w.ntree = 0;
         w.tree_checked = w.no_better = 0;
-        w.vlog_count = 0;
-        w.tk_count = 0;
+        w.vlog_count = st[6];
+        float* saved = iv.resume ? iv.resume + (size_t)q * kIterResumeWords : nullptr;
+        int count = 0, limit = 0;
+        if (resumed) {  // the call this query suspended in: m_Results, resultCount, checked and the SearchTrees limit
+            w.mres.load(saved, lane);
+            const int* si = reinterpret_cast<const int*>(saved + 32 * RPL);
+            count = si[0];
+            w.checked = si[1];
+            limit = si[2];
+        } else {
+            // WorkSpace::ResetResult(m_iMaxCheck, batch) (WorkSpace.h:280-286)
+            w.mres.reset(max(p.max_check / 16, batch), lane);
+            w.checked = 0;
+        }
+        w.tk_count = count;
         {   // the query (element type of the index) -> shared memory
             const unsigned char* qb = p.queries + (size_t)q * p.query_stride_bytes;
             unsigned char* qd = reinterpret_cast<unsigned char*>(w.qs);
@@ -2058,10 +2163,31 @@ __global__ void __launch_bounds__(32, 12) iterate_kernel(const SearchParams p, i
         }
         __syncwarp();
 
-        const int count = w.bkt_search_iterative(is_first, batch, relaxed);
+        w.bkt_search_iterative(at, batch, relaxed, count, limit, iv.margin);
 
-        // QueryResultSet::SortResult over the `count` returned entries; the rest of the caller's row is (-1, MaxDist)
         __syncwarp();
+        if (at != kIterDone) {  // suspended: keep the call's state, flush the queues, no outputs yet
+            w.mres.save(saved, lane);
+            if (lane == 0) {
+                int* si = reinterpret_cast<int*>(saved + 32 * RPL);
+                si[0] = count;
+                si[1] = w.checked;
+                si[2] = limit;
+            }
+            for (int i = 1 + lane; i <= min(w.ng.count, w.ng.H); i += 32) w.ng.g[i] = w.ng.s[i];
+            for (int i = 1 + lane; i <= min(w.spt.count, w.spt.H); i += 32) w.spt.g[i] = w.spt.s[i];
+            if (lane == 0) {
+                st[0] = w.ng.count;
+                st[1] = w.spt.count;
+                st[3] = relaxed;
+                st[6] = w.vlog_count;
+                st[7] = at;
+            }
+            suspend_iter_query(iv, q, at == kIterStep ? 1 : 2, lane);
+            __syncwarp();
+            continue;
+        }
+        // QueryResultSet::SortResult over the `count` returned entries; the rest of the caller's row is (-1, MaxDist)
         w.res_sort();
         for (int i = lane; i < p.k; i += 32) {
             const int2 e = (i < count) ? w.tk[i] : make_pair(-1, SPTAG_B200_MAXDIST);
@@ -2077,6 +2203,8 @@ __global__ void __launch_bounds__(32, 12) iterate_kernel(const SearchParams p, i
             st[2] = 0;
             st[3] = relaxed;
             st[4] = count;  // m_queryResult->SetResultNum(resultCount)
+            st[6] = w.vlog_count;
+            st[7] = 0;
             out_counts[q] = count;
             out_relaxed[q] = (unsigned char)relaxed;
         }
@@ -2090,12 +2218,16 @@ __global__ void __launch_bounds__(32, 12) iterate_kernel(const SearchParams p, i
 // the query's own work-space arenas, nodeCheckStatus.clear(), then every result re-seeds NGQueue from its graph row.
 // Later calls are iterate_kernel with batch = k (the host resets the result-slot cap: the caller's QueryResult keeps
 // its size there).
+// The search is not resumable mid-way: a query whose table reaches its limit joins iv.suspended and the host runs its
+// call again from the start on a larger, empty table (exact: the iterator was freshly opened).  The host sizes the
+// tables so that the seeding (at most k x (degree + 1) inserts) stays below the limit.
 // ------------------------------------------------------------------------------------------
 template <bool COSINE, int RPL, int ELEM>
-__global__ void __launch_bounds__(32, 12) nearest_first_kernel(const SearchParams p, int* __restrict__ state) {
+__global__ void __launch_bounds__(32, 12) nearest_first_kernel(const SearchParams p, int* __restrict__ state,
+                                                               const IterVisited iv) {
     extern __shared__ __align__(128) unsigned char smem[];
     const int lane = threadIdx.x;
-    WarpSearch<0, COSINE, RPL, false, ELEM> w(p, lane);
+    WarpSearch<0, COSINE, RPL, false, ELEM, false, true> w(p, lane);
     w.ring = smem;
     w.cand_id = reinterpret_cast<int*>(smem + p.off_cand);
     w.cand_dist = reinterpret_cast<float*>(smem + p.off_cand + 128);
@@ -2120,12 +2252,10 @@ __global__ void __launch_bounds__(32, 12) nearest_first_kernel(const SearchParam
     __syncwarp();
 
     for (;;) {
-        int q = 0;
-        if (lane == 0) q = (int)atomicAdd(p.work_counter, 1u);
-        q = __shfl_sync(kFull, q, 0);
-        if (q >= p.nq) break;
+        const int q = next_iter_query(p, iv, lane);
+        if (q < 0) break;
         int* st = state + (size_t)q * kIterStateInts;
-        w.visited = p.visited + (size_t)q * p.visited_words;  // zeroed when the iterator was opened
+        bind_iter_visited(w, p, iv, q, st[5]);  // empty: zeroed when the iterator was opened or the table was grown
         w.ng.g = p.ng_spill + (size_t)q * p.ng_spill_entries;
         w.spt.g = p.spt_spill + (size_t)q * p.spt_spill_entries;
         w.tk = (p.k > 32) ? p.topk + (size_t)q * p.topk_pad : nullptr;
@@ -2153,13 +2283,19 @@ __global__ void __launch_bounds__(32, 12) nearest_first_kernel(const SearchParam
         w.bkt_search();  // SearchIndex(query, workspace, p_searchDeleted, searchDuplicated = true)
 
         __syncwarp();
+        if (w.vset_full()) {  // the table filled: run the whole call again on a larger one
+            suspend_iter_query(iv, q, 0, lane);
+            __syncwarp();
+            continue;
+        }
         if (w.tk != nullptr) w.res_sort();
         // p_space->nodeCheckStatus.clear(): other nodes may be traversed again after the top k were found
         {
             uint4* v4 = reinterpret_cast<uint4*>(w.visited);
-            const size_t n4 = p.visited_words >> 2;
+            const size_t n4 = w.qmask ? (w.qmask + 1u) >> 2 : p.visited_words >> 2;
             for (size_t i = lane; i < n4; i += 32) v4[i] = make_uint4(0, 0, 0, 0);
         }
+        w.vlog_count = 0;
         __syncwarp();
         for (int i = 0; i < p.k; ++i) {
             int rid;
@@ -2188,6 +2324,7 @@ __global__ void __launch_bounds__(32, 12) nearest_first_kernel(const SearchParam
             st[1] = w.spt.count;
             st[2] = 0;
             st[4] = -1;
+            st[6] = w.vlog_count;
         }
         __syncwarp();
     }

@@ -135,6 +135,12 @@ struct sptag_b200_index {
     int visited_set = -1;
     int visited_hash_entries = 0;  // table entries per slot, 0 = 2^(bits(max(MaxCheck, MaxCheckForRefineGraph)) + 2)
     std::atomic<int> last_visited_overflows{0};  // queries the hashed set handed to the re-run, last blocking search
+    // iterators: -1 auto (the bitmaps unless their allocation fails), 0 bitmap, 1 a growing hash table per query
+    int iter_visited_set = -1;
+    int iter_hash_entries = 0;  // initial table entries per query, 0 = 2^(bits(max(MaxCheck, MaxCheckForRefineGraph)) + 2)
+    int max_dup = -1;           // largest duplicate group of the tree (the tree never changes); -1 = not computed yet
+    // the last iterator call: suspensions at a step top / before a SearchTrees pop, tables grown, visited-set bytes held
+    long last_iter_susp_step = 0, last_iter_susp_trees = 0, last_iter_growths = 0, last_iter_visited_bytes = 0;
     // PQ / OPQ quantizer (null when q_type == 0)
     int q_type = 0, q_rtype = SPTAG_B200_VT_FLOAT, q_m = 0, q_ks = 0, q_dsub = 0;
     int q_adc = 0;  // IQuantizer::SetEnableADC (not serialized by the reference either)
@@ -197,6 +203,21 @@ struct sptag_b200_iterator {
     int nearest_k = 0;       // > 0 once sptag_b200_iterator_next_from_nearest ran: the head QueryResult's size
     bool stepped = false;    // a Next of either kind has run
     DeviceBuffer d_queries, d_visited, d_ng, d_spt, d_state, d_topk, d_ids, d_dists, d_counts, d_relaxed;
+    // Hashed visited sets (B200.IteratorVisitedSet): each query's set is a table of 2^bits entries, or a bitmap (bits 0)
+    // once a table would outgrow one.  The sets live in vbufs: one buffer at open, one per growth round; a buffer is
+    // freed when no query's set lives in it any more.
+    bool hashed = false;
+    int margin = 0;  // degree + largest duplicate group + 1 (IterVisited::margin)
+    std::vector<int> q_bits, q_buf;
+    std::vector<unsigned int*> q_set;
+    std::vector<DeviceBuffer> vbufs;
+    std::vector<int> vbuf_refs;
+    DeviceBuffer d_tables, d_resume, d_susp[2], d_jobs;
+    size_t visited_bytes() const {
+        size_t b = d_visited.bytes;
+        for (const DeviceBuffer& v : vbufs) b += v.bytes;
+        return b;
+    }
 };
 
 namespace {
@@ -680,13 +701,60 @@ int plan_iterator_step(const sptag_b200_iterator* it, int k, SearchLaunch& L) {
     return plan_search(it->h, k, it->nq, iopts, L);
 }
 
+// Move the visited sets of queries qs[i] to one new, zeroed buffer: tables of 2^bits[i] entries, or bitmaps where such a
+// table would be larger than the query's bitmap.  keep: the ids are carried over; otherwise the sets start empty (the
+// query's call runs again from the start).  Blocks until the move is done.  Caller holds h->mu.
+int grow_iter_visited(sptag_b200_iterator* it, const std::vector<unsigned>& qs, const std::vector<int>& bits, bool keep,
+                      cudaStream_t stream) {
+    std::vector<IterGrowJob> jobs(qs.size());
+    size_t words = 0;
+    for (size_t i = 0; i < qs.size(); ++i) {
+        int b = bits[i];
+        if (b && ((size_t)1 << b) > it->visited_words) b = 0;  // converts to a bitmap and stays one
+        jobs[i].new_bits = b;
+        jobs[i].new_set = (unsigned int*)(words * 4);  // offset until the buffer exists
+        words += b ? ((size_t)1 << b) : it->visited_words;
+    }
+    DeviceBuffer buf;
+    if (int rc = buf.ensure(words * 4)) return rc;
+    CUDA_OK(cudaMemsetAsync(buf.ptr, 0, buf.bytes, stream));
+    for (size_t i = 0; i < qs.size(); ++i) {
+        const unsigned q = qs[i];
+        jobs[i].new_set = (unsigned int*)((char*)buf.ptr + (size_t)jobs[i].new_set);
+        jobs[i].old_set = it->q_set[q];
+        jobs[i].q = (int)q;
+        jobs[i].old_bits = it->q_bits[q];
+        jobs[i].keep = keep ? 1 : 0;
+    }
+    if (int rc = it->d_jobs.ensure(jobs.size() * sizeof(IterGrowJob))) return rc;
+    CUDA_OK(cudaMemcpyAsync(it->d_jobs.ptr, jobs.data(), jobs.size() * sizeof(IterGrowJob), cudaMemcpyHostToDevice, stream));
+    iter_grow_kernel<<<(unsigned)jobs.size(), 32, 0, stream>>>((const IterGrowJob*)it->d_jobs.ptr,
+                                                               (unsigned int**)it->d_tables.ptr, (int*)it->d_state.ptr);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    CUDA_OK(cudaStreamSynchronize(stream));
+    const int nb = (int)it->vbufs.size();
+    for (size_t i = 0; i < qs.size(); ++i) {
+        const unsigned q = qs[i];
+        if (--it->vbuf_refs[it->q_buf[q]] == 0) it->vbufs[it->q_buf[q]].release();
+        it->q_buf[q] = nb;
+        it->q_bits[q] = jobs[i].new_bits;
+        it->q_set[q] = jobs[i].new_set;
+    }
+    it->vbufs.push_back(std::move(buf));
+    it->vbuf_refs.push_back((int)qs.size());
+    return 0;
+}
+
 // Run one iterator step planned by plan_iterator_step.  The iterator's queue lengths and per-query arenas replace the
 // per-slot scratch of a search; of scratch set 0 only the work counter is used, with the same ordering as a search.
-// The grid stays the search kernel's.  launch(p, grid, smem, stream) enqueues the iterate or nearest-first kernel;
-// `what` names k in the refusal.  Caller holds h->mu.
+// The grid stays the search kernel's.  launch(p, grid, smem, stream, iv) enqueues the iterate or nearest-first kernel;
+// `what` names k in the refusal.  On hashed visited sets the kernel leaves the queries that reached their table's limit
+// on a list: their tables grow (restart: they are replaced by empty ones) and the kernel runs again over that list,
+// until the list is empty.  Caller holds h->mu.
 template <typename LaunchFn>
 int run_iterator_step(sptag_b200_iterator* it, int k, const char* what, SearchLaunch& L, int32_t* out_ids,
-                      float* out_dists, int32_t* out_counts, uint8_t* out_relaxed_mono, LaunchFn&& launch) {
+                      float* out_dists, int32_t* out_counts, uint8_t* out_relaxed_mono, bool restart, LaunchFn&& launch) {
     sptag_b200_index* h = it->h;
     if (it->topk_pad == 0) {  // the first Next creates the QueryResult: its size bounds every later batch
         it->topk_pad = topk_pad_for(k);
@@ -726,12 +794,46 @@ int run_iterator_step(sptag_b200_iterator* it, int k, const char* what, SearchLa
     p.work_counter = (unsigned int*)h->scratch[0].d_counter.ptr;
     if (smem > h->smem_optin) return fail(SPTAG_B200_MEMORY_OVERFLOW, "shared memory per query slot %zu exceeds %zu", smem, h->smem_optin);
     cudaStream_t stream = nullptr;
+    IterVisited iv = {};
+    iv.margin = it->margin;
+    if (it->hashed) {
+        iv.tables = (unsigned int* const*)it->d_tables.ptr;
+        iv.resume = (float*)it->d_resume.ptr;
+        iv.suspended = (unsigned int*)it->d_susp[0].ptr;
+    }
     if (int rc = scratch_acquire(h, stream)) return rc;
     CUDA_OK(cudaMemsetAsync(p.work_counter, 0, 4, stream));
+    if (it->hashed) CUDA_OK(cudaMemsetAsync(iv.suspended, 0, kIterListHeader * 4, stream));
     CUDA_OK(cudaEventRecord(h->ev_start, stream));
-    if (int rc = launch(p, L.grid, smem, stream)) return rc;
+    if (int rc = launch(p, L.grid, smem, stream, iv)) return rc;
     g_launches++;
     CUDA_OK(cudaGetLastError());
+    long susp_step = 0, susp_trees = 0, growths = 0;
+    for (int cur = 0; it->hashed; cur ^= 1) {  // at most ~log2(n) rounds: every round doubles the listed tables
+        unsigned hdr[kIterListHeader];
+        CUDA_OK(cudaMemcpyAsync(hdr, it->d_susp[cur].ptr, sizeof(hdr), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        susp_step += hdr[1];
+        susp_trees += hdr[2];
+        if (hdr[0] == 0) break;
+        std::vector<unsigned> qs(hdr[0]);
+        CUDA_OK(cudaMemcpy(qs.data(), (unsigned*)it->d_susp[cur].ptr + kIterListHeader, qs.size() * 4, cudaMemcpyDeviceToHost));
+        std::vector<int> bits(qs.size());
+        for (size_t i = 0; i < qs.size(); ++i) bits[i] = it->q_bits[qs[i]] + 1;
+        if (int rc = grow_iter_visited(it, qs, bits, !restart, stream)) return rc;
+        growths += (long)qs.size();
+        iv.list = (const unsigned int*)it->d_susp[cur].ptr;
+        iv.suspended = (unsigned int*)it->d_susp[cur ^ 1].ptr;
+        CUDA_OK(cudaMemsetAsync(p.work_counter, 0, 4, stream));
+        CUDA_OK(cudaMemsetAsync(iv.suspended, 0, kIterListHeader * 4, stream));
+        if (int rc = launch(p, std::min(L.grid, (int)qs.size()), smem, stream, iv)) return rc;
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+    }
+    h->last_iter_susp_step = susp_step;
+    h->last_iter_susp_trees = susp_trees;
+    h->last_iter_growths = growths;
+    h->last_iter_visited_bytes = (long)it->visited_bytes();
     CUDA_OK(cudaEventRecord(h->ev_stop, stream));
     h->timed = true;
     if (int rc = scratch_release(h, stream)) return rc;
@@ -1301,6 +1403,14 @@ int sptag_b200_set_param(sptag_b200_handle h, const char* name, const char* valu
         if (v != 0 && (v < 64 || v > (1l << 30) || (v & (v - 1)) != 0))
             return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.VisitedHashEntries %ld: 0 (default) or a power of two in [64, 2^30]", v);
         h->visited_hash_entries = (int)v;
+    } else if (n == "B200.IteratorVisitedSet") {  // taken by iterators opened afterwards
+        if (v < -1 || v > 1)
+            return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.IteratorVisitedSet %ld: -1 (auto), 0 (bitmap) or 1 (hashed)", v);
+        h->iter_visited_set = (int)v;
+    } else if (n == "B200.IteratorVisitedHashEntries") {
+        if (v != 0 && (v < 64 || v > (1l << 30) || (v & (v - 1)) != 0))
+            return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.IteratorVisitedHashEntries %ld: 0 (default) or a power of two in [64, 2^30]", v);
+        h->iter_hash_entries = (int)v;
     }
     else if (n == "B200.SlotScheme") h->slot_scheme = (int)v;
     else if (n == "EnableADC") h->q_adc = (v != 0);  // VectorIndex::SetQuantizerADC (VectorIndex.h:136-138)
@@ -1315,6 +1425,10 @@ int sptag_b200_get_param(sptag_b200_handle h, const char* name, char* value_out,
     long v;
     if (n == "RNGFactor") {  // float, printed like the reference's ini (ConvertToString)
         snprintf(value_out, (size_t)capacity, "%f", h->rng_factor);
+        return SPTAG_B200_SUCCESS;
+    }
+    if (n == "B200.LastIteratorSuspensions") {  // read-only: "step,trees" of the last iterator call
+        snprintf(value_out, (size_t)capacity, "%ld,%ld", h->last_iter_susp_step, h->last_iter_susp_trees);
         return SPTAG_B200_SUCCESS;
     }
     if (n == "MaxCheck") v = h->max_check;
@@ -1337,6 +1451,10 @@ int sptag_b200_get_param(sptag_b200_handle h, const char* name, char* value_out,
     else if (n == "B200.VisitedHashEntries") v = h->visited_hash_entries;
     else if (n == "B200.LastVisitedOverflows") v = h->last_visited_overflows;       // read-only
     else if (n == "B200.ScratchBytes") v = (long)(h->scratch[0].bytes() + h->scratch[1].bytes());  // read-only
+    else if (n == "B200.IteratorVisitedSet") v = h->iter_visited_set;
+    else if (n == "B200.IteratorVisitedHashEntries") v = h->iter_hash_entries;
+    else if (n == "B200.LastIteratorGrowths") v = h->last_iter_growths;                // read-only
+    else if (n == "B200.LastIteratorVisitedBytes") v = h->last_iter_visited_bytes;     // read-only
     else if (n == "B200.SlotScheme") v = h->slot_scheme;
     else if (n == "EnableADC") v = h->q_adc;
     else if (n == "B200.LastRefineSearchUs") v = (long)(h->refine_search_ms * 1000.0);    // read-only: device time
@@ -1668,21 +1786,75 @@ int sptag_b200_iterator_open_ex(sptag_b200_handle h, const void* queries, int32_
     it->spt_entries = p.spt_spill_entries;
     const size_t qbytes = (size_t)num_queries * query_bytes(h);
     int rc = 0;
-    if ((rc = it->d_queries.ensure(qbytes)) || (rc = it->d_visited.ensure((size_t)num_queries * it->visited_words * 4)) ||
-        (rc = it->d_ng.ensure((size_t)num_queries * it->ng_entries * 8)) ||
+    if ((rc = it->d_queries.ensure(qbytes)) || (rc = it->d_ng.ensure((size_t)num_queries * it->ng_entries * 8)) ||
         (rc = it->d_spt.ensure((size_t)num_queries * it->spt_entries * 8)) ||
         (rc = it->d_state.ensure((size_t)num_queries * kIterStateInts * 4)) ||
         (rc = it->d_counts.ensure((size_t)num_queries * 4)) || (rc = it->d_relaxed.ensure((size_t)num_queries))) {
         delete it;
         return rc;
     }
+    // The visited sets: a bitmap per query, or (B200.IteratorVisitedSet = 1, or auto when the bitmaps do not fit) a
+    // hash table per query that grows while the iterator runs
+    it->hashed = h->iter_visited_set == 1;
+    if (!it->hashed && (rc = it->d_visited.ensure((size_t)num_queries * it->visited_words * 4))) {
+        if (h->iter_visited_set == 0 || cudaGetLastError() != cudaErrorMemoryAllocation) {
+            delete it;
+            return rc;
+        }
+        it->hashed = true;  // auto: the bitmaps do not fit (the failed cudaMalloc's error is cleared above)
+    }
+    int bits = 0;
+    if (it->hashed) {
+        if (h->max_dup < 0) {  // computed once per handle: the tree does not change
+            int* d_max = (int*)h->scratch[0].d_counter.ptr + 16;
+            int m = 0;
+            cudaError_t e = cudaMemset(d_max, 0, 4);
+            max_dup_group_kernel<<<(h->node_count + 255) / 256, 256>>>((const int*)h->d_nodes.ptr, h->node_count, d_max);
+            g_launches++;
+            if (e == cudaSuccess) e = cudaMemcpy(&m, d_max, 4, cudaMemcpyDeviceToHost);
+            if (e != cudaSuccess) {
+                delete it;
+                return fail(SPTAG_B200_FAIL, "iterator set-up failed: %s", cudaGetErrorString(e));
+            }
+            h->max_dup = m;
+        }
+        it->margin = h->degree + h->max_dup + 1;
+        // initial entries: B200.IteratorVisitedHashEntries, or the reference's first-block size as for search; raised
+        // until one step fits below the limit, so that doubling a table always makes room for the step that suspended
+        if (h->iter_hash_entries > 0) {
+            while ((1 << bits) < h->iter_hash_entries) ++bits;
+        } else {
+            for (unsigned s = (unsigned)std::max(std::max(h->max_check, h->max_check_refine), 1); s != 0; s >>= 1) ++bits;
+            bits = std::min(std::max(bits + 2, 6), 30);
+        }
+        while (bits < 30 && (1 << (bits - 1)) < it->margin) ++bits;
+        const size_t entries = (size_t)1 << bits;
+        it->vbufs.emplace_back();
+        it->vbuf_refs.push_back(num_queries);
+        if ((rc = it->vbufs[0].ensure((size_t)num_queries * entries * 4)) ||
+            (rc = it->d_tables.ensure((size_t)num_queries * sizeof(unsigned int*))) ||
+            (rc = it->d_resume.ensure((size_t)num_queries * kIterResumeWords * 4)) ||
+            (rc = it->d_susp[0].ensure((size_t)(kIterListHeader + num_queries) * 4)) ||
+            (rc = it->d_susp[1].ensure((size_t)(kIterListHeader + num_queries) * 4))) {
+            delete it;
+            return rc;
+        }
+        it->q_bits.assign(num_queries, bits);
+        it->q_buf.assign(num_queries, 0);
+        it->q_set.resize(num_queries);
+        for (int q = 0; q < num_queries; ++q) it->q_set[q] = (unsigned int*)it->vbufs[0].ptr + (size_t)q * entries;
+    }
     std::vector<int> st((size_t)num_queries * kIterStateInts, 0);
     for (int q = 0; q < num_queries; ++q) {
         st[(size_t)q * kIterStateInts + 2] = 1;   // first call: InitSearchTrees + SearchTrees
         st[(size_t)q * kIterStateInts + 4] = -1;  // no QueryResult yet: the first Next sets the slot count
+        st[(size_t)q * kIterStateInts + 5] = bits;
     }
     cudaError_t e = cudaMemcpy(it->d_queries.ptr, queries, qbytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemset(it->d_visited.ptr, 0, it->d_visited.bytes);
+    if (e == cudaSuccess && !it->hashed) e = cudaMemset(it->d_visited.ptr, 0, it->d_visited.bytes);
+    if (e == cudaSuccess && it->hashed) e = cudaMemset(it->vbufs[0].ptr, 0, it->vbufs[0].bytes);
+    if (e == cudaSuccess && it->hashed)
+        e = cudaMemcpy(it->d_tables.ptr, it->q_set.data(), (size_t)num_queries * sizeof(unsigned int*), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(it->d_state.ptr, st.data(), st.size() * 4, cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
         delete it;
@@ -1705,11 +1877,11 @@ int sptag_b200_iterator_next(sptag_b200_iter it, int32_t batch, int32_t* out_ids
     if (int rc = plan_iterator_step(it, batch, L)) return rc;
     IterateKernelFn kern = pick_iterate_kernel_for(h->value_type, h->metric != SPTAG_B200_METRIC_L2, L.p.mres_cap);
     if (!kern) return fail(SPTAG_B200_LACK_OF_INPUTS, "max(MaxCheck/16, batch) = %d exceeds the supported 1024", L.p.mres_cap);
-    return run_iterator_step(it, batch, "batch", L, out_ids, out_dists, out_counts, out_relaxed_mono,
-                             [&](const SearchParams& p, int grid, size_t smem, cudaStream_t stream) {
+    return run_iterator_step(it, batch, "batch", L, out_ids, out_dists, out_counts, out_relaxed_mono, false,
+                             [&](const SearchParams& p, int grid, size_t smem, cudaStream_t stream, const IterVisited& iv) {
                                  CUDA_OK(cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                                  kern<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, (int*)it->d_counts.ptr,
-                                                                  (unsigned char*)it->d_relaxed.ptr);
+                                                                  (unsigned char*)it->d_relaxed.ptr, iv);
                                  return 0;
                              });
 }
@@ -1734,16 +1906,34 @@ int sptag_b200_iterator_next_from_nearest(sptag_b200_iter it, int32_t k, int32_t
     IterateKernelFn knext = pick_iterate_kernel_for(h->value_type, cosine, L.p.mres_cap);
     if (!kfirst || !knext)
         return fail(SPTAG_B200_LACK_OF_INPUTS, "max(MaxCheck/16, k) = %d exceeds the supported 1024", L.p.mres_cap);
+    if (first && it->hashed) {
+        // the seeding from the k results inserts at most k x (degree + 1) ids after nodeCheckStatus.clear(): every table
+        // holds that below its limit (the tables are still empty)
+        int need = 6;
+        while (((size_t)1 << (need - 1)) < (size_t)k * (h->degree + 1)) ++need;
+        std::vector<unsigned> qs;
+        std::vector<int> bits;
+        for (int q = 0; q < it->nq; ++q)
+            if (it->q_bits[q] != 0 && it->q_bits[q] < need) {
+                qs.push_back((unsigned)q);
+                bits.push_back(need);
+            }
+        if (!qs.empty())
+            if (int rc = grow_iter_visited(it, qs, bits, false, nullptr)) return rc;
+    }
     const int rc = run_iterator_step(
-        it, k, "k", L, out_ids, out_dists, nullptr, nullptr, [&](const SearchParams& p, int grid, size_t smem, cudaStream_t stream) {
+        it, k, "k", L, out_ids, out_dists, nullptr, nullptr, first,
+        [&](const SearchParams& p, int grid, size_t smem, cudaStream_t stream, const IterVisited& iv) {
             if (first) {
                 CUDA_OK(cudaFuncSetAttribute((const void*)kfirst, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                kfirst<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr);
+                kfirst<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, iv);
             } else {
-                // the caller Reset()s a QueryResult that keeps its k slots (SPANNIndex.cpp:284): no cap from the previous count
-                CUDA_OK(cudaMemset2DAsync((int*)it->d_state.ptr + 4, (size_t)kIterStateInts * 4, 0xFF, 4, (size_t)it->nq, stream));
+                // the caller Reset()s a QueryResult that keeps its k slots (SPANNIndex.cpp:284): no cap from the previous
+                // count (once per call: a resume launch must not undo what its completed queries set)
+                if (!iv.list)
+                    CUDA_OK(cudaMemset2DAsync((int*)it->d_state.ptr + 4, (size_t)kIterStateInts * 4, 0xFF, 4, (size_t)it->nq, stream));
                 CUDA_OK(cudaFuncSetAttribute((const void*)knext, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                knext<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, (int*)it->d_counts.ptr, (unsigned char*)it->d_relaxed.ptr);
+                knext<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, (int*)it->d_counts.ptr, (unsigned char*)it->d_relaxed.ptr, iv);
             }
             return 0;
         });
