@@ -595,9 +595,8 @@ struct IterGrowJob {
     int q, old_bits, new_bits;
     int keep;  // carry the ids over; 0: the query's call runs again from the start
 };
-// One warp per job: the keys (id + 1) of the old table into the new table (linear probing from the same multiplicative
-// hash as the kernels; the keys are distinct, so each lane only looks for an empty position) or into the new bitmap; then
-// the query's set pointer and capacity switch over
+// One warp per job: the keys of the old table into the new table (vhash_home's format; the keys are distinct, so each lane
+// only looks for an empty position) or into the new bitmap; then the query's set pointer and capacity switch over
 __global__ void iter_grow_kernel(const IterGrowJob* __restrict__ jobs, unsigned int** tables, int* __restrict__ state) {
     const IterGrowJob j = jobs[blockIdx.x];
     const int lane = threadIdx.x;
@@ -608,7 +607,7 @@ __global__ void iter_grow_kernel(const IterGrowJob* __restrict__ jobs, unsigned 
             const unsigned key = j.old_set[i];
             if (key == 0u) continue;
             if (j.new_bits) {
-                unsigned pos = ((key - 1u) * 2654435769u) >> (32 - j.new_bits);
+                unsigned pos = vhash_home(key - 1u, 32 - j.new_bits);
                 while (atomicCAS(&j.new_set[pos], 0u, key) != 0u) pos = (pos + 1u) & mask;
             } else {
                 atomicOr(&j.new_set[(key - 1u) >> 5], 1u << ((key - 1u) & 31));
@@ -617,7 +616,7 @@ __global__ void iter_grow_kernel(const IterGrowJob* __restrict__ jobs, unsigned 
     }
     if (lane == 0) {
         tables[j.q] = j.new_set;
-        state[(size_t)j.q * kIterStateInts + 5] = j.new_bits;
+        reinterpret_cast<IterState*>(state)[j.q].vbits = j.new_bits;
     }
 }
 

@@ -38,8 +38,19 @@ namespace sptag_b200 {
 constexpr unsigned kFull = 0xffffffffu;
 constexpr int kStatsPerQuery = 8;
 
-// Where an iterator call starts or resumes (state word 7 of a suspended query holds the resume point; 0: none)
+// Where an iterator call starts or resumes (IterState::resume of a suspended query; 0: none)
 constexpr int kIterDone = 0, kIterStep = 1, kIterInitTrees = 2, kIterStepTrees = 3, kIterFirst = 4;
+// What an open iterator keeps per query between calls (the kernels take it as `int* state`, 8 ints per query)
+struct IterState {
+    int ng_count, spt_count;  // NGQueue / SPTQueue sizes (the entries are in the query's HBM arenas)
+    int first;                // 1: the next call is the first (InitSearchTrees + SearchTrees)
+    int relaxed;              // relaxedMono
+    int slots;                // result slots of the caller's QueryResult, which cap the next batch; -1: none yet
+    int vbits;                // log2 of the visited table's entries; 0: the visited set is a bitmap
+    int vfill;                // ids in the visited set
+    int resume;               // where a suspended call resumes (kIterStep, ...); 0: not suspended
+};
+static_assert(sizeof(IterState) == 32, "IterState is 8 ints");
 // Per-query HBM area of a suspended iterator call: the m_Results multiset (32 x RPL <= 1024 floats), then resultCount,
 // the checked count and the pending SearchTrees limit
 constexpr int kIterResumeWords = 32 * 32 + 4;
@@ -48,7 +59,7 @@ constexpr int kIterListHeader = 4;
 
 // The iterator kernels' visited sets (the per-launch part; the per-query part is in the iterator state)
 struct IterVisited {
-    unsigned int* const* tables;  // per query: its hash table, or its bitmap (state word 5 = 0); nullptr: p.visited bitmaps
+    unsigned int* const* tables;  // per query: its hash table, or its bitmap (IterState::vbits = 0); nullptr: p.visited bitmaps
     float* resume;                // per query kIterResumeWords
     unsigned int* suspended;      // the queries that stopped at their table's limit (kIterListHeader + nq words)
     const unsigned int* list;     // resume launch: run only the queries listed here (same layout); nullptr = all nq
@@ -91,11 +102,11 @@ struct SearchParams {
     // large N: instead of clearing the whole bitmap per query, log the words that were set and clear only those
     unsigned int* vlog;                    // per slot, vlog_entries words; nullptr = clear the bitmap per query
     unsigned long long vlog_entries;
-    // hashed visited set (search_kernel only): per slot an open-addressed table of keys id + 1 (0 = empty), linear probing
-    // from a multiplicative hash; `vlog` then logs the table positions a query filled.  nullptr = the bitmap above.
+    // hashed visited set (search_kernel only): per slot an open-addressed table (format: vhash_home); `vlog` then logs the
+    // table positions a query filled.  nullptr = the bitmap above.
     unsigned int* vhash;
     unsigned vhash_mask;                   // table entries per slot - 1 (a power of two)
-    int vhash_shift;                       // 32 - log2(entries): the home position is the top bits of id * 2654435769
+    int vhash_shift;                       // 32 - log2(entries)
     int vhash_limit;                       // distinct ids a query may insert before it is abandoned; INT_MAX without a table
     unsigned int* overflow;                // {count, query indices}: the queries abandoned at the limit
     const unsigned int* rerun;             // re-run launch: the same list; the kernel searches only the queries listed there
@@ -551,6 +562,11 @@ static __device__ __noinline__ int heap_full_slot(const int2* hs, const int2* hg
     return (d > best) ? -1 : besti;
 }
 
+// The hashed visited set's table format (the search kernels and iter_grow_kernel's rehash): an id is stored as the key
+// id + 1 (0 = an empty position) and probed linearly from its home position, the top log2(entries) bits of a multiplicative
+// hash (shift = 32 - log2(entries)); inserts stop at half the capacity.
+__host__ __device__ __forceinline__ unsigned vhash_home(unsigned id, int shift) { return (id * 2654435769u) >> shift; }
+
 // Hashed visited set (open addressing, keys id + 1, 0 = empty, linear probing).  The per-lane probe past the home position
 // is rare and kept out of line like heap_full_slot, so that it adds nothing to the kernels' register allocation; the
 // warp-uniform insert has an out-of-line copy too (which one costs fewer registers depends on the kernel).
@@ -902,6 +918,69 @@ struct WarpSearch {
     __device__ __forceinline__ WarpSearch(const SearchParams& p_, int lane_)
         : p(p_), lane(lane_), half(lane_ >> 4), j(lane_ & 15) {}
 
+    // The kernels' set-up: the shared-memory carve-up, the queue heads' descriptors (the caller binds their HBM arenas),
+    // the ring's barriers and the queues' sentinels
+    __device__ __forceinline__ void setup_warp(unsigned char* smem) {
+        ring = smem;
+        cand_id = reinterpret_cast<int*>(smem + p.off_cand);
+        cand_dist = reinterpret_cast<float*>(smem + p.off_cand + 128);
+        bars = reinterpret_cast<uint64_t*>(smem + p.off_bar);
+        qs = reinterpret_cast<float*>(smem + p.off_query);
+        ng.s = reinterpret_cast<int2*>(smem + p.off_ng);
+        ng.H = p.h_ng;
+        ng.length = p.ng_length;
+        ng.lastlevel = p.ng_lastlevel;
+        spt.s = reinterpret_cast<int2*>(smem + p.off_spt);
+        spt.H = p.h_spt;
+        spt.length = p.spt_length;
+        spt.lastlevel = p.spt_lastlevel;
+        phase_bits = 0;
+        if (lane == 0) {
+            for (int s = 0; s < p.stages; ++s) mbar_init(&bars[s], 1);
+            mbar_fence_init();
+            ng.s[0] = make_pair(-1, SPTAG_B200_MAXDIST);
+            spt.s[0] = make_pair(-1, SPTAG_B200_MAXDIST);
+        }
+        __syncwarp();
+    }
+    // WorkSpace::Reset + ResetResult (WorkSpace.h:265-286) but the visited set's contents: no ids inserted, empty queues,
+    // an m_Results of `mres_cap`, an empty top-K, zero counters
+    __device__ __forceinline__ void reset_workspace(int mres_cap) {
+        vlog_count = 0;
+        ng.count = 0;
+        spt.count = 0;
+        ng.tail_idx = spt.tail_idx = -1;
+        mres.reset(mres_cap, lane);
+        tk_d = SPTAG_B200_MAXDIST;
+        tk_id = -1;
+        worst_d = SPTAG_B200_MAXDIST;
+        worst_id = -1;
+        if (tk != nullptr) res_reset();
+        checked = ndist = nexpand = ntree = 0;
+        tree_checked = no_better = 0;
+    }
+    // the iterator kernels: the query (element type of the index) -> shared memory
+    __device__ __forceinline__ void load_query_bytes(int q) {
+        const unsigned char* qb = p.queries + (size_t)q * p.query_stride_bytes;
+        unsigned char* qd = reinterpret_cast<unsigned char*>(qs);
+        const int qbytes = p.dim * (ELEM == 0 ? 4 : (ELEM == 3 ? 2 : 1));
+        for (int i = lane; i < qbytes; i += 32) qd[i] = qb[i];
+    }
+    // the queue heads of a query whose queues persist in HBM: back into shared memory, and out again
+    __device__ __forceinline__ void restore_queue_heads() {
+        for (int i = 1 + lane; i <= min(ng.count, ng.H); i += 32) ng.s[i] = ng.g[i];
+        for (int i = 1 + lane; i <= min(spt.count, spt.H); i += 32) spt.s[i] = spt.g[i];
+    }
+    __device__ __forceinline__ void flush_queue_heads() {
+        for (int i = 1 + lane; i <= min(ng.count, ng.H); i += 32) ng.g[i] = ng.s[i];
+        for (int i = 1 + lane; i <= min(spt.count, spt.H); i += 32) spt.g[i] = spt.s[i];
+    }
+    // result i of query q into the caller's arrays (ids shifted by the index's id offset; -1 stays -1)
+    __device__ __forceinline__ void write_result(size_t q, int i, int id, float d) const {
+        p.out_ids[q * p.k + i] = (id >= 0) ? id + p.id_offset : id;
+        p.out_dists[q * p.k + i] = d;
+    }
+
     // Everything but the 512-byte-row fast path keeps the round-1 step order and queue code (see heap_pop_seq): those
     // kernels' residency is set by a register cap (768-d: 15 slots at 127 registers, PQ: 24 at 80) or by the uncapped
     // register count (integer rows), and the extra live values of the newer code cost them 7-17 % on a B200.
@@ -928,7 +1007,7 @@ struct WarpSearch {
     __device__ __forceinline__ unsigned vhash_mask() const { return QHASH ? qmask : p.vhash_mask; }
     // hashed visited set: home position of an id in this slot's table
     __device__ __forceinline__ unsigned vhash_home(int id) const {
-        return ((unsigned)id * 2654435769u) >> (QHASH ? qshift : p.vhash_shift);
+        return sptag_b200::vhash_home(id, QHASH ? qshift : p.vhash_shift);
     }
     // the query has filled its table to the load limit: it is abandoned (nothing counts as new any more, the search loops
     // stop) and search_kernel re-runs it on the bitmap.  Never true on the bitmap.  QHASH: the iterator kernels suspend
@@ -1400,6 +1479,45 @@ struct WarpSearch {
         if (nn >= 0) asm volatile("prefetch.global.L2 [%0];" ::"l"(visited + (hashed() ? vhash_home(nn) : (unsigned)(nn >> 5))));
     }
 
+    // One graph-row chunk after issue_mark: its fresh ids compacted into cand_id in neighbour order (and logged), and their
+    // distances in cand_dist.  Returns how many there are.  The iterator kernels bind no clear log (vlog = nullptr: their
+    // sets persist across calls), so the log store compiles away there; binding one would add it to every chunk.
+    __device__ __forceinline__ int expand_chunk(RowMark& mark, int nn) {
+        const bool fresh = mark_fresh(mark, nn);
+        const unsigned freshmask = __ballot_sync(kFull, fresh);
+        const int cnt = __popc(freshmask);
+        __syncwarp();
+        if (fresh) {
+            const int rank = __popc(freshmask & ((1u << lane) - 1u));
+            cand_id[rank] = nn;
+            if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = mark_word(mark, nn);
+        }
+        vlog_count += cnt;
+        compute_dists(cnt);
+        return cnt;
+    }
+
+    // BKT Search's accept of the popped node (BKTIndex.cpp:292-320): a node whose last graph entry `checkNode` points back
+    // to a duplicate group (< -1) offers every live member of that group to m_Results at its distance
+    __device__ __forceinline__ void add_node_or_group(int tmpNode, float gdist, int checkNode) {
+        if (checkNode < -1) {
+            const int tn = -2 - checkNode;
+            const int tcs = p.nodes[3 * tn + 1], tce = p.nodes[3 * tn + 2];
+            int i = -tcs;
+            do {
+                if (not_deleted(tmpNode)) {
+                    if (check_filter(tmpNode)) {
+                        if (!add_point(tmpNode, gdist) || p.never_dup) break;
+                    }
+                }
+                if (i <= 0) break;
+                tmpNode = p.nodes[3 * i];
+            } while (i++ < tce);
+        } else {
+            if (not_deleted(tmpNode) && check_filter(tmpNode)) add_point(tmpNode, gdist);
+        }
+    }
+
     // BKT::Index<T>::Search<notDeleted, CheckDup, AlwaysTrue> (BKTIndex.cpp:268-352).
     // One step's memory round trips are data-dependent (queue root -> graph row -> visited set -> vectors), so the order
     // inside a step is chosen to overlap them: the root of NGQueue is the popped node before the sift-down runs, so the
@@ -1433,24 +1551,7 @@ struct WarpSearch {
 
             bool stop = false;
             if (gdist <= worst_d) {
-                const int checkNode = (checkPos < 32) ? __shfl_sync(kFull, nn, checkPos) : node[checkPos];
-                if (checkNode < -1) {
-                    // duplicate group: the back-pointer names the BKT node listing exact duplicates
-                    const int tn = -2 - checkNode;
-                    const int tcs = p.nodes[3 * tn + 1], tce = p.nodes[3 * tn + 2];
-                    int i = -tcs;
-                    do {
-                        if (not_deleted(tmpNode)) {
-                            if (check_filter(tmpNode)) {
-                                if (!add_point(tmpNode, gdist) || p.never_dup) break;
-                            }
-                        }
-                        if (i <= 0) break;
-                        tmpNode = p.nodes[3 * i];
-                    } while (i++ < tce);
-                } else {
-                    if (not_deleted(tmpNode) && check_filter(tmpNode)) add_point(tmpNode, gdist);
-                }
+                add_node_or_group(tmpNode, gdist, (checkPos < 32) ? __shfl_sync(kFull, nn, checkPos) : node[checkPos]);
             } else {
                 if (not_deleted(tmpNode)) stop = (gdist > mres.worst || checked > p.max_check);
             }
@@ -1472,17 +1573,7 @@ struct WarpSearch {
                     nn = (cbase + lane <= checkPos) ? node[cbase + lane] : -1;
                     mark = issue_mark(nn, cbase + lane <= checkPos);
                 }
-                const bool fresh = mark_fresh(mark, nn);
-                const unsigned freshmask = __ballot_sync(kFull, fresh);
-                const int cnt = __popc(freshmask);
-                __syncwarp();
-                if (fresh) {
-                    const int rank = __popc(freshmask & ((1u << lane) - 1u));
-                    cand_id[rank] = nn;
-                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = mark_word(mark, nn);
-                }
-                vlog_count += cnt;
-                compute_dists(cnt);
+                const int cnt = expand_chunk(mark, nn);
                 // m_Results.worst() never increases, so a candidate above the current worst is rejected
                 // whenever its turn comes; only the others are replayed in neighbour order (BKTIndex.cpp:338-344)
                 const float myd = (lane < cnt) ? cand_dist[lane] : SPTAG_B200_MAXDIST;
@@ -1523,24 +1614,7 @@ struct WarpSearch {
             int nn = (lane <= checkPos) ? node[lane] : -1;
 
             if (gdist <= worst_d) {
-                const int checkNode = node[checkPos];
-                if (checkNode < -1) {
-                    // duplicate group: the back-pointer names the BKT node listing exact duplicates
-                    const int tn = -2 - checkNode;
-                    const int tcs = p.nodes[3 * tn + 1], tce = p.nodes[3 * tn + 2];
-                    int i = -tcs;
-                    do {
-                        if (not_deleted(tmpNode)) {
-                            if (check_filter(tmpNode)) {
-                                if (!add_point(tmpNode, gdist) || p.never_dup) break;
-                            }
-                        }
-                        if (i <= 0) break;
-                        tmpNode = p.nodes[3 * i];
-                    } while (i++ < tce);
-                } else {
-                    if (not_deleted(tmpNode) && check_filter(tmpNode)) add_point(tmpNode, gdist);
-                }
+                add_node_or_group(tmpNode, gdist, node[checkPos]);
             } else {
                 if (not_deleted(tmpNode)) {
                     if (gdist > mres.worst || checked > p.max_check) return;
@@ -1552,17 +1626,7 @@ struct WarpSearch {
                 // the scan stops at the first negative entry (BKTIndex.cpp:333-336); a repeated id inside the row is
                 // "visited" by the time its second copy is reached
                 RowMark mark = issue_mark(nn, cbase + lane <= checkPos);
-                const bool fresh = mark_fresh(mark, nn);
-                const unsigned freshmask = __ballot_sync(kFull, fresh);
-                const int cnt = __popc(freshmask);
-                __syncwarp();
-                if (fresh) {
-                    const int rank = __popc(freshmask & ((1u << lane) - 1u));
-                    cand_id[rank] = nn;
-                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = mark_word(mark, nn);
-                }
-                vlog_count += cnt;
-                compute_dists(cnt);
+                const int cnt = expand_chunk(mark, nn);
                 // m_Results.worst() never increases, so a candidate above the current worst is rejected
                 // whenever its turn comes; only the others are replayed in neighbour order (BKTIndex.cpp:338-344)
                 const float myd = (lane < cnt) ? cand_dist[lane] : SPTAG_B200_MAXDIST;
@@ -1665,13 +1729,7 @@ struct WarpSearch {
             for (int cbase = 0; cbase <= checkPos; cbase += 32) {
                 if (cbase > 0) nn = (cbase + lane <= checkPos) ? node[cbase + lane] : -1;
                 RowMark mark = issue_mark(nn, cbase + lane <= checkPos);
-                const bool fresh = mark_fresh(mark, nn);
-                const unsigned freshmask = __ballot_sync(kFull, fresh);
-                const int cnt = __popc(freshmask);
-                __syncwarp();
-                if (fresh) cand_id[__popc(freshmask & ((1u << lane) - 1u))] = nn;
-                vlog_count += cnt;
-                compute_dists(cnt);
+                const int cnt = expand_chunk(mark, nn);
                 checked += cnt;
                 for (int r = 0; r < cnt; ++r) {
                     const int id = cand_id[r];
@@ -1707,13 +1765,7 @@ struct WarpSearch {
             const bool in_row = (cbase + lane <= checkPos);
             const int nn = in_row ? node[cbase + lane] : -1;
             RowMark mark = issue_mark(nn, in_row);
-            const bool fresh = mark_fresh(mark, nn);
-            const unsigned freshmask = __ballot_sync(kFull, fresh);
-            const int cnt = __popc(freshmask);
-            __syncwarp();
-            if (fresh) cand_id[__popc(freshmask & ((1u << lane) - 1u))] = nn;
-            vlog_count += cnt;
-            compute_dists(cnt);
+            const int cnt = expand_chunk(mark, nn);
             for (int r = 0; r < cnt; ++r) hins(ng, cand_id[r], cand_dist[r]);
             __syncwarp();
             if (mark.first_neg < 32) break;
@@ -1800,17 +1852,7 @@ struct WarpSearch {
                     nn = (cbase + lane < p.degree) ? node[cbase + lane] : -1;
                     mark = issue_mark(nn, cbase + lane < p.degree);
                 }
-                const bool fresh = mark_fresh(mark, nn);
-                const unsigned freshmask = __ballot_sync(kFull, fresh);
-                const int cnt = __popc(freshmask);
-                __syncwarp();
-                if (fresh) {
-                    const int rank = __popc(freshmask & ((1u << lane) - 1u));
-                    cand_id[rank] = nn;
-                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = mark_word(mark, nn);
-                }
-                vlog_count += cnt;
-                compute_dists(cnt);
+                const int cnt = expand_chunk(mark, nn);
                 // every new neighbour enters NGQueue, in neighbour order (KDTIndex.cpp:212-223)
                 const float myd = (lane < cnt) ? cand_dist[lane] : SPTAG_B200_MAXDIST;
                 const int myid = (lane < cnt) ? cand_id[lane] : -1;
@@ -1851,17 +1893,7 @@ struct WarpSearch {
             for (int cbase = 0; cbase < p.degree; cbase += 32) {
                 if (cbase > 0) nn = (cbase + lane < p.degree) ? node[cbase + lane] : -1;
                 RowMark mark = issue_mark(nn, cbase + lane < p.degree);
-                const bool fresh = mark_fresh(mark, nn);
-                const unsigned freshmask = __ballot_sync(kFull, fresh);
-                const int cnt = __popc(freshmask);
-                __syncwarp();
-                if (fresh) {
-                    const int rank = __popc(freshmask & ((1u << lane) - 1u));
-                    cand_id[rank] = nn;
-                    if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = mark_word(mark, nn);
-                }
-                vlog_count += cnt;
-                compute_dists(cnt);
+                const int cnt = expand_chunk(mark, nn);
                 for (int r = 0; r < cnt; ++r) {
                     const float d = cand_dist[r];
                     if (d <= upperBound) bLocalOpt = false;
@@ -1895,33 +1927,12 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
     extern __shared__ __align__(128) unsigned char smem[];
     const int lane = threadIdx.x;
     WarpSearch<DIM, COSINE, RPL, PQ, ELEM, true> w(p, lane);
-    w.ring = smem;
-    w.cand_id = reinterpret_cast<int*>(smem + p.off_cand);
-    w.cand_dist = reinterpret_cast<float*>(smem + p.off_cand + 128);
-    w.bars = reinterpret_cast<uint64_t*>(smem + p.off_bar);
-    w.qs = reinterpret_cast<float*>(smem + p.off_query);
     w.visited = p.vhash ? p.vhash + (size_t)blockIdx.x * (p.vhash_mask + 1ull) : p.visited + (size_t)blockIdx.x * p.visited_words;
     w.vlog = p.vlog ? p.vlog + (size_t)blockIdx.x * p.vlog_entries : nullptr;
     w.tk = p.topk ? p.topk + (size_t)blockIdx.x * p.topk_pad : nullptr;
-    w.ng.s = reinterpret_cast<int2*>(smem + p.off_ng);
     w.ng.g = p.ng_spill + (size_t)blockIdx.x * p.ng_spill_entries;
-    w.ng.H = p.h_ng;
-    w.ng.length = p.ng_length;
-    w.ng.lastlevel = p.ng_lastlevel;
-    w.spt.s = reinterpret_cast<int2*>(smem + p.off_spt);
     w.spt.g = p.spt_spill + (size_t)blockIdx.x * p.spt_spill_entries;
-    w.spt.H = p.h_spt;
-    w.spt.length = p.spt_length;
-    w.spt.lastlevel = p.spt_lastlevel;
-    w.phase_bits = 0;
-
-    if (lane == 0) {
-        for (int s = 0; s < p.stages; ++s) mbar_init(&w.bars[s], 1);
-        mbar_fence_init();
-        w.ng.s[0] = make_pair(-1, SPTAG_B200_MAXDIST);
-        w.spt.s[0] = make_pair(-1, SPTAG_B200_MAXDIST);
-    }
-    __syncwarp();
+    w.setup_warp(smem);
 
     for (;;) {
         // unsigned: the output offsets below zero-extend it, so nothing about it has to be kept live across the search
@@ -1942,18 +1953,7 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
             const size_t n4 = p.visited_words >> 2;
             for (size_t i = lane; i < n4; i += 32) v4[i] = make_uint4(0, 0, 0, 0);
         }
-        w.vlog_count = 0;
-        w.ng.count = 0;
-        w.spt.count = 0;
-        w.ng.tail_idx = w.spt.tail_idx = -1;
-        w.mres.reset(p.mres_cap, lane);
-        w.tk_d = SPTAG_B200_MAXDIST;
-        w.tk_id = -1;
-        w.worst_d = SPTAG_B200_MAXDIST;
-        w.worst_id = -1;
-        if (w.tk != nullptr) w.res_reset();
-        w.checked = w.ndist = w.nexpand = w.ntree = 0;
-        w.tree_checked = w.no_better = 0;
+        w.reset_workspace(p.mres_cap);
         // query -> shared memory (+ registers for the static-DIM variants)
         if (PQ && p.pq_adc) {
             // PQQuantizer::QuantizeVector with ADC on (PQQuantizer.h:141-157): table[i][j] = L2(query sub-vector i,
@@ -2027,13 +2027,10 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
             w.res_sort();
             for (int i = lane; i < p.k; i += 32) {
                 const int2 e = w.tk[i];
-                p.out_ids[(size_t)q * p.k + i] = (e.x >= 0) ? e.x + p.id_offset : e.x;
-                p.out_dists[(size_t)q * p.k + i] = __int_as_float(e.y);
+                w.write_result(q, i, e.x, __int_as_float(e.y));
             }
         } else if (lane < p.k) {
-            const int id = w.tk_id;
-            p.out_ids[(size_t)q * p.k + lane] = (id >= 0) ? id + p.id_offset : id;
-            p.out_dists[(size_t)q * p.k + lane] = w.tk_d;
+            w.write_result(q, lane, w.tk_id, w.tk_d);
         }
         if (p.out_stats != nullptr && lane == 0) {
             int* s = p.out_stats + (size_t)q * kStatsPerQuery;
@@ -2054,8 +2051,7 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
 // ResultIterator::Next for a batch of open iterators (ResultIterator.cpp:31-55 -> SearchIndexIterativeNext,
 // BKTIndex.cpp:659-675).  Every query owns persistent arenas in HBM -- visited bitmap, NGQueue, SPTQueue (the
 // reference's rented WorkSpace) -- indexed by query, not by slot; the shared-memory queue heads are restored from and
-// flushed to those arenas around each call.  state[q] = {ng count, spt count, first call, relaxedMono, result slots,
-// log2 of the visited table's entries (0: a bitmap), the visited set's fill, resume point}.
+// flushed to those arenas around each call, and the rest of its state is an IterState.
 // p.k = the batch the caller asked for; the effective batch of a query is capped by the result count of its previous
 // call (QueryResult::SetResultNum(resultCount), ResultIterator.cpp:36-41, :52).
 // A query on a hash table that reaches the table's limit suspends (bkt_search_iterative): it saves what the call has
@@ -2063,8 +2059,6 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
 // that list (iv.list), where the query continues from the saved state.  The visited set has exact set semantics in
 // both forms, so the results do not depend on where, or how often, a query was suspended.
 // ------------------------------------------------------------------------------------------
-constexpr int kIterStateInts = 8;
-
 // The per-query visited set of an iterator kernel: its table or bitmap, and the table's capacity
 template <typename W>
 __device__ __forceinline__ void bind_iter_visited(W& w, const SearchParams& p, const IterVisited& iv, int q, int bits) {
@@ -2095,52 +2089,31 @@ __global__ void __launch_bounds__(32, 12) iterate_kernel(const SearchParams p, i
                                                          unsigned char* __restrict__ out_relaxed, const IterVisited iv) {
     extern __shared__ __align__(128) unsigned char smem[];
     const int lane = threadIdx.x;
+    IterState* const states = reinterpret_cast<IterState*>(state);
     WarpSearch<0, COSINE, RPL, false, ELEM, false, true> w(p, lane);
-    w.ring = smem;
-    w.cand_id = reinterpret_cast<int*>(smem + p.off_cand);
-    w.cand_dist = reinterpret_cast<float*>(smem + p.off_cand + 128);
-    w.bars = reinterpret_cast<uint64_t*>(smem + p.off_bar);
-    w.qs = reinterpret_cast<float*>(smem + p.off_query);
     w.vlog = nullptr;  // the bitmap belongs to the iterator and is never cleared between calls
-    w.ng.s = reinterpret_cast<int2*>(smem + p.off_ng);
-    w.ng.H = p.h_ng;
-    w.ng.length = p.ng_length;
-    w.ng.lastlevel = p.ng_lastlevel;
-    w.spt.s = reinterpret_cast<int2*>(smem + p.off_spt);
-    w.spt.H = p.h_spt;
-    w.spt.length = p.spt_length;
-    w.spt.lastlevel = p.spt_lastlevel;
-    w.phase_bits = 0;
-    if (lane == 0) {
-        for (int s = 0; s < p.stages; ++s) mbar_init(&w.bars[s], 1);
-        mbar_fence_init();
-        w.ng.s[0] = make_pair(-1, SPTAG_B200_MAXDIST);
-        w.spt.s[0] = make_pair(-1, SPTAG_B200_MAXDIST);
-    }
-    __syncwarp();
+    w.setup_warp(smem);
 
     for (;;) {
         const int q = next_iter_query(p, iv, lane);
         if (q < 0) break;
-        int* st = state + (size_t)q * kIterStateInts;
-        bind_iter_visited(w, p, iv, q, st[5]);
+        IterState& st = states[q];
+        bind_iter_visited(w, p, iv, q, st.vbits);
         w.ng.g = p.ng_spill + (size_t)q * p.ng_spill_entries;
         w.spt.g = p.spt_spill + (size_t)q * p.spt_spill_entries;
         w.tk = p.topk + (size_t)q * p.topk_pad;
-        w.ng.count = st[0];
-        w.spt.count = st[1];
+        w.ng.count = st.ng_count;
+        w.spt.count = st.spt_count;
         w.ng.tail_idx = w.spt.tail_idx = -1;
-        const int resumed = st[7];
-        int at = resumed ? resumed : (st[2] != 0 ? kIterFirst : kIterStep);
-        int relaxed = st[3];
-        const int slots = st[4];
+        const int resumed = st.resume;
+        int at = resumed ? resumed : (st.first != 0 ? kIterFirst : kIterStep);
+        int relaxed = st.relaxed;
+        const int slots = st.slots;
         const int batch = (slots < 0) ? p.k : min(p.k, slots);
-        // queue heads back into shared memory
-        for (int i = 1 + lane; i <= min(w.ng.count, w.ng.H); i += 32) w.ng.s[i] = w.ng.g[i];
-        for (int i = 1 + lane; i <= min(w.spt.count, w.spt.H); i += 32) w.spt.s[i] = w.spt.g[i];
+        w.restore_queue_heads();
         w.ndist = w.nexpand = w.ntree = 0;
         w.tree_checked = w.no_better = 0;
-        w.vlog_count = st[6];
+        w.vlog_count = st.vfill;
         float* saved = iv.resume ? iv.resume + (size_t)q * kIterResumeWords : nullptr;
         int count = 0, limit = 0;
         if (resumed) {  // the call this query suspended in: m_Results, resultCount, checked and the SearchTrees limit
@@ -2155,12 +2128,7 @@ __global__ void __launch_bounds__(32, 12) iterate_kernel(const SearchParams p, i
             w.checked = 0;
         }
         w.tk_count = count;
-        {   // the query (element type of the index) -> shared memory
-            const unsigned char* qb = p.queries + (size_t)q * p.query_stride_bytes;
-            unsigned char* qd = reinterpret_cast<unsigned char*>(w.qs);
-            const int qbytes = p.dim * (ELEM == 0 ? 4 : (ELEM == 3 ? 2 : 1));
-            for (int i = lane; i < qbytes; i += 32) qd[i] = qb[i];
-        }
+        w.load_query_bytes(q);
         __syncwarp();
 
         w.bkt_search_iterative(at, batch, relaxed, count, limit, iv.margin);
@@ -2174,14 +2142,13 @@ __global__ void __launch_bounds__(32, 12) iterate_kernel(const SearchParams p, i
                 si[1] = w.checked;
                 si[2] = limit;
             }
-            for (int i = 1 + lane; i <= min(w.ng.count, w.ng.H); i += 32) w.ng.g[i] = w.ng.s[i];
-            for (int i = 1 + lane; i <= min(w.spt.count, w.spt.H); i += 32) w.spt.g[i] = w.spt.s[i];
+            w.flush_queue_heads();
             if (lane == 0) {
-                st[0] = w.ng.count;
-                st[1] = w.spt.count;
-                st[3] = relaxed;
-                st[6] = w.vlog_count;
-                st[7] = at;
+                st.ng_count = w.ng.count;
+                st.spt_count = w.spt.count;
+                st.relaxed = relaxed;
+                st.vfill = w.vlog_count;
+                st.resume = at;
             }
             suspend_iter_query(iv, q, at == kIterStep ? 1 : 2, lane);
             __syncwarp();
@@ -2191,20 +2158,18 @@ __global__ void __launch_bounds__(32, 12) iterate_kernel(const SearchParams p, i
         w.res_sort();
         for (int i = lane; i < p.k; i += 32) {
             const int2 e = (i < count) ? w.tk[i] : make_pair(-1, SPTAG_B200_MAXDIST);
-            p.out_ids[(size_t)q * p.k + i] = (e.x >= 0) ? e.x + p.id_offset : e.x;
-            p.out_dists[(size_t)q * p.k + i] = __int_as_float(e.y);
+            w.write_result(q, i, e.x, __int_as_float(e.y));
         }
         // flush the queue heads and the scalars
-        for (int i = 1 + lane; i <= min(w.ng.count, w.ng.H); i += 32) w.ng.g[i] = w.ng.s[i];
-        for (int i = 1 + lane; i <= min(w.spt.count, w.spt.H); i += 32) w.spt.g[i] = w.spt.s[i];
+        w.flush_queue_heads();
         if (lane == 0) {
-            st[0] = w.ng.count;
-            st[1] = w.spt.count;
-            st[2] = 0;
-            st[3] = relaxed;
-            st[4] = count;  // m_queryResult->SetResultNum(resultCount)
-            st[6] = w.vlog_count;
-            st[7] = 0;
+            st.ng_count = w.ng.count;
+            st.spt_count = w.spt.count;
+            st.first = 0;
+            st.relaxed = relaxed;
+            st.slots = count;  // m_queryResult->SetResultNum(resultCount)
+            st.vfill = w.vlog_count;
+            st.resume = 0;
             out_counts[q] = count;
             out_relaxed[q] = (unsigned char)relaxed;
         }
@@ -2227,6 +2192,7 @@ __global__ void __launch_bounds__(32, 12) nearest_first_kernel(const SearchParam
                                                                const IterVisited iv) {
     extern __shared__ __align__(128) unsigned char smem[];
     const int lane = threadIdx.x;
+    IterState* const states = reinterpret_cast<IterState*>(state);
     WarpSearch<0, COSINE, RPL, false, ELEM, false, true> w(p, lane);
     w.ring = smem;
     w.cand_id = reinterpret_cast<int*>(smem + p.off_cand);
@@ -2254,8 +2220,8 @@ __global__ void __launch_bounds__(32, 12) nearest_first_kernel(const SearchParam
     for (;;) {
         const int q = next_iter_query(p, iv, lane);
         if (q < 0) break;
-        int* st = state + (size_t)q * kIterStateInts;
-        bind_iter_visited(w, p, iv, q, st[5]);  // empty: zeroed when the iterator was opened or the table was grown
+        IterState& st = states[q];
+        bind_iter_visited(w, p, iv, q, st.vbits);  // empty: zeroed when the iterator was opened or the table was grown
         w.ng.g = p.ng_spill + (size_t)q * p.ng_spill_entries;
         w.spt.g = p.spt_spill + (size_t)q * p.spt_spill_entries;
         w.tk = (p.k > 32) ? p.topk + (size_t)q * p.topk_pad : nullptr;
@@ -2320,11 +2286,11 @@ __global__ void __launch_bounds__(32, 12) nearest_first_kernel(const SearchParam
         for (int i = 1 + lane; i <= min(w.ng.count, w.ng.H); i += 32) w.ng.g[i] = w.ng.s[i];
         for (int i = 1 + lane; i <= min(w.spt.count, w.spt.H); i += 32) w.spt.g[i] = w.spt.s[i];
         if (lane == 0) {
-            st[0] = w.ng.count;
-            st[1] = w.spt.count;
-            st[2] = 0;
-            st[4] = -1;
-            st[6] = w.vlog_count;
+            st.ng_count = w.ng.count;
+            st.spt_count = w.spt.count;
+            st.first = 0;
+            st.slots = -1;
+            st.vfill = w.vlog_count;
         }
         __syncwarp();
     }

@@ -15,6 +15,7 @@
 #include <climits>
 #include <cmath>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -300,6 +301,21 @@ int check_supported(const sptag_b200_index* h, int k) {
     return 0;
 }
 
+// log2 of a hashed visited set's entries: `entries` (B200.VisitedHashEntries, B200.IteratorVisitedHashEntries) rounded up
+// to a power of two, or when it is 0 the reference's first-block size 2^(bits(max(MaxCheck, MaxCheckForRefineGraph)) +
+// HashTableExponent 2) (WorkSpace.h:83-93) for `check` = that maximum.  At least 64 entries: a query stops inserting at
+// half the capacity, and the last row chunk may add up to 31 ids past that, which must still find an empty position (the
+// probes end only at one).
+int vhash_log2_entries(int entries, int check) {
+    int bits = 0;
+    if (entries > 0) {
+        while ((1 << bits) < entries) ++bits;
+        return bits;
+    }
+    for (unsigned s = (unsigned)std::max(check, 1); s != 0; s >>= 1) ++bits;
+    return std::min(std::max(bits + 2, 6), 30);
+}
+
 // SearchParams from the handle and the call's options, including the per-slot arena sizes; the shared-memory layout
 // (lay_out) and the scratch pointers (bind_scratch) come later
 void fill_params(const sptag_b200_index* h, int k, const CallOpts& opts, SearchParams& p) {
@@ -355,17 +371,8 @@ void fill_params(const sptag_b200_index* h, int k, const CallOpts& opts, SearchP
                                                           : (size_t)std::max(65536, 8 * alloc_check);
         p.vlog_entries = std::min(entries, (size_t)h->n + 2);
     }
-    // hashed visited set, bound only by bind_scratch: the reference's first-block size 2^(bits(max(MaxCheck,
-    // MaxCheckForRefineGraph)) + HashTableExponent 2) (WorkSpace.h:83-93) unless B200.VisitedHashEntries sets it
-    // At least 64 entries: a query stops inserting at half the capacity, and the last row chunk may add up to 31 ids past
-    // that, which must still find an empty position (the probes end only at one).
-    int log2_entries = 0;
-    if (h->visited_hash_entries > 0) {
-        while ((1 << log2_entries) < h->visited_hash_entries) ++log2_entries;
-    } else {
-        for (unsigned s = (unsigned)std::max(alloc_check, 1); s != 0; s >>= 1) ++log2_entries;
-        log2_entries = std::min(std::max(log2_entries + 2, 6), 30);
-    }
+    // hashed visited set, bound only by bind_scratch
+    const int log2_entries = vhash_log2_entries(h->visited_hash_entries, alloc_check);
     p.vhash_mask = (1u << log2_entries) - 1u;
     p.vhash_shift = 32 - log2_entries;
     p.vhash_limit = INT_MAX;
@@ -1788,7 +1795,7 @@ int sptag_b200_iterator_open_ex(sptag_b200_handle h, const void* queries, int32_
     int rc = 0;
     if ((rc = it->d_queries.ensure(qbytes)) || (rc = it->d_ng.ensure((size_t)num_queries * it->ng_entries * 8)) ||
         (rc = it->d_spt.ensure((size_t)num_queries * it->spt_entries * 8)) ||
-        (rc = it->d_state.ensure((size_t)num_queries * kIterStateInts * 4)) ||
+        (rc = it->d_state.ensure((size_t)num_queries * sizeof(IterState))) ||
         (rc = it->d_counts.ensure((size_t)num_queries * 4)) || (rc = it->d_relaxed.ensure((size_t)num_queries))) {
         delete it;
         return rc;
@@ -1821,12 +1828,7 @@ int sptag_b200_iterator_open_ex(sptag_b200_handle h, const void* queries, int32_
         it->margin = h->degree + h->max_dup + 1;
         // initial entries: B200.IteratorVisitedHashEntries, or the reference's first-block size as for search; raised
         // until one step fits below the limit, so that doubling a table always makes room for the step that suspended
-        if (h->iter_hash_entries > 0) {
-            while ((1 << bits) < h->iter_hash_entries) ++bits;
-        } else {
-            for (unsigned s = (unsigned)std::max(std::max(h->max_check, h->max_check_refine), 1); s != 0; s >>= 1) ++bits;
-            bits = std::min(std::max(bits + 2, 6), 30);
-        }
+        bits = vhash_log2_entries(h->iter_hash_entries, std::max(h->max_check, h->max_check_refine));
         while (bits < 30 && (1 << (bits - 1)) < it->margin) ++bits;
         const size_t entries = (size_t)1 << bits;
         it->vbufs.emplace_back();
@@ -1844,18 +1846,17 @@ int sptag_b200_iterator_open_ex(sptag_b200_handle h, const void* queries, int32_
         it->q_set.resize(num_queries);
         for (int q = 0; q < num_queries; ++q) it->q_set[q] = (unsigned int*)it->vbufs[0].ptr + (size_t)q * entries;
     }
-    std::vector<int> st((size_t)num_queries * kIterStateInts, 0);
-    for (int q = 0; q < num_queries; ++q) {
-        st[(size_t)q * kIterStateInts + 2] = 1;   // first call: InitSearchTrees + SearchTrees
-        st[(size_t)q * kIterStateInts + 4] = -1;  // no QueryResult yet: the first Next sets the slot count
-        st[(size_t)q * kIterStateInts + 5] = bits;
-    }
+    IterState st0 = {};
+    st0.first = 1;   // first call: InitSearchTrees + SearchTrees
+    st0.slots = -1;  // no QueryResult yet: the first Next sets the slot count
+    st0.vbits = bits;
+    const std::vector<IterState> st(num_queries, st0);
     cudaError_t e = cudaMemcpy(it->d_queries.ptr, queries, qbytes, cudaMemcpyHostToDevice);
     if (e == cudaSuccess && !it->hashed) e = cudaMemset(it->d_visited.ptr, 0, it->d_visited.bytes);
     if (e == cudaSuccess && it->hashed) e = cudaMemset(it->vbufs[0].ptr, 0, it->vbufs[0].bytes);
     if (e == cudaSuccess && it->hashed)
         e = cudaMemcpy(it->d_tables.ptr, it->q_set.data(), (size_t)num_queries * sizeof(unsigned int*), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(it->d_state.ptr, st.data(), st.size() * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(it->d_state.ptr, st.data(), st.size() * sizeof(IterState), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
         delete it;
         return fail(SPTAG_B200_FAIL, "iterator set-up failed: %s", cudaGetErrorString(e));
@@ -1931,7 +1932,8 @@ int sptag_b200_iterator_next_from_nearest(sptag_b200_iter it, int32_t k, int32_t
                 // the caller Reset()s a QueryResult that keeps its k slots (SPANNIndex.cpp:284): no cap from the previous
                 // count (once per call: a resume launch must not undo what its completed queries set)
                 if (!iv.list)
-                    CUDA_OK(cudaMemset2DAsync((int*)it->d_state.ptr + 4, (size_t)kIterStateInts * 4, 0xFF, 4, (size_t)it->nq, stream));
+                    CUDA_OK(cudaMemset2DAsync((char*)it->d_state.ptr + offsetof(IterState, slots), sizeof(IterState), 0xFF,
+                                              sizeof(int), (size_t)it->nq, stream));
                 CUDA_OK(cudaFuncSetAttribute((const void*)knext, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                 knext<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, (int*)it->d_counts.ptr, (unsigned char*)it->d_relaxed.ptr, iv);
             }
