@@ -114,7 +114,10 @@ void sptag_b200_destroy(sptag_b200_handle h);
 /* Replaces: VectorIndex::SetParameter / GetParameter (BKTIndex.cpp:980-1025) for the search-time
  * parameters, same names as the ini file: MaxCheck, MaxCheckForRefineGraph,
  * NumberOfInitialDynamicPivots, NumberOfOtherDynamicPivots,
- * ThresholdOfNumberOfContinuousNoBetterPropagation; the update parameters AddCEF (500), CEF (1000) and RNGFactor (1.0,
+ * ThresholdOfNumberOfContinuousNoBetterPropagation; EnableBfs (BKT only, any int, default 0: BKTree::m_bfs, the number
+ * of breadth-first seeding levels of every search, BKTree.h:703-758; negative values seed breadth-first with no level;
+ * read when a search call is made, and by an iterator at its first Next / SearchIndexIterativeFromNeareast call; on a
+ * KDT handle it is ParamNotFound, and sptag_b200_load ignores it there); the update parameters AddCEF (500), CEF (1000) and RNGFactor (1.0,
  * a float) used by sptag_b200_add / sptag_b200_delete_vectors; "EnableADC" = VectorIndex::SetQuantizerADC
  * (VectorIndex.h:136-138) for quantized indexes; "SearchDeleted" (0/1) = the handle-wide DEFAULT of the
  * p_searchDeleted argument (the per-call value is sptag_b200_search_options.search_deleted /

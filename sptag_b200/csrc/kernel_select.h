@@ -25,5 +25,14 @@ SearchKernelFn pick_pq_kernel(int mres_cap);
 // ResultIterator::Next and SearchIndexIterativeFromNeareast's first call; value_type as in include/sptag_b200.h
 IterateKernelFn pick_iterate_kernel_for(int value_type, bool cosine, int mres_cap);
 NearestFirstKernelFn pick_nearest_first_kernel_for(int value_type, bool cosine, int mres_cap);
+// EnableBfs != 0 (BKT only): the same families with breadth-first tree seeding.  Float rows of every dimension take the
+// generic-dimension instantiations (no 128- / 768-d specialisation).
+SearchKernelFn pick_float_bfs_kernel_l2(int mres_cap);
+SearchKernelFn pick_float_bfs_kernel_cosine(int mres_cap);
+SearchKernelFn pick_int8_bfs_kernel(bool is_unsigned, bool cosine, int mres_cap);
+SearchKernelFn pick_int16_bfs_kernel(bool cosine, int mres_cap);
+SearchKernelFn pick_pq_bfs_kernel(int mres_cap);
+IterateKernelFn pick_iterate_bfs_kernel_for(int value_type, bool cosine, int mres_cap);
+NearestFirstKernelFn pick_nearest_first_bfs_kernel_for(int value_type, bool cosine, int mres_cap);
 
 }  // namespace sptag_b200

@@ -74,6 +74,9 @@ struct SearchParams {
     int n, dim;
     const int* graph;
     int degree;
+    // EnableBfs (BKTree::m_bfs, the bfs:: kernels only): != 0 seeds each tree breadth-first.  (Here it fills the padding
+    // before `nodes`: a longer struct would move the iterator kernels' later arguments and change their code.)
+    int bfs;
     const int* nodes;                      // BKT: 3 x int32 per node; KDT: 4 x 32 bit per node
     const int* tree_starts;
     int tree_num, node_count;
@@ -134,6 +137,11 @@ struct SearchParams {
     // a duplicate group contributes its first live member only
     int never_dup;
 };
+
+// BKTree::InitSearchTrees with m_bfs != 0 (BKTree.h:703-758): MaxBFSNodes, and the entries of one BFS heap (1-based, so
+// index 0 is never written).  The two heaps sit at the end of the query's SPTQueue arena, which is that much longer.
+constexpr int kBfsMaxNodes = 100;
+constexpr int kBfsHeapEntries = kBfsMaxNodes + 1;
 
 // ------------------------------------------------------------------------------------------
 // PTX helpers: mbarrier + 1-D TMA bulk copy
@@ -880,7 +888,8 @@ struct BktNodeDev {
 
 // HASH: the hashed visited set can be bound (search_kernel).  QHASH: the visited set is chosen per query (the iterator
 // kernels): a hash table whose capacity the query carries in qmask / qshift / qlimit, or a bitmap (qmask = 0).
-template <int DIM, bool COSINE, int RPL, bool PQ, int ELEM, bool HASH = false, bool QHASH = false>
+// BFS: the kernel seeds BKT trees breadth-first when p.bfs != 0 (the bfs:: kernels)
+template <int DIM, bool COSINE, int RPL, bool PQ, int ELEM, bool HASH = false, bool QHASH = false, bool BFS = false>
 struct WarpSearch {
     const SearchParams& p;
     const int lane, half, j;
@@ -1397,8 +1406,79 @@ struct WarpSearch {
                 compute_dists(1);
                 hins(spt, start, cand_dist[0]);
             } else {
+                // (a compile-time branch: a dead call alone changes the other kernels' code)
+                if constexpr (BFS) {
+                    if (p.bfs != 0) {
+                        init_search_trees_bfs(cs, ce);
+                        continue;
+                    }
+                }
                 push_children(cs, ce);
             }
+        }
+    }
+
+    // ---- BKTree::InitSearchTrees, m_bfs != 0 (BKTree.h:703-758) ----
+    // m_currBSPTQueue / m_nextBSPTQueue: Heap<NodeDistPair> of MaxBFSNodes entries, held wholly in HBM at the end of this
+    // query's SPTQueue arena (s = g, so every access is a plain global load / store) and emulated by the same insert and
+    // pop as the queues.  They live only while a tree is seeded.
+    __device__ __forceinline__ WarpHeap bfs_heap(int which) const {
+        WarpHeap h;
+        h.s = h.g = spt.g + p.spt_spill_entries - (size_t)(2 - which) * kBfsHeapEntries;
+        h.H = kBfsMaxNodes;
+        h.count = 0;
+        h.length = kBfsMaxNodes;
+        h.lastlevel = 64;  // never read: admission keeps count below length, so insert never takes the full-heap branch
+        h.tail_idx = -1;
+        return h;
+    }
+    // The children [cs, ce) in child order: into `q` while dist <= 1.1f * q.Top() (an fp32 product) and q holds fewer than
+    // MaxBFSNodes, into SPTQueue otherwise.  Top() of the empty heap is the 1e9 the reference writes into heap[0]; the
+    // top after an insert is the new pair exactly when it is smaller than the old top (the sift-up compares with <).
+    __device__ __forceinline__ void bfs_admit(WarpHeap& q, int cs, int ce) {
+        float top = q.count == 0 ? 1e9f : pair_dist(heap_ld(q, 1));
+        for (int base = cs; base < ce; base += 32) {
+            const int cnt = min(32, ce - base);
+            __syncwarp();
+            if (lane < cnt) cand_id[lane] = p.nodes[3 * (base + lane)];
+            ntree += cnt;
+            compute_dists(cnt);
+            for (int r = 0; r < cnt; ++r) {
+                const float d = cand_dist[r];
+                if (d <= __fmul_rn(1.1f, top) && q.count < kBfsMaxNodes) {
+                    if (q.count == 0 || d < top) top = d;
+                    heap_insert<false>(q, base + r, d, lane);
+                } else {
+                    hins(spt, base + r, d);
+                }
+            }
+        }
+    }
+    // One tree whose root has children [cs, ce).  Levels run while `curr` holds nodes: once it is empty every later level
+    // of the reference's m_bfs loop does nothing.  A popped leaf goes to SPTQueue (no CheckAndSet, not counted); a popped
+    // internal node's centre enters NGQueue if new (not counted as a checked leaf) and its children are admitted to `next`.
+    __device__ __forceinline__ void init_search_trees_bfs(int cs, int ce) {
+        WarpHeap curr = bfs_heap(0), next = bfs_heap(1);
+        bfs_admit(curr, cs, ce);
+        for (int level = 1; level <= p.bfs && curr.count != 0; ++level) {
+            while (curr.count != 0) {
+                const int2 tmp = heap_pop_seq(curr, lane);
+                const int tcenter = p.nodes[3 * tmp.x], tcs = p.nodes[3 * tmp.x + 1], tce = p.nodes[3 * tmp.x + 2];
+                ntree++;
+                if (tcs < 0) {
+                    hins(spt, tmp.x, pair_dist(tmp));
+                } else {
+                    if (!check_and_set_uniform(tcenter)) hins(ng, tcenter, pair_dist(tmp));
+                    bfs_admit(next, tcs, tce);
+                }
+            }
+            const WarpHeap t = curr;
+            curr = next;
+            next = t;
+        }
+        while (curr.count != 0) {
+            const int2 e = heap_pop_seq(curr, lane);
+            hins(spt, e.x, pair_dist(e));
         }
     }
 
@@ -1917,148 +1997,6 @@ struct WarpSearch {
     }
 };
 
-// ------------------------------------------------------------------------------------------
-// kernel: persistent warps pull queries from a global counter
-// ------------------------------------------------------------------------------------------
-// MINB = minimum resident single-warp CTAs per SM the compiler must allow (caps registers): the PQ variant is
-// bound by per-step latency, so more resident queries win (80 registers, 24 per SM)
-template <int DIM, bool COSINE, int RPL, bool KDT, bool PQ = false, int ELEM = 0, int MINB = 1>
-__global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) {
-    extern __shared__ __align__(128) unsigned char smem[];
-    const int lane = threadIdx.x;
-    WarpSearch<DIM, COSINE, RPL, PQ, ELEM, true> w(p, lane);
-    w.visited = p.vhash ? p.vhash + (size_t)blockIdx.x * (p.vhash_mask + 1ull) : p.visited + (size_t)blockIdx.x * p.visited_words;
-    w.vlog = p.vlog ? p.vlog + (size_t)blockIdx.x * p.vlog_entries : nullptr;
-    w.tk = p.topk ? p.topk + (size_t)blockIdx.x * p.topk_pad : nullptr;
-    w.ng.g = p.ng_spill + (size_t)blockIdx.x * p.ng_spill_entries;
-    w.spt.g = p.spt_spill + (size_t)blockIdx.x * p.spt_spill_entries;
-    w.setup_warp(smem);
-
-    for (;;) {
-        // unsigned: the output offsets below zero-extend it, so nothing about it has to be kept live across the search
-        unsigned q = 0;
-        if (lane == 0) q = atomicAdd(p.work_counter, 1u);
-        q = __shfl_sync(kFull, q, 0);
-        // the re-run launch after a hashed-set launch searches the queries on the overflow list that launch left behind
-        if (p.rerun) {
-            if (q >= p.rerun[0]) break;
-            q = p.rerun[1 + q];
-        } else if (q >= (unsigned)p.nq) {
-            break;
-        }
-
-        // ---- WorkSpace::Reset (WorkSpace.h:265-278) ----
-        if (w.vlog == nullptr) {
-            uint4* v4 = reinterpret_cast<uint4*>(w.visited);
-            const size_t n4 = p.visited_words >> 2;
-            for (size_t i = lane; i < n4; i += 32) v4[i] = make_uint4(0, 0, 0, 0);
-        }
-        w.reset_workspace(p.mres_cap);
-        // query -> shared memory (+ registers for the static-DIM variants)
-        if (PQ && p.pq_adc) {
-            // PQQuantizer::QuantizeVector with ADC on (PQQuantizer.h:141-157): table[i][j] = L2(query sub-vector i,
-            // codeword j of sub-space i), built by the warp into its slot's arena
-            const float* qrot = reinterpret_cast<const float*>(p.queries + (size_t)q * p.query_stride_bytes);
-            float* table = p.adc_tables + (size_t)blockIdx.x * p.pq_m * p.pq_ks;
-            const int total = p.pq_m * p.pq_ks;
-            for (int t = lane; t < total; t += 32) {
-                const int i = t / p.pq_ks;
-                table[t] = exact_dist_thread<false>(qrot + (size_t)i * p.pq_dsub, p.codebooks + (size_t)t * p.pq_dsub, p.pq_dsub);
-            }
-            int* qoff = reinterpret_cast<int*>(w.qs);
-            for (int i = lane; i < p.pq_m; i += 32) qoff[i] = i * p.pq_ks;
-            w.pq_table = table;
-        } else if (PQ) {
-            // the (already quantized) query: M code bytes -> row offsets of its SDC table rows
-            const unsigned char* qc = p.queries + (size_t)q * p.query_stride_bytes;
-            int* qoff = reinterpret_cast<int*>(w.qs);
-            for (int i = lane; i < p.pq_m; i += 32) qoff[i] = (i * p.pq_ks + (int)qc[i]) * p.pq_ks;
-            w.pq_table = p.sdc;
-        } else if (ELEM != 0) {
-            const unsigned char* qb = p.queries + (size_t)q * p.query_stride_bytes;
-            unsigned char* qd = reinterpret_cast<unsigned char*>(w.qs);
-            const int qbytes = p.dim * (ELEM == 3 ? 2 : 1);
-            for (int i = lane; i < qbytes; i += 32) qd[i] = qb[i];
-        } else {
-            const float* qg = reinterpret_cast<const float*>(p.queries + (size_t)q * p.query_stride_bytes);
-            // static dims that are multiples of 16 never read the shared copy in the BKT flavour (no tails, no
-            // KD split test), so those instantiations keep the query in registers only and give the 3 KB back
-            // (128-d rows: the fast path reads the query from shared memory with broadcast LDS.128 and holds no slice)
-            constexpr bool kRegsOnly = (DIM == 768) && !KDT;
-            constexpr bool kFastRows128 = (DIM == 128) && (ELEM == 0) && !PQ;
-            if (!kRegsOnly) {
-                for (int i = lane; i < p.dim; i += 32) w.qs[i] = qg[i];
-                __syncwarp();
-            }
-            if (DIM > 0 && !kFastRows128) {
-#pragma unroll
-                for (int c = 0; c < DIM / 16; ++c) w.qr.q[c] = __ldg(qg + 16 * c + (lane & 15));
-            }
-        }
-        __syncwarp();
-
-        if (KDT)
-            w.kdt_search();
-        else
-            w.bkt_search();
-
-        // log mode and hashed set: leave the bitmap / table clean for the next query of this slot (the table's log never
-        // overflows: it holds the load limit plus one row chunk)
-        if (w.vlog != nullptr) {
-            __syncwarp();
-            if (w.vlog_count <= (int)p.vlog_entries) {
-                for (int i = lane; i < w.vlog_count; i += 32) w.visited[w.vlog[i]] = 0u;
-            } else {  // the log overflowed: clear everything
-                uint4* v4 = reinterpret_cast<uint4*>(w.visited);
-                const size_t n4 = p.visited_words >> 2;
-                for (size_t i = lane; i < n4; i += 32) v4[i] = make_uint4(0, 0, 0, 0);
-            }
-            __syncwarp();
-        }
-        // hashed set filled to its limit: the result is incomplete; the re-run launch searches the query again and writes
-        // all of its outputs
-        if (w.vset_full()) {
-            if (lane == 0) p.overflow[1 + atomicAdd(p.overflow, 1u)] = q;
-            __syncwarp();
-            continue;
-        }
-        // ---- QueryResultSet::SortResult: the register list is already ascending by (dist, id) ----
-        if (w.tk != nullptr) {
-            w.res_sort();
-            for (int i = lane; i < p.k; i += 32) {
-                const int2 e = w.tk[i];
-                w.write_result(q, i, e.x, __int_as_float(e.y));
-            }
-        } else if (lane < p.k) {
-            w.write_result(q, lane, w.tk_id, w.tk_d);
-        }
-        if (p.out_stats != nullptr && lane == 0) {
-            int* s = p.out_stats + (size_t)q * kStatsPerQuery;
-            s[0] = w.checked;
-            s[1] = w.tree_checked;
-            s[2] = w.ng.count;
-            s[3] = w.spt.count;
-            s[4] = w.ndist;
-            s[5] = w.nexpand;
-            s[6] = w.ntree;
-            s[7] = 0;
-        }
-        __syncwarp();
-    }
-}
-
-// ------------------------------------------------------------------------------------------
-// ResultIterator::Next for a batch of open iterators (ResultIterator.cpp:31-55 -> SearchIndexIterativeNext,
-// BKTIndex.cpp:659-675).  Every query owns persistent arenas in HBM -- visited bitmap, NGQueue, SPTQueue (the
-// reference's rented WorkSpace) -- indexed by query, not by slot; the shared-memory queue heads are restored from and
-// flushed to those arenas around each call, and the rest of its state is an IterState.
-// p.k = the batch the caller asked for; the effective batch of a query is capped by the result count of its previous
-// call (QueryResult::SetResultNum(resultCount), ResultIterator.cpp:36-41, :52).
-// A query on a hash table that reaches the table's limit suspends (bkt_search_iterative): it saves what the call has
-// built so far, writes no outputs and joins iv.suspended; the host grows its table and launches the kernel again over
-// that list (iv.list), where the query continues from the saved state.  The visited set has exact set semantics in
-// both forms, so the results do not depend on where, or how often, a query was suspended.
-// ------------------------------------------------------------------------------------------
 // The per-query visited set of an iterator kernel: its table or bitmap, and the table's capacity
 template <typename W>
 __device__ __forceinline__ void bind_iter_visited(W& w, const SearchParams& p, const IterVisited& iv, int q, int bits) {
@@ -2083,217 +2021,15 @@ __device__ __forceinline__ void suspend_iter_query(const IterVisited& iv, int q,
     }
 }
 
-template <bool COSINE, int RPL, int ELEM>
-__global__ void __launch_bounds__(32, 12) iterate_kernel(const SearchParams p, int* __restrict__ state,
-                                                         int* __restrict__ out_counts,
-                                                         unsigned char* __restrict__ out_relaxed, const IterVisited iv) {
-    extern __shared__ __align__(128) unsigned char smem[];
-    const int lane = threadIdx.x;
-    IterState* const states = reinterpret_cast<IterState*>(state);
-    WarpSearch<0, COSINE, RPL, false, ELEM, false, true> w(p, lane);
-    w.vlog = nullptr;  // the bitmap belongs to the iterator and is never cleared between calls
-    w.setup_warp(smem);
-
-    for (;;) {
-        const int q = next_iter_query(p, iv, lane);
-        if (q < 0) break;
-        IterState& st = states[q];
-        bind_iter_visited(w, p, iv, q, st.vbits);
-        w.ng.g = p.ng_spill + (size_t)q * p.ng_spill_entries;
-        w.spt.g = p.spt_spill + (size_t)q * p.spt_spill_entries;
-        w.tk = p.topk + (size_t)q * p.topk_pad;
-        w.ng.count = st.ng_count;
-        w.spt.count = st.spt_count;
-        w.ng.tail_idx = w.spt.tail_idx = -1;
-        const int resumed = st.resume;
-        int at = resumed ? resumed : (st.first != 0 ? kIterFirst : kIterStep);
-        int relaxed = st.relaxed;
-        const int slots = st.slots;
-        const int batch = (slots < 0) ? p.k : min(p.k, slots);
-        w.restore_queue_heads();
-        w.ndist = w.nexpand = w.ntree = 0;
-        w.tree_checked = w.no_better = 0;
-        w.vlog_count = st.vfill;
-        float* saved = iv.resume ? iv.resume + (size_t)q * kIterResumeWords : nullptr;
-        int count = 0, limit = 0;
-        if (resumed) {  // the call this query suspended in: m_Results, resultCount, checked and the SearchTrees limit
-            w.mres.load(saved, lane);
-            const int* si = reinterpret_cast<const int*>(saved + 32 * RPL);
-            count = si[0];
-            w.checked = si[1];
-            limit = si[2];
-        } else {
-            // WorkSpace::ResetResult(m_iMaxCheck, batch) (WorkSpace.h:280-286)
-            w.mres.reset(max(p.max_check / 16, batch), lane);
-            w.checked = 0;
-        }
-        w.tk_count = count;
-        w.load_query_bytes(q);
-        __syncwarp();
-
-        w.bkt_search_iterative(at, batch, relaxed, count, limit, iv.margin);
-
-        __syncwarp();
-        if (at != kIterDone) {  // suspended: keep the call's state, flush the queues, no outputs yet
-            w.mres.save(saved, lane);
-            if (lane == 0) {
-                int* si = reinterpret_cast<int*>(saved + 32 * RPL);
-                si[0] = count;
-                si[1] = w.checked;
-                si[2] = limit;
-            }
-            w.flush_queue_heads();
-            if (lane == 0) {
-                st.ng_count = w.ng.count;
-                st.spt_count = w.spt.count;
-                st.relaxed = relaxed;
-                st.vfill = w.vlog_count;
-                st.resume = at;
-            }
-            suspend_iter_query(iv, q, at == kIterStep ? 1 : 2, lane);
-            __syncwarp();
-            continue;
-        }
-        // QueryResultSet::SortResult over the `count` returned entries; the rest of the caller's row is (-1, MaxDist)
-        w.res_sort();
-        for (int i = lane; i < p.k; i += 32) {
-            const int2 e = (i < count) ? w.tk[i] : make_pair(-1, SPTAG_B200_MAXDIST);
-            w.write_result(q, i, e.x, __int_as_float(e.y));
-        }
-        // flush the queue heads and the scalars
-        w.flush_queue_heads();
-        if (lane == 0) {
-            st.ng_count = w.ng.count;
-            st.spt_count = w.spt.count;
-            st.first = 0;
-            st.relaxed = relaxed;
-            st.slots = count;  // m_queryResult->SetResultNum(resultCount)
-            st.vfill = w.vlog_count;
-            st.resume = 0;
-            out_counts[q] = count;
-            out_relaxed[q] = (unsigned char)relaxed;
-        }
-        __syncwarp();
-    }
-}
-
-// ------------------------------------------------------------------------------------------
-// BKT::Index<T>::SearchIndexIterativeFromNeareast, FIRST call (BKTIndex.cpp:543-573), for a batch of freshly opened
-// iterators -- the head-index call of SPANN's iterative search (SPANNIndex.cpp:273): a full Search for the p.k nearest on
-// the query's own work-space arenas, nodeCheckStatus.clear(), then every result re-seeds NGQueue from its graph row.
-// Later calls are iterate_kernel with batch = k (the host resets the result-slot cap: the caller's QueryResult keeps
-// its size there).
-// The search is not resumable mid-way: a query whose table reaches its limit joins iv.suspended and the host runs its
-// call again from the start on a larger, empty table (exact: the iterator was freshly opened).  The host sizes the
-// tables so that the seeding (at most k x (degree + 1) inserts) stays below the limit.
-// ------------------------------------------------------------------------------------------
-template <bool COSINE, int RPL, int ELEM>
-__global__ void __launch_bounds__(32, 12) nearest_first_kernel(const SearchParams p, int* __restrict__ state,
-                                                               const IterVisited iv) {
-    extern __shared__ __align__(128) unsigned char smem[];
-    const int lane = threadIdx.x;
-    IterState* const states = reinterpret_cast<IterState*>(state);
-    WarpSearch<0, COSINE, RPL, false, ELEM, false, true> w(p, lane);
-    w.ring = smem;
-    w.cand_id = reinterpret_cast<int*>(smem + p.off_cand);
-    w.cand_dist = reinterpret_cast<float*>(smem + p.off_cand + 128);
-    w.bars = reinterpret_cast<uint64_t*>(smem + p.off_bar);
-    w.qs = reinterpret_cast<float*>(smem + p.off_query);
-    w.vlog = nullptr;
-    w.ng.s = reinterpret_cast<int2*>(smem + p.off_ng);
-    w.ng.H = p.h_ng;
-    w.ng.length = p.ng_length;
-    w.ng.lastlevel = p.ng_lastlevel;
-    w.spt.s = reinterpret_cast<int2*>(smem + p.off_spt);
-    w.spt.H = p.h_spt;
-    w.spt.length = p.spt_length;
-    w.spt.lastlevel = p.spt_lastlevel;
-    w.phase_bits = 0;
-    if (lane == 0) {
-        for (int s = 0; s < p.stages; ++s) mbar_init(&w.bars[s], 1);
-        mbar_fence_init();
-        w.ng.s[0] = make_pair(-1, SPTAG_B200_MAXDIST);
-        w.spt.s[0] = make_pair(-1, SPTAG_B200_MAXDIST);
-    }
-    __syncwarp();
-
-    for (;;) {
-        const int q = next_iter_query(p, iv, lane);
-        if (q < 0) break;
-        IterState& st = states[q];
-        bind_iter_visited(w, p, iv, q, st.vbits);  // empty: zeroed when the iterator was opened or the table was grown
-        w.ng.g = p.ng_spill + (size_t)q * p.ng_spill_entries;
-        w.spt.g = p.spt_spill + (size_t)q * p.spt_spill_entries;
-        w.tk = (p.k > 32) ? p.topk + (size_t)q * p.topk_pad : nullptr;
-        // the rented WorkSpace after Reset(MaxCheck, k) + ResetResult(MaxCheck, k)
-        w.vlog_count = 0;
-        w.ng.count = 0;
-        w.spt.count = 0;
-        w.ng.tail_idx = w.spt.tail_idx = -1;
-        w.mres.reset(max(p.max_check / 16, p.k), lane);
-        w.tk_d = SPTAG_B200_MAXDIST;
-        w.tk_id = -1;
-        w.worst_d = SPTAG_B200_MAXDIST;
-        w.worst_id = -1;
-        if (w.tk != nullptr) w.res_reset();
-        w.checked = w.ndist = w.nexpand = w.ntree = 0;
-        w.tree_checked = w.no_better = 0;
-        {
-            const unsigned char* qb = p.queries + (size_t)q * p.query_stride_bytes;
-            unsigned char* qd = reinterpret_cast<unsigned char*>(w.qs);
-            const int qbytes = p.dim * (ELEM == 0 ? 4 : (ELEM == 3 ? 2 : 1));
-            for (int i = lane; i < qbytes; i += 32) qd[i] = qb[i];
-        }
-        __syncwarp();
-
-        w.bkt_search();  // SearchIndex(query, workspace, p_searchDeleted, searchDuplicated = true)
-
-        __syncwarp();
-        if (w.vset_full()) {  // the table filled: run the whole call again on a larger one
-            suspend_iter_query(iv, q, 0, lane);
-            __syncwarp();
-            continue;
-        }
-        if (w.tk != nullptr) w.res_sort();
-        // p_space->nodeCheckStatus.clear(): other nodes may be traversed again after the top k were found
-        {
-            uint4* v4 = reinterpret_cast<uint4*>(w.visited);
-            const size_t n4 = w.qmask ? (w.qmask + 1u) >> 2 : p.visited_words >> 2;
-            for (size_t i = lane; i < n4; i += 32) v4[i] = make_uint4(0, 0, 0, 0);
-        }
-        w.vlog_count = 0;
-        __syncwarp();
-        for (int i = 0; i < p.k; ++i) {
-            int rid;
-            float rd;
-            if (w.tk != nullptr) {
-                const int2 e = w.tk[i];
-                rid = e.x;
-                rd = __int_as_float(e.y);
-            } else {
-                rid = __shfl_sync(kFull, w.tk_id, i);
-                rd = __shfl_sync(kFull, w.tk_d, i);
-            }
-            if (lane == 0) {
-                p.out_ids[(size_t)q * p.k + i] = (rid >= 0) ? rid + p.id_offset : rid;
-                p.out_dists[(size_t)q * p.k + i] = rd;
-            }
-            if (rid < 0) continue;
-            w.seed_from_result(rid);
-        }
-        // flush the queue heads and the scalars
-        __syncwarp();
-        for (int i = 1 + lane; i <= min(w.ng.count, w.ng.H); i += 32) w.ng.g[i] = w.ng.s[i];
-        for (int i = 1 + lane; i <= min(w.spt.count, w.spt.H); i += 32) w.spt.g[i] = w.spt.s[i];
-        if (lane == 0) {
-            st.ng_count = w.ng.count;
-            st.spt_count = w.spt.count;
-            st.first = 0;
-            st.slots = -1;
-            st.vfill = w.vlog_count;
-        }
-        __syncwarp();
-    }
-}
+// The kernels: search_kernel, iterate_kernel and nearest_first_kernel as they are, and the same text in namespace bfs with
+// breadth-first tree seeding (EnableBfs != 0), instantiated for the generic-dimension, integer and PQ rows only
+#define SPTAG_B200_BFS false
+#include "search_kernel_defs.cuh"
+#undef SPTAG_B200_BFS
+namespace bfs {
+#define SPTAG_B200_BFS true
+#include "search_kernel_defs.cuh"
+#undef SPTAG_B200_BFS
+}  // namespace bfs
 
 }  // namespace sptag_b200

@@ -114,6 +114,7 @@ struct sptag_b200_index {
     int search_deleted = 0;   // handle-wide default of p_searchDeleted (parameter "SearchDeleted"); per-call value: sptag_b200_search_ex
     // search parameters (reference names)
     int max_check = 8192, max_check_refine = 8192, initial_pivots = 50, other_pivots = 4, no_better_threshold = 3;
+    int bfs = 0;  // EnableBfs (BKT only): != 0 seeds each tree breadth-first (BKTree.h:703-758)
     // graph-update parameters (reference names, BKT/ParameterDefinitionList.h:28-31): AddIndex's refine budget, the
     // result count of DeleteIndex(vectors), RebuildNeighbors' factor
     int add_cef = 500, cef = 1000;
@@ -228,12 +229,22 @@ int heap_lastlevel(int size) {
     return (int)std::pow(2.0, std::floor(std::log2((float)size)));
 }
 
+// EnableBfs is in force: a BKT handle with a non-zero value.  Its searches take the bfs:: kernels.
+bool bfs_seeding(const sptag_b200_index* h) { return h->algo == SPTAG_B200_ALGO_BKT && h->bfs != 0; }
+
 // The kernel instantiation for this index / parameter set (nullptr: unsupported m_Results capacity); the
 // instantiations live in kern_*.cu (kernel_select.h)
 SearchKernelFn pick_kernel(const sptag_b200_index* h, int mres_cap, int slots = 0) {
     const bool kdt = (h->algo == SPTAG_B200_ALGO_KDT);
-    if (h->q_type != 0) return pick_pq_kernel(mres_cap);  // quantized: BKT + L2 only (PQQuantizer.h:130-136)
     const bool l2 = (h->metric == SPTAG_B200_METRIC_L2);
+    if (bfs_seeding(h)) {
+        if (h->q_type != 0) return pick_pq_bfs_kernel(mres_cap);
+        if (h->value_type == SPTAG_B200_VT_INT8) return pick_int8_bfs_kernel(false, !l2, mres_cap);
+        if (h->value_type == SPTAG_B200_VT_UINT8) return pick_int8_bfs_kernel(true, !l2, mres_cap);
+        if (h->value_type == SPTAG_B200_VT_INT16) return pick_int16_bfs_kernel(!l2, mres_cap);
+        return l2 ? pick_float_bfs_kernel_l2(mres_cap) : pick_float_bfs_kernel_cosine(mres_cap);
+    }
+    if (h->q_type != 0) return pick_pq_kernel(mres_cap);  // quantized: BKT + L2 only (PQQuantizer.h:130-136)
     if (h->value_type == SPTAG_B200_VT_INT8) return pick_int8_kernel(false, !l2, mres_cap, kdt);
     if (h->value_type == SPTAG_B200_VT_UINT8) return pick_int8_kernel(true, !l2, mres_cap, kdt);
     if (h->value_type == SPTAG_B200_VT_INT16) return pick_int16_kernel(!l2, mres_cap, kdt);
@@ -344,6 +355,7 @@ void fill_params(const sptag_b200_index* h, int k, const CallOpts& opts, SearchP
     p.initial_pivots = h->initial_pivots;
     p.other_pivots = h->other_pivots;
     p.no_better_threshold = h->no_better_threshold;
+    p.bfs = bfs_seeding(h) ? h->bfs : 0;
     // a fresh thread's WorkSpace: Initialize(max(MaxCheck, MaxCheckForRefineGraph)) then
     // Reset(MaxCheck, K) (BKTIndex.cpp:600-605, WorkSpace.h:243-278)
     const int alloc_check = std::max(eff_max_check, h->max_check_refine);
@@ -365,6 +377,7 @@ void fill_params(const sptag_b200_index* h, int k, const CallOpts& opts, SearchP
     // (even entry counts keep every slot's arena 16-byte aligned for the paired child loads)
     p.ng_spill_entries = round_up((size_t)std::min<long long>((long long)p.ng_length, (long long)h->n + 2) + 2, 2);
     p.spt_spill_entries = round_up((size_t)std::min<long long>((long long)p.spt_length, (long long)h->node_count + 2) + 2, 2);
+    if (p.bfs) p.spt_spill_entries += 2 * kBfsHeapEntries;  // the two BFS heaps (WarpSearch::bfs_heap)
     const bool use_log = h->visited_log < 0 ? (p.visited_words * 4 > 256 * 1024) : (h->visited_log != 0);
     if (use_log) {
         const size_t entries = h->visited_log_entries > 0 ? (size_t)h->visited_log_entries
@@ -404,8 +417,8 @@ int lay_out(const sptag_b200_index* h, int nq, SearchLaunch& L) {
         p.slot_stride = (int)(p.slot_stagger ? a : b);
     }
     // 512-byte float rows run the fixed-shape fast path (search_kernels.cuh kFast): 2 stages x 8 rows, slots 576 B apart;
-    // must mirror WarpSearch::kFast
-    const bool fast128 = !pq && h->value_type == SPTAG_B200_VT_FLOAT && h->dim == 128 && h->simd_width == 16;
+    // must mirror WarpSearch::kFast (BFS seeding runs the generic-dimension kernels)
+    const bool fast128 = !p.bfs && !pq && h->value_type == SPTAG_B200_VT_FLOAT && h->dim == 128 && h->simd_width == 16;
     // ... with register-capped kernel variants for more than 16 query slots per SM (B200.QueriesPerSM); those run a
     // one-stage ring (B200.Stages = 1 selects it at any residency) so that the slot's shared memory still fits
     // Default residency for 512-byte rows: all warps start together and a query costs about the same for every warp,
@@ -459,7 +472,7 @@ int lay_out(const sptag_b200_index* h, int nq, SearchLaunch& L) {
         p.off_bar = (int)off;
         off += round_up((size_t)stages * 8, 16);
         p.off_query = (int)off;
-        const bool query_in_regs_only = !pq && h->value_type == SPTAG_B200_VT_FLOAT && h->algo == SPTAG_B200_ALGO_BKT &&
+        const bool query_in_regs_only = !p.bfs && !pq && h->value_type == SPTAG_B200_VT_FLOAT && h->algo == SPTAG_B200_ALGO_BKT &&
                                         h->dim == 768 && h->simd_width == 16;  // must mirror kRegsOnly in search_kernel
         off += query_in_regs_only ? 16 : round_up((size_t)h->dim * 4 + 16, 16);  // float query, or M row offsets for PQ
         L.smem = round_up(off, 128);
@@ -751,6 +764,23 @@ int grow_iter_visited(sptag_b200_iterator* it, const std::vector<unsigned>& qs, 
     it->vbufs.push_back(std::move(buf));
     it->vbuf_refs.push_back((int)qs.size());
     return 0;
+}
+
+// The first Next of an iterator on hash tables with EnableBfs = bfs > 0: the breadth-first seeding cannot suspend, and it
+// inserts at most MaxBFSNodes centres per level and tree.  Tables below that limit are replaced by empty ones that hold it
+// (still empty: nothing has run), or by bitmaps where such a table would be larger.  Caller holds h->mu.
+int fit_bfs_seeding(sptag_b200_iterator* it, int bfs) {
+    const long long seeds = std::min<long long>((long long)kBfsMaxNodes * bfs * it->h->tree_num, (long long)it->h->n + 1);
+    int need = 6;
+    while (need < 31 && ((long long)1 << (need - 1)) < seeds) ++need;
+    std::vector<unsigned> qs;
+    std::vector<int> bits;
+    for (int q = 0; q < it->nq; ++q)
+        if (it->q_bits[q] != 0 && it->q_bits[q] < need) {
+            qs.push_back((unsigned)q);
+            bits.push_back(need);
+        }
+    return qs.empty() ? 0 : grow_iter_visited(it, qs, bits, false, nullptr);
 }
 
 // Run one iterator step planned by plan_iterator_step.  The iterator's queue lengths and per-query arenas replace the
@@ -1222,11 +1252,6 @@ int sptag_b200_load(const char* folder, int32_t device, int32_t id_offset, sptag
     const std::string dm = get("DistCalcMethod", "Cosine");  // reference default is Cosine
     sh.metric = (dm == "L2") ? SPTAG_B200_METRIC_L2
                              : (dm == "InnerProduct" ? SPTAG_B200_METRIC_INNERPRODUCT : SPTAG_B200_METRIC_COSINE);
-    // the kernels implement the default seeding only (BKTree.h:696-769 with m_bfs == 0); a BFS-seeded index would
-    // return different neighbours than the reference, so refuse it
-    if (std::atoi(get("EnableBfs", "0").c_str()) != 0)
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "EnableBfs != 0 (BFS tree seeding, BKTree.h:703-758) is not built");
-
     FileCloser fc;
     FILE* fv = fc.open(dir + "/" + get("VectorFilePath", "vectors.bin"));
     FILE* fg = fc.open(dir + "/" + get("GraphFilePath", "graph.bin"));
@@ -1299,9 +1324,10 @@ int sptag_b200_load(const char* folder, int32_t device, int32_t id_offset, sptag
     }
     static const char* names[] = {"MaxCheck", "MaxCheckForRefineGraph", "NumberOfInitialDynamicPivots",
                                   "NumberOfOtherDynamicPivots", "ThresholdOfNumberOfContinuousNoBetterPropagation",
-                                  "AddCEF", "CEF", "RNGFactor"};
+                                  "AddCEF", "CEF", "RNGFactor", "EnableBfs"};
     for (const char* nm : names) {
         auto it = kv.find(nm);
+        // (EnableBfs is a BKT parameter: set_param refuses it on a KDT handle, and the KDT loader ignores the key)
         if (it != kv.end()) sptag_b200_set_param(h, nm, it->second.c_str());
     }
     *out = h;
@@ -1394,6 +1420,7 @@ int sptag_b200_set_param(sptag_b200_handle h, const char* name, const char* valu
     else if (n == "NumberOfInitialDynamicPivots") h->initial_pivots = (int)v;
     else if (n == "NumberOfOtherDynamicPivots") h->other_pivots = (int)v;
     else if (n == "ThresholdOfNumberOfContinuousNoBetterPropagation") h->no_better_threshold = (int)v;
+    else if (n == "EnableBfs" && h->algo == SPTAG_B200_ALGO_BKT) h->bfs = (int)v;  // any int, like BKTree::m_bfs
     else if (n == "B200.QueriesPerSM") h->queries_per_sm = (int)v;
     else if (n == "B200.StageRows") h->stage_rows = (int)v;
     else if (n == "B200.Stages") { h->stages = (int)v; h->stages_set = true; }
@@ -1446,6 +1473,7 @@ int sptag_b200_get_param(sptag_b200_handle h, const char* name, char* value_out,
     else if (n == "NumberOfInitialDynamicPivots") v = h->initial_pivots;
     else if (n == "NumberOfOtherDynamicPivots") v = h->other_pivots;
     else if (n == "ThresholdOfNumberOfContinuousNoBetterPropagation") v = h->no_better_threshold;
+    else if (n == "EnableBfs" && h->algo == SPTAG_B200_ALGO_BKT) v = h->bfs;
     else if (n == "B200.QueriesPerSM") v = h->queries_per_sm;
     else if (n == "B200.StageRows") v = h->stage_rows;
     else if (n == "B200.Stages") v = h->stages;
@@ -1790,7 +1818,8 @@ int sptag_b200_iterator_open_ex(sptag_b200_handle h, const void* queries, int32_
     // SearchIndexIterativeFromNeareast's nodeCheckStatus.clear() the leftovers of the finished search stay queued while
     // every node may enter once more, so 2 (n + 2) is the bound; Heap::insert itself stops at `length`
     it->ng_entries = round_up((size_t)std::min<long long>((long long)p.ng_length, 2 * ((long long)h->n + 2)) + 2, 2);
-    it->spt_entries = p.spt_spill_entries;
+    // (with room for the two BFS heaps whatever EnableBfs is now: the value in force at the first Next decides)
+    it->spt_entries = p.spt_spill_entries + (p.bfs ? 0 : 2 * kBfsHeapEntries);
     const size_t qbytes = (size_t)num_queries * query_bytes(h);
     int rc = 0;
     if ((rc = it->d_queries.ensure(qbytes)) || (rc = it->d_ng.ensure((size_t)num_queries * it->ng_entries * 8)) ||
@@ -1876,8 +1905,12 @@ int sptag_b200_iterator_next(sptag_b200_iter it, int32_t batch, int32_t* out_ids
     DeviceGuard guard(h->device);
     SearchLaunch L;
     if (int rc = plan_iterator_step(it, batch, L)) return rc;
-    IterateKernelFn kern = pick_iterate_kernel_for(h->value_type, h->metric != SPTAG_B200_METRIC_L2, L.p.mres_cap);
+    const bool cosine = h->metric != SPTAG_B200_METRIC_L2;
+    IterateKernelFn kern = L.p.bfs ? pick_iterate_bfs_kernel_for(h->value_type, cosine, L.p.mres_cap)
+                                   : pick_iterate_kernel_for(h->value_type, cosine, L.p.mres_cap);
     if (!kern) return fail(SPTAG_B200_LACK_OF_INPUTS, "max(MaxCheck/16, batch) = %d exceeds the supported 1024", L.p.mres_cap);
+    if (!it->stepped && it->nearest_k == 0 && it->hashed && L.p.bfs > 0)
+        if (int rc = fit_bfs_seeding(it, L.p.bfs)) return rc;
     return run_iterator_step(it, batch, "batch", L, out_ids, out_dists, out_counts, out_relaxed_mono, false,
                              [&](const SearchParams& p, int grid, size_t smem, cudaStream_t stream, const IterVisited& iv) {
                                  CUDA_OK(cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1903,8 +1936,10 @@ int sptag_b200_iterator_next_from_nearest(sptag_b200_iter it, int32_t k, int32_t
     SearchLaunch L;
     if (int rc = plan_iterator_step(it, k, L)) return rc;
     const bool cosine = h->metric != SPTAG_B200_METRIC_L2;
-    NearestFirstKernelFn kfirst = pick_nearest_first_kernel_for(h->value_type, cosine, L.p.mres_cap);
-    IterateKernelFn knext = pick_iterate_kernel_for(h->value_type, cosine, L.p.mres_cap);
+    NearestFirstKernelFn kfirst = L.p.bfs ? pick_nearest_first_bfs_kernel_for(h->value_type, cosine, L.p.mres_cap)
+                                          : pick_nearest_first_kernel_for(h->value_type, cosine, L.p.mres_cap);
+    IterateKernelFn knext = L.p.bfs ? pick_iterate_bfs_kernel_for(h->value_type, cosine, L.p.mres_cap)
+                                    : pick_iterate_kernel_for(h->value_type, cosine, L.p.mres_cap);
     if (!kfirst || !knext)
         return fail(SPTAG_B200_LACK_OF_INPUTS, "max(MaxCheck/16, k) = %d exceeds the supported 1024", L.p.mres_cap);
     if (first && it->hashed) {
@@ -2464,7 +2499,9 @@ int sptag_b200_save(sptag_b200_handle h, const char* folder) {
             "NumberOfOtherDynamicPivots=%d\n",
             bkt ? "BKT" : "KDT", value_type_name(h->value_type), h->degree, h->cef, h->add_cef, h->max_check_refine,
             h->rng_factor, metric, h->max_check, h->no_better_threshold, h->initial_pivots, h->other_pivots);
-        ok = w > 0 && std::fclose(f) == 0 && ok;
+        // written only when set, so that the folders of handles without it stay as they were
+        const int wb = (bkt && h->bfs != 0) ? std::fprintf(f, "EnableBfs=%d\n", h->bfs) : 1;
+        ok = w > 0 && wb > 0 && std::fclose(f) == 0 && ok;
     } else ok = false;
     if (!ok) return fail(SPTAG_B200_FAIL, "cannot write the index files in %s", folder);
     return SPTAG_B200_SUCCESS;

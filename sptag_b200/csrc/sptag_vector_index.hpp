@@ -413,8 +413,9 @@ private:
     }
 
     void PushSearchParameters() const {
+        // (EnableBfs: BKT only -- a KDT index has no such parameter, and the device refuses it there)
         static const char* names[] = {"MaxCheck", "MaxCheckForRefineGraph", "NumberOfInitialDynamicPivots", "NumberOfOtherDynamicPivots",
-                                      "ThresholdOfNumberOfContinuousNoBetterPropagation"};
+                                      "ThresholdOfNumberOfContinuousNoBetterPropagation", "EnableBfs"};
         for (const char* nm : names) {
             const std::string v = m_cpu->GetParameter(nm, "Index");
             if (!v.empty()) sptag_b200_set_param(m_handle, nm, v.c_str());
