@@ -361,6 +361,42 @@ int sptag_b200_add(sptag_b200_handle h, const void* vectors, int32_t num, int32_
  * if needed.  Quantized handles: LackOfInputs (the quantizer blob is not kept). */
 int sptag_b200_save(sptag_b200_handle h, const char* folder);
 
+/* ---- SPANN with its posting lists in HBM ----
+ * Replaces: VectorIndex::LoadIndex(folder) for a SPANN folder (VectorIndex.cpp:617-681, SPANN::Index<T>::LoadConfig /
+ * LoadIndexData, SPANNIndex.cpp:59-140, ExtraFullGraphSearcher::LoadIndex / LoadingHeadInfo, ExtraFullGraphSearcher.h:
+ * 163-220, :1030-1120).  Reads indexloader.ini ([Base] ValueType, HeadIndexFolder, HeadVectorIDs; [BuildSSDIndex]
+ * SSDIndex, SearchInternalResultNum, MaxDistRatio, SearchPostingPageLimit, PostingVectorLimit,
+ * EnablePostingListRearrange), loads the head folder with sptag_b200_load and applies the [BuildHead] search parameters
+ * to it as SPANN::Index::SetParameter does (:1033-1038), reads the translate map and every posting file (SSDIndex,
+ * SSDIndex_1, ...) in the plain or the rearranged layout, and packs the lists into HBM.  Each list keeps its full element
+ * count; SearchPostingPageLimit truncates at search time.  Section and parameter names are read case-insensitively, as
+ * Helper::IniReader reads them.  LackOfInputs for EnableDataCompression, EnableDeltaEncoding and quantized SPANN.  Device
+ * memory: the packed lists (rows at the head's row stride, one int32 id each), plus during the load a staging buffer of
+ * at most 64 MB (or the largest list, if larger); MemoryOverFlow when that does not fit. */
+typedef struct sptag_b200_spann* sptag_b200_spann_handle;
+int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_handle* out);
+void sptag_b200_spann_destroy(sptag_b200_spann_handle s);
+
+/* Replaces: SPANN::Index<T>::SearchIndex(QueryResult&) (SPANNIndex.cpp:193-250) with ExtraFullGraphSearcher::SearchIndex
+ * (ExtraFullGraphSearcher.h:226-375) for a batch.  The head search runs at W = max(K, SearchInternalResultNum); the
+ * postings are chosen from its results, the result array is reversed, every chosen list is scanned in order with the
+ * deduper, the head's distance function and QueryResultSet::AddPoint, and SortResult orders the array
+ * (QueryResultSet.h:77-112); the first K entries are returned.  Results equal the reference's bit for bit.
+ * queries: HOST, num_queries x dim of the value type.  out_ids / out_dists: HOST [num_queries x k].  out_stats: HOST
+ * [num_queries x 3] int32 or NULL: postings scanned (m_diskIOCount), list elements read (m_totalListElementsCount),
+ * distances computed.  k <= 2048.  Thread-safe; two callers overlap.  LackOfInputs when the page limit truncates lists
+ * of the rearranged layout (the reference then reads ids from an offset computed with the truncated count,
+ * ExtraFullGraphSearcher.h:1186-1190, which is not reproduced). */
+int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int32_t num_queries, int32_t k, int32_t* out_ids,
+                            float* out_dists, int32_t* out_stats);
+
+/* Replaces: SPANN::Index<T>::SetParameter / GetParameter (SPANNIndex.cpp:1033-1073) for SearchInternalResultNum,
+ * MaxDistRatio (a float), SearchPostingPageLimit (raised at search time to the pages of PostingVectorLimit vectors, as
+ * ExtraFullGraphSearcher::LoadIndex does, :167) and MaxCheck (the head's).  Read-only: PostingBytes (device bytes of the
+ * posting lists and the translate map). */
+int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, const char* value);
+int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char* value_out, int32_t capacity);
+
 /* Labelset::Count(): tombstones set so far. */
 int32_t sptag_b200_num_deleted(sptag_b200_handle h);
 

@@ -30,7 +30,8 @@ EXPORTS = [
     "sptag_b200_iterator_next_from_nearest", "sptag_b200_search_ex", "sptag_b200_iterator_open_ex",
     "sptag_b200_refine_search", "sptag_b200_refine_schedule", "sptag_b200_rebuild_graph", "sptag_b200_group_create", "sptag_b200_group_search",
     "sptag_b200_group_destroy", "sptag_b200_add", "sptag_b200_delete", "sptag_b200_delete_vectors", "sptag_b200_save",
-    "sptag_b200_num_deleted",
+    "sptag_b200_num_deleted", "sptag_b200_spann_load", "sptag_b200_spann_destroy", "sptag_b200_spann_search",
+    "sptag_b200_spann_set_param", "sptag_b200_spann_get_param",
 ]
 
 
@@ -107,6 +108,12 @@ def lib():
         L.sptag_b200_num_deleted.argtypes = [C.c_void_p]
         L.sptag_b200_last_kernel_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
         L.sptag_b200_launch_count.restype = C.c_int64
+        L.sptag_b200_spann_load.argtypes = [C.c_char_p, C.c_int32, C.POINTER(C.c_void_p)]
+        L.sptag_b200_spann_destroy.argtypes = [C.c_void_p]
+        L.sptag_b200_spann_destroy.restype = None
+        L.sptag_b200_spann_search.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.sptag_b200_spann_set_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p]
+        L.sptag_b200_spann_get_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_int32]
         for f in ("num_vectors", "dim", "value_type", "metric", "algo"):
             getattr(L, "sptag_b200_" + f).argtypes = [C.c_void_p]
         L.sptag_b200_last_error.restype = C.c_char_p
@@ -432,3 +439,50 @@ def merge_topk(device, d_ids_ptr, d_dists_ptr, num_lists, nq, k, d_out_ids_ptr, 
 
 def launch_count():
     return int(lib().sptag_b200_launch_count())
+
+
+class B200SpannIndex:
+    """Handle to a SPANN index whose head and posting lists live in HBM (SPANN::Index<T>: LoadIndex, SearchIndex)."""
+
+    STATS_PER_QUERY = 3  # postings scanned, list elements read, distances computed
+
+    def __init__(self, handle):
+        self._h = C.c_void_p(handle)
+
+    @classmethod
+    def load(cls, folder, device=-1):
+        """VectorIndex::LoadIndex(folder) for a SPANN folder."""
+        h = C.c_void_p()
+        _check(lib().sptag_b200_spann_load(os.fsencode(folder), device, C.byref(h)))
+        return cls(h.value)
+
+    def close(self):
+        if self._h:
+            lib().sptag_b200_spann_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_param(self, name, value):
+        """SearchInternalResultNum, MaxDistRatio, SearchPostingPageLimit, MaxCheck (the head's)."""
+        _check(lib().sptag_b200_spann_set_param(self._h, name.encode(), str(value).encode()))
+
+    def get_param(self, name):
+        buf = C.create_string_buffer(64)
+        _check(lib().sptag_b200_spann_get_param(self._h, name.encode(), buf, 64))
+        return buf.value.decode()
+
+    def search(self, queries, k, want_stats=False):
+        """SPANN::Index::SearchIndex for a batch of HOST queries: ids [nq, k], dists [nq, k] (and stats [nq, 3])."""
+        queries = np.ascontiguousarray(queries)
+        nq = queries.shape[0]
+        ids = np.empty((nq, k), np.int32)
+        dists = np.empty((nq, k), np.float32)
+        stats = np.zeros((nq, self.STATS_PER_QUERY), np.int32) if want_stats else None
+        _check(lib().sptag_b200_spann_search(self._h, queries.ctypes.data, nq, k, ids.ctypes.data, dists.ctypes.data,
+                                             stats.ctypes.data if want_stats else None))
+        return (ids, dists, stats) if want_stats else (ids, dists)

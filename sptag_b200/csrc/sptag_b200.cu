@@ -8,9 +8,11 @@
 #include "../../include/sptag_b200.h"
 #include "aux_kernels.cuh"
 #include "kernel_select.h"
+#include "spann_scan.h"
 
 #include <algorithm>
 #include <atomic>
+#include <cctype>
 #include <cfloat>
 #include <climits>
 #include <cmath>
@@ -2511,6 +2513,482 @@ int32_t sptag_b200_num_deleted(sptag_b200_handle h) {
     if (!h) return 0;
     std::lock_guard<std::mutex> lock(h->mu);  // written by the delete calls under the same lock
     return h->num_deleted;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------
+// SPANN with its posting lists in HBM (SPANN::Index<T>, SPANNIndex.cpp; ExtraFullGraphSearcher.h).  The head is an
+// ordinary handle loaded by sptag_b200_load; the lists are packed into one id array and one array of rows padded to the
+// head's row stride, with one element offset per list.  The search runs the head search kernels at width W, then the
+// posting scan kernel (kern_spann.cu).
+// ---------------------------------------------------------------------------------------------------------------
+struct sptag_b200_spann {
+    sptag_b200_index* head = nullptr;
+    int vis = 0;          // m_vectorInfoSize: dim * sizeof(T) + sizeof(int)
+    int rearranged = 0;   // EnablePostingListRearrange
+    int num_lists = 0;
+    std::vector<int> cnt, pages;  // per list: full element count, page count (host copies for the table size)
+    // search parameters (SPANN/ParameterDefinitionList.h:110-117)
+    int internal = 64;
+    float max_dist_ratio = 10000.0f;
+    int page_limit = 3;       // SearchPostingPageLimit as set
+    int vector_limit_pages = 0;  // ceil(PostingVectorLimit * vis / PageSize): the least page limit in force
+    int longest = 0;          // spann_update_shape
+    bool truncated = false;
+    DeviceBuffer d_translate, d_off, d_cnt, d_pages, d_ids, d_rows;
+    // Host-buffer calls run on one of two staging sets, each with its own stream, head results, dedup tables and outputs,
+    // so that two callers overlap; the head search kernels are ordered by the head handle (search_device_impl)
+    struct Staging {
+        std::mutex mu;
+        cudaStream_t stream = nullptr;
+        DeviceBuffer d_q, d_qpad, d_hids, d_hdists, d_ids, d_dists, d_stats, d_tables;
+    } staging[2];
+    std::atomic<unsigned> staging_rr{0};
+    std::mutex mu;  // the search parameters
+};
+
+namespace {
+
+// The page limit a search uses: LoadIndex raises SearchPostingPageLimit to the pages of PostingVectorLimit vectors
+// (ExtraFullGraphSearcher.h:167)
+int spann_page_limit(const sptag_b200_spann* s) { return std::max(s->page_limit, s->vector_limit_pages); }
+
+// Elements of list l that a search reads (LoadingHeadInfo, ExtraFullGraphSearcher.h:1093-1097)
+int spann_searched(const sptag_b200_spann* s, int l, int limit) {
+    return (int)std::min<long long>(s->cnt[l], ((long long)std::min(s->pages[l], limit) << 12) / s->vis);
+}
+
+// indexloader.ini as Helper::IniReader reads it (SimpleIniReader.cpp:40-135): [Section] headers and Name=Value lines,
+// section and parameter names trimmed and lower-cased; values trimmed here too
+typedef std::map<std::string, std::map<std::string, std::string>> IniSections;
+std::string trim(const std::string& v) {
+    const size_t a = v.find_first_not_of(" \t\r");
+    if (a == std::string::npos) return std::string();
+    return v.substr(a, v.find_last_not_of(" \t\r") + 1 - a);
+}
+std::string lower(std::string v) {
+    for (char& c : v) c = (char)std::tolower((unsigned char)c);
+    return v;
+}
+bool read_ini(const std::string& path, IniSections& out) {
+    std::ifstream ini(path);
+    if (!ini) return false;
+    std::string line, section;
+    while (std::getline(ini, line)) {
+        line = trim(line);
+        if (line.empty() || line[0] == ';' || line[0] == '#') continue;
+        if (line[0] == '[') {
+            const size_t close = line.find(']');
+            section = lower(trim(line.substr(1, close == std::string::npos ? std::string::npos : close - 1)));
+            continue;
+        }
+        const size_t eq = line.find('=');
+        if (eq != std::string::npos) out[section][lower(trim(line.substr(0, eq)))] = trim(line.substr(eq + 1));
+    }
+    return true;
+}
+std::string ini_get(const IniSections& ini, const char* section, const char* name, const std::string& def) {
+    auto s = ini.find(lower(section));
+    if (s == ini.end()) return def;
+    auto it = s->second.find(lower(name));
+    return it == s->second.end() ? def : it->second;
+}
+
+bool ini_true(const std::string& v) { return lower(v) == "true" || v == "1"; }
+
+// The longest list a search reads at the page limit in force, and whether that limit truncates any list (recomputed when
+// the limit changes).  Caller holds s->mu.
+void spann_update_shape(sptag_b200_spann* s) {
+    const int limit = spann_page_limit(s);
+    s->longest = 0;
+    s->truncated = false;
+    for (int l = 0; l < s->num_lists; ++l) {
+        const int tc = spann_searched(s, l, limit);
+        s->longest = std::max(s->longest, tc);
+        s->truncated = s->truncated || tc < s->cnt[l];
+    }
+}
+
+// One posting file (OutputSSDIndexFile, ExtraFullGraphSearcher.h:1292-1420; read as LoadingHeadInfo does, :1030-1120):
+// int32 listCount, totalDocCount, dim, listPageOffset; per list int32 pageNum, uint16 pageOffset, int32 listEleCount,
+// uint16 listPageCount; list l's bytes start at ((listPageOffset + pageNum) << 12) + pageOffset
+struct PostingFile {
+    FILE* f = nullptr;
+    int lists = 0, dim = 0;
+    std::vector<long long> start;
+    std::vector<int> cnt, pages;
+};
+int read_posting_header(FILE* f, PostingFile& pf, const char* name) {
+    int32_t hdr[4];
+    if (std::fread(hdr, 4, 4, f) != 4) return fail(SPTAG_B200_FAIL, "posting file %s: truncated header", name);
+    pf.f = f;
+    pf.lists = hdr[0];
+    pf.dim = hdr[2];
+    if (pf.lists < 0) return fail(SPTAG_B200_FAIL, "posting file %s: bad list count %d", name, pf.lists);
+    const long long fsz = file_size(f);
+    fseeko(f, 16, SEEK_SET);
+    pf.start.resize((size_t)pf.lists);
+    pf.cnt.resize((size_t)pf.lists);
+    pf.pages.resize((size_t)pf.lists);
+    for (int i = 0; i < pf.lists; ++i) {
+        unsigned char b[12];
+        if (std::fread(b, 1, 12, f) != 12) return fail(SPTAG_B200_FAIL, "posting file %s: truncated list infos", name);
+        int32_t page_num, ele;
+        uint16_t page_off, page_cnt;
+        memcpy(&page_num, b, 4);
+        memcpy(&page_off, b + 4, 2);
+        memcpy(&ele, b + 6, 4);
+        memcpy(&page_cnt, b + 10, 2);
+        if (ele < 0) return fail(SPTAG_B200_FAIL, "posting file %s: list %d has %d elements", name, i, ele);
+        pf.start[i] = (((long long)hdr[3] + page_num) << 12) + page_off;
+        pf.cnt[i] = ele;
+        pf.pages[i] = page_cnt;
+        if (pf.start[i] < 0 || pf.start[i] > fsz) return fail(SPTAG_B200_FAIL, "posting file %s: list %d outside the file", name, i);
+    }
+    return 0;
+}
+
+
+// Everything sptag_b200_spann_load reads after the head: the head's [BuildHead] parameters, the search parameters, the
+// translate map and the posting files.  The caller destroys s on failure.
+int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& ini) {
+    auto get = [&](const char* section, const char* name, const char* def) { return ini_get(ini, section, name, def); };
+    sptag_b200_handle head = s->head;
+    // SPANN::Index::LoadConfig hands every [BuildHead] entry to the head (SPANNIndex.cpp:59-71, :1033-1038)
+    static const char* head_names[] = {"MaxCheck", "NumberOfInitialDynamicPivots", "NumberOfOtherDynamicPivots",
+                                       "ThresholdOfNumberOfContinuousNoBetterPropagation", "EnableBfs"};
+    for (const char* nm : head_names) {
+        const std::string v = get("BuildHead", nm, "");
+        if (!v.empty()) sptag_b200_set_param(head, nm, v.c_str());
+    }
+    s->vis = head->dim * (int)value_size(head->value_type) + 4;
+    s->rearranged = ini_true(get("BuildSSDIndex", "EnablePostingListRearrange", "false")) ? 1 : 0;
+    s->internal = atoi(get("BuildSSDIndex", "SearchInternalResultNum", "64").c_str());
+    s->max_dist_ratio = strtof(get("BuildSSDIndex", "MaxDistRatio", "10000").c_str(), nullptr);
+    s->page_limit = atoi(get("BuildSSDIndex", "SearchPostingPageLimit", "3").c_str());
+    const long long vector_limit = atoll(get("BuildSSDIndex", "PostingVectorLimit", "118").c_str());
+    s->vector_limit_pages = (int)((vector_limit * s->vis + 4095) / 4096);
+    DeviceGuard guard(head->device);
+    for (auto& st : s->staging)
+        if (cudaStreamCreate(&st.stream) != cudaSuccess) return fail(SPTAG_B200_FAIL, "cudaStreamCreate failed");
+    cudaStream_t up = s->staging[0].stream;
+    // m_vectorTranslateMap: one uint64 per head (SPANNIndex.cpp:133-134), kept as the SizeType the search casts it to
+    {
+        FileCloser fc;
+        const std::string path = dir + "/" + get("Base", "HeadVectorIDs", "SPTAGHeadVectorIDs.bin");
+        FILE* f = fc.open(path);
+        if (!f) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot read %s", path.c_str());
+        std::vector<uint64_t> map((size_t)head->n);
+        if (std::fread(map.data(), 8, map.size(), f) != map.size())
+            return fail(SPTAG_B200_FAIL, "%s holds fewer than %d ids", path.c_str(), head->n);
+        std::vector<int32_t> tr(map.size());
+        for (size_t i = 0; i < map.size(); ++i) tr[i] = (int32_t)(uint32_t)map[i];
+        if (int rc = s->d_translate.ensure(tr.size() * 4)) return rc;
+        CUDA_OK(cudaMemcpy(s->d_translate.ptr, tr.data(), tr.size() * 4, cudaMemcpyHostToDevice));
+    }
+    // the posting files: SSDIndex, SSDIndex_1, ... while they exist (ExtraFullGraphSearcher.h:165-206)
+    FileCloser fc;
+    std::vector<PostingFile> files;
+    const std::string base = dir + "/" + get("BuildSSDIndex", "SSDIndex", get("Base", "SSDIndex", "SPTAGFullList.bin").c_str());
+    for (std::string cur = base;; cur = base + "_" + std::to_string(files.size())) {
+        FILE* f = fc.open(cur);
+        if (!f) break;
+        files.emplace_back();
+        if (int rc = read_posting_header(f, files.back(), cur.c_str())) return rc;
+        if (files.back().dim != head->dim)
+            return fail(SPTAG_B200_DIMENSION_MISMATCH, "%s: dimension %d, head index %d", cur.c_str(), files.back().dim, head->dim);
+    }
+    if (files.empty()) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot read %s", base.c_str());
+    long long total = 0;
+    for (const PostingFile& pf : files) {
+        for (int i = 0; i < pf.lists; ++i) {
+            s->cnt.push_back(pf.cnt[i]);
+            s->pages.push_back(pf.pages[i]);
+            total += pf.cnt[i];
+        }
+    }
+    s->num_lists = (int)s->cnt.size();
+    if (s->num_lists < head->n) return fail(SPTAG_B200_FAIL, "%d posting lists for %d heads", s->num_lists, head->n);
+    const size_t rs = head->row_stride, row_bytes = (size_t)s->vis - 4;
+    std::vector<long long> off(s->cnt.size());
+    for (size_t l = 0, acc = 0; l < off.size(); acc += (size_t)s->cnt[l], ++l) off[l] = (long long)acc;
+    if (int rc = s->d_off.ensure(off.size() * 8)) return rc;
+    if (int rc = s->d_cnt.ensure(off.size() * 4)) return rc;
+    if (int rc = s->d_pages.ensure(off.size() * 4)) return rc;
+    if (int rc = s->d_ids.ensure(((size_t)total + 1) * 4)) return rc;
+    if (int rc = s->d_rows.ensure(((size_t)total + 1) * rs)) return rc;
+    CUDA_OK(cudaMemcpy(s->d_off.ptr, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(s->d_cnt.ptr, s->cnt.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(s->d_pages.ptr, s->pages.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemset(s->d_rows.ptr, 0, s->d_rows.bytes));
+    // The lists of a file are read in file order, in runs of consecutive lists of at most kRun bytes (a longer list is a
+    // run of its own), each run streamed through upload_rows' pinned chunks into one device staging buffer and split
+    // there: ParsePostingList lays an element out as int32 id + row, ParsePostingListRearrange as every row of the list,
+    // then every id (ExtraFullGraphSearcher.h:1186-1196).  HBM beyond the packed lists: the largest run.
+    const long long kRun = 64ll << 20;
+    DeviceBuffer stage;
+    size_t first_list = 0;
+    for (const PostingFile& pf : files) {
+        const long long fsz = file_size(pf.f);
+        std::vector<int> order;
+        for (int i = 0; i < pf.lists; ++i) {
+            if (pf.cnt[i] == 0) continue;
+            if (pf.start[i] + (long long)pf.cnt[i] * s->vis > fsz)
+                return fail(SPTAG_B200_FAIL, "posting list %zu runs past the end of its file", first_list + i);
+            order.push_back(i);
+        }
+        std::sort(order.begin(), order.end(), [&](int x, int y) { return pf.start[x] < pf.start[y]; });
+        for (size_t r0 = 0; r0 < order.size();) {
+            const long long begin = pf.start[order[r0]];
+            long long end = begin + (long long)pf.cnt[order[r0]] * s->vis;
+            size_t r1 = r0 + 1;
+            for (; r1 < order.size(); ++r1) {
+                const long long e = std::max(end, pf.start[order[r1]] + (long long)pf.cnt[order[r1]] * s->vis);
+                if (e - begin > kRun) break;
+                end = e;
+            }
+            const size_t bytes = (size_t)(end - begin);
+            if (int rc = stage.ensure(bytes)) return rc;
+            ArraySource src;
+            src.file = pf.f;
+            src.offset = begin;
+            const size_t pages = bytes >> 12, tail = bytes & 4095;
+            if (int rc = upload_rows(src, stage.ptr, pages, 4096, 4096, up)) return rc;
+            src.offset = begin + (long long)(pages << 12);
+            if (int rc = upload_rows(src, (unsigned char*)stage.ptr + (pages << 12), 1, tail, tail, up)) return rc;
+            for (size_t r = r0; r < r1; ++r) {
+                const int i = order[r];
+                const size_t c = (size_t)pf.cnt[i], l = first_list + (size_t)i;
+                const unsigned char* src_list = (const unsigned char*)stage.ptr + (pf.start[i] - begin);
+                unsigned char* drow = (unsigned char*)s->d_rows.ptr + (size_t)off[l] * rs;
+                int32_t* did = (int32_t*)s->d_ids.ptr + off[l];
+                if (s->rearranged) {
+                    CUDA_OK(cudaMemcpy2DAsync(drow, rs, src_list, row_bytes, row_bytes, c, cudaMemcpyDeviceToDevice, up));
+                    CUDA_OK(cudaMemcpyAsync(did, src_list + c * row_bytes, c * 4, cudaMemcpyDeviceToDevice, up));
+                } else {
+                    CUDA_OK(cudaMemcpy2DAsync(did, 4, src_list, (size_t)s->vis, 4, c, cudaMemcpyDeviceToDevice, up));
+                    CUDA_OK(cudaMemcpy2DAsync(drow, rs, src_list + 4, (size_t)s->vis, row_bytes, c, cudaMemcpyDeviceToDevice, up));
+                }
+            }
+            CUDA_OK(cudaStreamSynchronize(up));  // the next run reuses the staging buffer
+            r0 = r1;
+        }
+        first_list += (size_t)pf.lists;
+    }
+    std::lock_guard<std::mutex> lock(s->mu);
+    spann_update_shape(s);
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+void sptag_b200_spann_destroy(sptag_b200_spann_handle s) {
+    if (!s) return;
+    {
+        DeviceGuard guard(s->head ? s->head->device : 0);
+        cudaDeviceSynchronize();
+        for (auto& st : s->staging)
+            if (st.stream) cudaStreamDestroy(st.stream);
+        sptag_b200_handle head = s->head;
+        delete s;  // frees the device buffers, with the index's device current
+        sptag_b200_destroy(head);
+    }
+}
+
+int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_handle* out) {
+    if (!folder || !out) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
+    *out = nullptr;
+    const std::string dir(folder);
+    IniSections ini;
+    if (!read_ini(dir + "/indexloader.ini", ini)) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot open %s/indexloader.ini", folder);
+    auto get = [&](const char* section, const char* name, const char* def) { return ini_get(ini, section, name, def); };
+    if (get("Index", "IndexAlgoType", "SPANN") != "SPANN") return fail(SPTAG_B200_LACK_OF_INPUTS, "%s is not a SPANN index", folder);
+    // Refusals: what the device does not hold or decode (SPANN/ParameterDefinitionList.h:34, :79-81)
+    if (!get("Base", "QuantizerFilePath", "").empty())
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "quantized SPANN indexes are not supported on the device");
+    if (ini_true(get("BuildSSDIndex", "EnableDataCompression", "false")))
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "EnableDataCompression (zstd posting lists) is not supported on the device");
+    if (ini_true(get("BuildSSDIndex", "EnableDeltaEncoding", "false")))
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "EnableDeltaEncoding is not supported on the device");
+    const std::string vt = get("Base", "ValueType", "Undefined");
+    int value_type = -1;
+    if (vt == "Float") value_type = SPTAG_B200_VT_FLOAT;
+    else if (vt == "Int8") value_type = SPTAG_B200_VT_INT8;
+    else if (vt == "UInt8") value_type = SPTAG_B200_VT_UINT8;
+    else if (vt == "Int16") value_type = SPTAG_B200_VT_INT16;
+    else return fail(SPTAG_B200_LACK_OF_INPUTS, "unsupported ValueType %s", vt.c_str());
+
+    sptag_b200_handle head = nullptr;
+    const std::string head_dir = dir + "/" + get("Base", "HeadIndexFolder", "HeadIndex");
+    if (int rc = sptag_b200_load(head_dir.c_str(), device, 0, &head)) return rc;
+    auto* s = new sptag_b200_spann();
+    s->head = head;
+    if (head->value_type != value_type || head->q_type != 0) {
+        sptag_b200_spann_destroy(s);
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "head index value type %d does not match ValueType %s", head->value_type, vt.c_str());
+    }
+    if (int rc = spann_fill(s, dir, ini)) {
+        sptag_b200_spann_destroy(s);
+        return rc;
+    }
+    *out = s;
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int32_t num_queries, int32_t k, int32_t* out_ids,
+                            float* out_dists, int32_t* out_stats) {
+    if (!s) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (num_queries < 0 || (num_queries > 0 && (!queries || !out_ids || !out_dists)))
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    if (k < 1 || k > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "k = %d outside the supported range [1, 2048]", k);
+    if (num_queries == 0) return SPTAG_B200_SUCCESS;
+    sptag_b200_handle h = s->head;
+    SpannScanParams p;
+    memset(&p, 0, sizeof(p));
+    int longest = 0;
+    bool truncated = false;
+    {
+        std::lock_guard<std::mutex> lock(s->mu);
+        p.internal = s->internal;
+        p.max_dist_ratio = s->max_dist_ratio;
+        p.page_limit = spann_page_limit(s);
+        longest = s->longest;
+        truncated = s->truncated;
+    }
+    // SPANNIndex.cpp:197-201: the head search runs at K when K >= SearchInternalResultNum, else at SearchInternalResultNum
+    const int w = k >= p.internal ? k : p.internal;
+    if (w > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchInternalResultNum %d exceeds 2048", p.internal);
+    // With the rearranged layout the reference reads a truncated list's ids from an offset computed with the truncated
+    // count (ExtraFullGraphSearcher.h:1186-1190); its results on such lists are not reproduced, so the search is refused
+    if (truncated && s->rearranged)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchPostingPageLimit %d truncates posting lists of the rearranged layout",
+                    p.page_limit);
+    // the dedup table holds every element a query may read at half load
+    const long long reads = (long long)std::min(std::max(p.internal, 0), w) * longest;
+    long long entries = 64;
+    while (entries < 2 * reads) entries <<= 1;
+    if (entries > (1ll << 30)) return fail(SPTAG_B200_MEMORY_OVERFLOW, "dedup table of %lld entries", entries);
+    sptag_b200_spann::Staging* st = nullptr;
+    std::unique_lock<std::mutex> slock;
+    for (auto& cand : s->staging) {
+        std::unique_lock<std::mutex> l(cand.mu, std::try_to_lock);
+        if (l.owns_lock()) {
+            st = &cand;
+            slock = std::move(l);
+            break;
+        }
+    }
+    if (!st) {
+        st = &s->staging[s->staging_rr.fetch_add(1) & 1u];
+        slock = std::unique_lock<std::mutex>(st->mu);
+    }
+    DeviceGuard guard(h->device);
+    cudaStream_t stream = st->stream;
+    const size_t nq = (size_t)num_queries;
+    const size_t qrow = (size_t)h->dim * value_size(h->value_type);
+    const bool cosine = h->metric != SPTAG_B200_METRIC_L2;
+    int elem = 0;
+    with_elem(h, [&](auto el) { elem = el; });
+    int per_sm = spann_scan_blocks_per_sm(cosine, elem, w);
+    if (per_sm < 1) return fail(SPTAG_B200_MEMORY_OVERFLOW, "the posting scan kernel does not fit on an SM at W = %d", w);
+    // resident blocks, but no more dedup-table bytes than kTableBytes unless one block per SM needs more
+    const long long kTableBytes = 256ll << 20;
+    const long long blocks = std::max<long long>(h->num_sms, kTableBytes / (entries * 4));
+    const int grid = (int)std::min<long long>(std::min<long long>((long long)num_queries, (long long)h->num_sms * per_sm), blocks);
+    if (int rc = st->d_q.ensure(nq * qrow)) return rc;
+    if (int rc = st->d_qpad.ensure(nq * h->row_stride)) return rc;
+    if (int rc = st->d_hids.ensure(nq * w * 4)) return rc;
+    if (int rc = st->d_hdists.ensure(nq * w * 4)) return rc;
+    if (int rc = st->d_ids.ensure(nq * k * 4)) return rc;
+    if (int rc = st->d_dists.ensure(nq * k * 4)) return rc;
+    if (out_stats)
+        if (int rc = st->d_stats.ensure(nq * 3 * 4)) return rc;
+    if (int rc = st->d_tables.ensure((size_t)grid * entries * 4)) return rc;
+    CUDA_OK(cudaMemcpyAsync(st->d_q.ptr, queries, nq * qrow, cudaMemcpyHostToDevice, stream));
+    // the scan reads the queries as rows of the head's stride (16-byte aligned, zero padded)
+    CUDA_OK(cudaMemsetAsync(st->d_qpad.ptr, 0, nq * h->row_stride, stream));
+    CUDA_OK(cudaMemcpy2DAsync(st->d_qpad.ptr, h->row_stride, st->d_q.ptr, qrow, qrow, nq, cudaMemcpyDeviceToDevice, stream));
+    {
+        std::lock_guard<std::mutex> lock(h->mu);
+        if (int rc = search_device_impl(h, st->d_q.ptr, num_queries, w, (int*)st->d_hids.ptr, (float*)st->d_hdists.ptr,
+                                        nullptr, stream)) {
+            cudaStreamSynchronize(stream);
+            return rc;
+        }
+    }
+    p.head_ids = (const int*)st->d_hids.ptr;
+    p.head_dists = (const float*)st->d_hdists.ptr;
+    p.nq = num_queries;
+    p.w = w;
+    p.k = k;
+    p.queries = (const unsigned char*)st->d_qpad.ptr;
+    p.row_stride = h->row_stride;
+    p.dim = h->dim;
+    p.simd_width = h->simd_width;
+    p.translate = (const int*)s->d_translate.ptr;
+    p.off = (const long long*)s->d_off.ptr;
+    p.cnt = (const int*)s->d_cnt.ptr;
+    p.pages = (const int*)s->d_pages.ptr;
+    p.ids = (const int*)s->d_ids.ptr;
+    p.rows = (const unsigned char*)s->d_rows.ptr;
+    p.vector_info_size = s->vis;
+    p.tables = (int*)st->d_tables.ptr;
+    p.table_entries = (int)entries;
+    p.out_ids = (int*)st->d_ids.ptr;
+    p.out_dists = (float*)st->d_dists.ptr;
+    p.out_stats = out_stats ? (int*)st->d_stats.ptr : nullptr;
+    cudaError_t e = launch_spann_scan(p, cosine, elem, grid, stream);
+    g_launches++;
+    if (e != cudaSuccess) {
+        cudaStreamSynchronize(stream);
+        return fail(SPTAG_B200_FAIL, "posting scan launch failed: %s", cudaGetErrorString(e));
+    }
+    CUDA_OK(cudaMemcpyAsync(out_ids, st->d_ids.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaMemcpyAsync(out_dists, st->d_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
+    if (out_stats) CUDA_OK(cudaMemcpyAsync(out_stats, st->d_stats.ptr, nq * 3 * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, const char* value) {
+    if (!s || !name || !value) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
+    const std::string n(name);
+    if (n == "MaxCheck") return sptag_b200_set_param(s->head, name, value);  // the head's (SPANNIndex.cpp:901)
+    char* end = nullptr;
+    std::lock_guard<std::mutex> lock(s->mu);
+    if (n == "MaxDistRatio") {
+        const float v = strtof(value, &end);
+        if (end == value) return fail(SPTAG_B200_FAILED_PARSE_VALUE, "cannot parse '%s' for %s", value, name);
+        s->max_dist_ratio = v;
+        return SPTAG_B200_SUCCESS;
+    }
+    const long v = strtol(value, &end, 10);
+    if (n == "SearchInternalResultNum" || n == "SearchPostingPageLimit") {
+        if (end == value) return fail(SPTAG_B200_FAILED_PARSE_VALUE, "cannot parse '%s' for %s", value, name);
+        if (v < 0 || v > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "%s %ld outside [0, 2048]", name, v);
+        (n == "SearchInternalResultNum" ? s->internal : s->page_limit) = (int)v;
+        spann_update_shape(s);
+        return SPTAG_B200_SUCCESS;
+    }
+    if (n == "PostingBytes") return fail(SPTAG_B200_LACK_OF_INPUTS, "PostingBytes is read-only");
+    return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
+}
+
+int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char* value_out, int32_t capacity) {
+    if (!s || !name || !value_out || capacity <= 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
+    const std::string n(name);
+    if (n == "MaxCheck") return sptag_b200_get_param(s->head, name, value_out, capacity);
+    std::lock_guard<std::mutex> lock(s->mu);
+    if (n == "MaxDistRatio") snprintf(value_out, (size_t)capacity, "%f", s->max_dist_ratio);
+    else if (n == "SearchInternalResultNum") snprintf(value_out, (size_t)capacity, "%d", s->internal);
+    else if (n == "SearchPostingPageLimit") snprintf(value_out, (size_t)capacity, "%d", s->page_limit);
+    else if (n == "PostingBytes")
+        snprintf(value_out, (size_t)capacity, "%zu", s->d_translate.bytes + s->d_off.bytes + s->d_cnt.bytes + s->d_pages.bytes +
+                                                         s->d_ids.bytes + s->d_rows.bytes);
+    else return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
+    return SPTAG_B200_SUCCESS;
 }
 
 }  // extern "C"
