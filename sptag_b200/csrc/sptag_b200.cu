@@ -491,7 +491,8 @@ int lay_out(const sptag_b200_index* h, int nq, SearchLaunch& L) {
         if (fit < 1) return fail(SPTAG_B200_MEMORY_OVERFLOW, "search kernel does not fit on an SM (smem %zu)", L.smem);
         int per_sm = h->queries_per_sm;
         if (per_sm <= 0) per_sm = fit;  // the kernel is latency-bound per warp: fill the SM
-        if (h->queries_per_sm <= 0 && big_rows) per_sm = std::min(per_sm, 14);  // 3 KB rows: 14 beats 15 (HBM-bound)
+        // 3 KB rows (HBM-bound): 11-12 slots, with larger queue heads, were the fastest of 10-18 on an H100 (DESIGN.md §5)
+        if (h->queries_per_sm <= 0 && big_rows) per_sm = std::min(per_sm, 12);
         // 512 B rows: 14 slots leave 2 KB more shared memory per queue head than 16 and shorten the tail of a 10k-query batch
         if (h->queries_per_sm <= 0 && fast128) per_sm = std::min(per_sm, want_slots);
         L.per_sm = std::max(1, std::min(per_sm, fit));
