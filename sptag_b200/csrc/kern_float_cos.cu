@@ -1,7 +1,5 @@
 // float rows, cosine / inner product as 1 - dot (DistanceUtils.cpp:1016-1046)
-#include "kern_float_impl.cuh"
+#include "kernel_select_impl.cuh"
 namespace sptag_b200 {
-SearchKernelFn pick_float_kernel_cosine(int dim, int mres_cap, bool kdt, int slots) {
-    return pick_dim<true>(dim, mres_cap, kdt, slots);
-}
+template SearchKernelFn pick_float_kernel<false, true>(int, int, bool, int);
 }  // namespace sptag_b200

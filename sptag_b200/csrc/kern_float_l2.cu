@@ -1,7 +1,5 @@
 // float rows, squared L2 (DistanceUtils.cpp:650-682)
-#include "kern_float_impl.cuh"
+#include "kernel_select_impl.cuh"
 namespace sptag_b200 {
-SearchKernelFn pick_float_kernel_l2(int dim, int mres_cap, bool kdt, int slots) {
-    return pick_dim<false>(dim, mres_cap, kdt, slots);
-}
+template SearchKernelFn pick_float_kernel<false, false>(int, int, bool, int);
 }  // namespace sptag_b200

@@ -1,7 +1,5 @@
 // int16 rows (DistanceUtils.cpp:559-596, :930-967)
-#include "kern_int_impl.cuh"
+#include "kernel_select_impl.cuh"
 namespace sptag_b200 {
-SearchKernelFn pick_int16_kernel(bool cosine, int mres_cap, bool kdt) {
-    return cosine ? pick_int<true, 3>(mres_cap, kdt) : pick_int<false, 3>(mres_cap, kdt);
-}
+template SearchKernelFn pick_int_kernel<false, 3>(bool, int, bool);
 }  // namespace sptag_b200

@@ -1,8 +1,6 @@
 // int8 / uint8 rows (DistanceUtils.cpp:363-400, :460-496, :744-780, :838-874)
-#include "kern_int_impl.cuh"
+#include "kernel_select_impl.cuh"
 namespace sptag_b200 {
-SearchKernelFn pick_int8_kernel(bool is_unsigned, bool cosine, int mres_cap, bool kdt) {
-    if (is_unsigned) return cosine ? pick_int<true, 2>(mres_cap, kdt) : pick_int<false, 2>(mres_cap, kdt);
-    return cosine ? pick_int<true, 1>(mres_cap, kdt) : pick_int<false, 1>(mres_cap, kdt);
-}
+template SearchKernelFn pick_int_kernel<false, 1>(bool, int, bool);
+template SearchKernelFn pick_int_kernel<false, 2>(bool, int, bool);
 }  // namespace sptag_b200

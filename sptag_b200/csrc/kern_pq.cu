@@ -1,10 +1,5 @@
 // PQ / OPQ code rows: SDC / ADC table look-ups (PQQuantizer.h:110-128)
-#include "kernel_select.h"
-#include "search_kernels.cuh"
+#include "kernel_select_impl.cuh"
 namespace sptag_b200 {
-SearchKernelFn pick_pq_kernel(int mres_cap) {
-    if (mres_cap <= 32 * 16) return search_kernel<0, false, 16, false, true, 0, 24>;
-    if (mres_cap <= 32 * 32) return search_kernel<0, false, 32, false, true, 0, 16>;
-    return nullptr;
-}
+template SearchKernelFn pick_pq_kernel<false>(int);
 }  // namespace sptag_b200

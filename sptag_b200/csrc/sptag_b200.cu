@@ -104,6 +104,41 @@ size_t value_size(int vt) {
 
 size_t round_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// The two staging sets of a handle's host-buffer calls, each with its own lock and stream, so that two callers overlap.
+// Buffers: what a set holds besides them.  The streams go with the pool, which its owner destroys with the handle's
+// device current.
+template <typename Buffers>
+struct StagingPool {
+    struct Set : Buffers {
+        std::mutex mu;
+        cudaStream_t stream = nullptr;
+    };
+    Set sets[2];
+    std::atomic<unsigned> rr{0};
+    ~StagingPool() {
+        for (Set& s : sets)
+            if (s.stream) cudaStreamDestroy(s.stream);
+    }
+    bool create_streams() {
+        for (Set& s : sets)
+            if (cudaStreamCreate(&s.stream) != cudaSuccess) return false;
+        return true;
+    }
+    // A set of the caller's own for the whole call: the one that is free, else wait for the next in turn
+    Set* acquire(std::unique_lock<std::mutex>& lock) {
+        for (Set& s : sets) {
+            std::unique_lock<std::mutex> l(s.mu, std::try_to_lock);
+            if (l.owns_lock()) {
+                lock = std::move(l);
+                return &s;
+            }
+        }
+        Set* s = &sets[rr.fetch_add(1) & 1u];
+        lock = std::unique_lock<std::mutex>(s->mu);
+        return s;
+    }
+};
+
 }  // namespace
 
 struct sptag_b200_index {
@@ -179,12 +214,10 @@ struct sptag_b200_index {
     DeviceBuffer d_ids, d_dists;                      // refine pass: per-batch result lists
     // Host-buffer entry points: two staging sets, each with its own stream, so that one caller's H2D / D2H overlaps
     // another caller's kernel (the kernels themselves share the per-slot scratch and are ordered by ev_done)
-    struct Staging {
-        std::mutex mu;
-        cudaStream_t stream = nullptr;
+    struct StagingBuffers {
         DeviceBuffer d_queries, d_ids, d_dists, d_stats, d_filter, d_overflows;
-    } staging[2];
-    std::atomic<unsigned> staging_rr{0};
+    };
+    StagingPool<StagingBuffers> staging;
     DeviceBuffer d_graph_new;                         // sptag_b200_refine_graph: the pass's output rows
     cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_aux = nullptr;
     double refine_search_ms = 0.0, refine_rebuild_ms = 0.0;  // device time of the last sptag_b200_refine_graph call
@@ -234,24 +267,32 @@ int heap_lastlevel(int size) {
 // EnableBfs is in force: a BKT handle with a non-zero value.  Its searches take the bfs:: kernels.
 bool bfs_seeding(const sptag_b200_index* h) { return h->algo == SPTAG_B200_ALGO_BKT && h->bfs != 0; }
 
+template <bool BFS>
+SearchKernelFn pick_kernel_seeded(const sptag_b200_index* h, int mres_cap, int slots) {
+    const bool kdt = (h->algo == SPTAG_B200_ALGO_KDT);
+    const bool cosine = (h->metric != SPTAG_B200_METRIC_L2);
+    if (h->q_type != 0) return pick_pq_kernel<BFS>(mres_cap);  // quantized: BKT + L2 only (PQQuantizer.h:130-136)
+    if (h->value_type == SPTAG_B200_VT_INT8) return pick_int_kernel<BFS, 1>(cosine, mres_cap, kdt);
+    if (h->value_type == SPTAG_B200_VT_UINT8) return pick_int_kernel<BFS, 2>(cosine, mres_cap, kdt);
+    if (h->value_type == SPTAG_B200_VT_INT16) return pick_int_kernel<BFS, 3>(cosine, mres_cap, kdt);
+    const int kdim = (h->simd_width == 16) ? h->dim : 0;  // the 128- / 768-d specialisations are AVX-512 trees
+    return cosine ? pick_float_kernel<BFS, true>(kdim, mres_cap, kdt, slots)
+                  : pick_float_kernel<BFS, false>(kdim, mres_cap, kdt, slots);
+}
+
 // The kernel instantiation for this index / parameter set (nullptr: unsupported m_Results capacity); the
 // instantiations live in kern_*.cu (kernel_select.h)
 SearchKernelFn pick_kernel(const sptag_b200_index* h, int mres_cap, int slots = 0) {
-    const bool kdt = (h->algo == SPTAG_B200_ALGO_KDT);
-    const bool l2 = (h->metric == SPTAG_B200_METRIC_L2);
-    if (bfs_seeding(h)) {
-        if (h->q_type != 0) return pick_pq_bfs_kernel(mres_cap);
-        if (h->value_type == SPTAG_B200_VT_INT8) return pick_int8_bfs_kernel(false, !l2, mres_cap);
-        if (h->value_type == SPTAG_B200_VT_UINT8) return pick_int8_bfs_kernel(true, !l2, mres_cap);
-        if (h->value_type == SPTAG_B200_VT_INT16) return pick_int16_bfs_kernel(!l2, mres_cap);
-        return l2 ? pick_float_bfs_kernel_l2(mres_cap) : pick_float_bfs_kernel_cosine(mres_cap);
-    }
-    if (h->q_type != 0) return pick_pq_kernel(mres_cap);  // quantized: BKT + L2 only (PQQuantizer.h:130-136)
-    if (h->value_type == SPTAG_B200_VT_INT8) return pick_int8_kernel(false, !l2, mres_cap, kdt);
-    if (h->value_type == SPTAG_B200_VT_UINT8) return pick_int8_kernel(true, !l2, mres_cap, kdt);
-    if (h->value_type == SPTAG_B200_VT_INT16) return pick_int16_kernel(!l2, mres_cap, kdt);
-    const int kdim = (h->simd_width == 16) ? h->dim : 0;  // the 128- / 768-d specialisations are AVX-512 trees
-    return l2 ? pick_float_kernel_l2(kdim, mres_cap, kdt, slots) : pick_float_kernel_cosine(kdim, mres_cap, kdt, slots);
+    return bfs_seeding(h) ? pick_kernel_seeded<true>(h, mres_cap, slots) : pick_kernel_seeded<false>(h, mres_cap, slots);
+}
+
+// The ResultIterator::Next (Fn = IterateKernelFn) or SearchIndexIterativeFromNeareast first-call (NearestFirstKernelFn)
+// kernel of an iterator step planned with parameters p (nullptr: unsupported m_Results capacity)
+template <typename Fn>
+Fn pick_iter_step_kernel(const sptag_b200_index* h, const SearchParams& p) {
+    const bool cosine = h->metric != SPTAG_B200_METRIC_L2;
+    return p.bfs ? pick_iter_kernel<Fn, true>(h->value_type, cosine, p.mres_cap)
+                 : pick_iter_kernel<Fn, false>(h->value_type, cosine, p.mres_cap);
 }
 
 // What one call may override (the reference passes these per call: p_searchDeleted of SearchIndex / GetIterator,
@@ -769,13 +810,10 @@ int grow_iter_visited(sptag_b200_iterator* it, const std::vector<unsigned>& qs, 
     return 0;
 }
 
-// The first Next of an iterator on hash tables with EnableBfs = bfs > 0: the breadth-first seeding cannot suspend, and it
-// inserts at most MaxBFSNodes centres per level and tree.  Tables below that limit are replaced by empty ones that hold it
-// (still empty: nothing has run), or by bitmaps where such a table would be larger.  Caller holds h->mu.
-int fit_bfs_seeding(sptag_b200_iterator* it, int bfs) {
-    const long long seeds = std::min<long long>((long long)kBfsMaxNodes * bfs * it->h->tree_num, (long long)it->h->n + 1);
-    int need = 6;
-    while (need < 31 && ((long long)1 << (need - 1)) < seeds) ++need;
+// Before an iterator's first call, whose seeding cannot suspend: every hashed table of fewer than 2^need entries is
+// replaced by an empty one of 2^need (the tables are still empty: nothing has run), or by a bitmap where such a table
+// would be larger.  Caller holds h->mu.
+int fit_iter_tables(sptag_b200_iterator* it, int need) {
     std::vector<unsigned> qs;
     std::vector<int> bits;
     for (int q = 0; q < it->nq; ++q)
@@ -784,6 +822,15 @@ int fit_bfs_seeding(sptag_b200_iterator* it, int bfs) {
             bits.push_back(need);
         }
     return qs.empty() ? 0 : grow_iter_visited(it, qs, bits, false, nullptr);
+}
+
+// The first Next of an iterator on hash tables with EnableBfs = bfs > 0: the breadth-first seeding inserts at most
+// MaxBFSNodes centres per level and tree.  Caller holds h->mu.
+int fit_bfs_seeding(sptag_b200_iterator* it, int bfs) {
+    const long long seeds = std::min<long long>((long long)kBfsMaxNodes * bfs * it->h->tree_num, (long long)it->h->n + 1);
+    int need = 6;
+    while (need < 31 && ((long long)1 << (need - 1)) < seeds) ++need;
+    return fit_iter_tables(it, need);
 }
 
 // Run one iterator step planned by plan_iterator_step.  The iterator's queue lengths and per-query arenas replace the
@@ -1093,9 +1140,9 @@ int build_handle(const IndexShape& sh, const ArraySource& vectors, const ArraySo
         cudaEventCreate(&h->ev_aux) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->scratch[0].ev_done, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->scratch[1].ev_done, cudaEventDisableTiming) != cudaSuccess ||
-        cudaStreamCreate(&h->staging[0].stream) != cudaSuccess || cudaStreamCreate(&h->staging[1].stream) != cudaSuccess)
+        !h->staging.create_streams())
         return destroy_on_fail(fail(SPTAG_B200_FAIL, "cudaEventCreate / cudaStreamCreate failed"));
-    cudaStream_t up = h->staging[0].stream;
+    cudaStream_t up = h->staging.sets[0].stream;
     // one spare row so a 16-byte padded read of the last row stays in bounds
     if (int rc = h->d_vectors.ensure(((size_t)h->n + 1) * h->row_stride)) return destroy_on_fail(rc);
     if (h->row_stride != row_bytes) cudaMemsetAsync(h->d_vectors.ptr, 0, ((size_t)h->n + 1) * h->row_stride, up);
@@ -1138,6 +1185,67 @@ int build_handle(const IndexShape& sh, const ArraySource& vectors, const ArraySo
         return destroy_on_fail(fail(SPTAG_B200_FAIL, "index upload failed"));
     *out = h;
     return SPTAG_B200_SUCCESS;
+}
+
+// indexloader.ini as Helper::IniReader reads it (SimpleIniReader.cpp:40-135): [Section] headers and Name=Value lines,
+// section and parameter names trimmed and lower-cased; values trimmed here too
+typedef std::map<std::string, std::map<std::string, std::string>> IniSections;
+std::string trim(const std::string& v) {
+    const size_t a = v.find_first_not_of(" \t\r");
+    if (a == std::string::npos) return std::string();
+    return v.substr(a, v.find_last_not_of(" \t\r") + 1 - a);
+}
+std::string lower(std::string v) {
+    for (char& c : v) c = (char)std::tolower((unsigned char)c);
+    return v;
+}
+bool read_ini(const std::string& path, IniSections& out) {
+    std::ifstream ini(path);
+    if (!ini) return false;
+    std::string line, section;
+    while (std::getline(ini, line)) {
+        line = trim(line);
+        if (line.empty() || line[0] == ';' || line[0] == '#') continue;
+        if (line[0] == '[') {
+            const size_t close = line.find(']');
+            section = lower(trim(line.substr(1, close == std::string::npos ? std::string::npos : close - 1)));
+            continue;
+        }
+        const size_t eq = line.find('=');
+        if (eq != std::string::npos) out[section][lower(trim(line.substr(0, eq)))] = trim(line.substr(eq + 1));
+    }
+    return true;
+}
+std::string ini_get(const IniSections& ini, const char* section, const char* name, const std::string& def) {
+    auto s = ini.find(lower(section));
+    if (s == ini.end()) return def;
+    auto it = s->second.find(lower(name));
+    return it == s->second.end() ? def : it->second;
+}
+
+bool ini_true(const std::string& v) { return lower(v) == "true" || v == "1"; }
+
+// The names of IndexAlgoType, VectorValueType and DistCalcMethod in an ini (DefinitionList.h), matched exactly
+struct EnumName {
+    int value;
+    const char* name;
+};
+const EnumName kIndexAlgoTypes[] = {{SPTAG_B200_ALGO_BKT, "BKT"}, {SPTAG_B200_ALGO_KDT, "KDT"}};
+const EnumName kValueTypes[] = {{SPTAG_B200_VT_INT8, "Int8"}, {SPTAG_B200_VT_UINT8, "UInt8"},
+                                {SPTAG_B200_VT_INT16, "Int16"}, {SPTAG_B200_VT_FLOAT, "Float"}};
+const EnumName kDistCalcMethods[] = {{SPTAG_B200_METRIC_L2, "L2"}, {SPTAG_B200_METRIC_COSINE, "Cosine"},
+                                     {SPTAG_B200_METRIC_INNERPRODUCT, "InnerProduct"}};
+template <size_t N>
+int enum_value(const EnumName (&names)[N], const std::string& name) {  // -1: not a name of the table
+    for (const EnumName& e : names)
+        if (name == e.name) return e.value;
+    return -1;
+}
+template <size_t N>
+const char* enum_name(const EnumName (&names)[N], int value) {
+    for (const EnumName& e : names)
+        if (value == e.value) return e.name;
+    return "Undefined";
 }
 
 }  // namespace
@@ -1183,8 +1291,6 @@ void sptag_b200_destroy(sptag_b200_handle h) {
     cudaDeviceSynchronize();
     for (auto& sc : h->scratch)
         if (sc.ev_done) cudaEventDestroy(sc.ev_done);
-    for (auto& st : h->staging)
-        if (st.stream) cudaStreamDestroy(st.stream);
     if (h->ev_start) cudaEventDestroy(h->ev_start);
     if (h->ev_stop) cudaEventDestroy(h->ev_stop);
     if (h->ev_aux) cudaEventDestroy(h->ev_aux);
@@ -1215,46 +1321,22 @@ int sptag_b200_load(const char* folder, int32_t device, int32_t id_offset, sptag
     if (!folder || !out) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
     *out = nullptr;
     const std::string dir(folder);
-    // indexloader.ini: "[Index]" section of Name=Value lines (VectorIndex.cpp:197-222, :617-681)
-    std::ifstream ini(dir + "/indexloader.ini");
-    if (!ini) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot open %s/indexloader.ini", folder);
-    std::map<std::string, std::string> kv;
-    std::string line;
-    while (std::getline(ini, line)) {
-        while (!line.empty() && (line.back() == '\r' || line.back() == ' ')) line.pop_back();
-        if (line.empty() || line[0] == '[' || line[0] == ';' || line[0] == '#') continue;
-        size_t eq = line.find('=');
-        if (eq == std::string::npos) continue;
-        kv[line.substr(0, eq)] = line.substr(eq + 1);
-    }
-    auto get = [&](const char* name, const char* def) {
-        auto it = kv.find(name);
-        return it == kv.end() ? std::string(def) : it->second;
-    };
+    // indexloader.ini as VectorIndex::LoadIndex reads it (VectorIndex.cpp:617-681): the index's parameters and files
+    // from [Index] (BKTIndex.cpp:21-31), its quantizer from [Quantizer] (VectorIndex.cpp:188-192)
+    IniSections ini;
+    if (!read_ini(dir + "/indexloader.ini", ini)) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot open %s/indexloader.ini", folder);
+    auto get = [&](const char* name, const char* def) { return ini_get(ini, "Index", name, def); };
     IndexShape sh;
     sh.device = device;
     sh.id_offset = id_offset;
     const std::string algo = get("IndexAlgoType", "BKT");
-    if (algo == "BKT")
-        sh.algo = SPTAG_B200_ALGO_BKT;
-    else if (algo == "KDT")
-        sh.algo = SPTAG_B200_ALGO_KDT;
-    else
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "unsupported IndexAlgoType %s", algo.c_str());
+    sh.algo = enum_value(kIndexAlgoTypes, algo);
+    if (sh.algo < 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "unsupported IndexAlgoType %s", algo.c_str());
     const std::string vt = get("ValueType", "Float");
-    if (vt == "Float")
-        sh.value_type = SPTAG_B200_VT_FLOAT;
-    else if (vt == "Int8")
-        sh.value_type = SPTAG_B200_VT_INT8;
-    else if (vt == "UInt8")
-        sh.value_type = SPTAG_B200_VT_UINT8;
-    else if (vt == "Int16")
-        sh.value_type = SPTAG_B200_VT_INT16;
-    else
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "unsupported ValueType %s", vt.c_str());
-    const std::string dm = get("DistCalcMethod", "Cosine");  // reference default is Cosine
-    sh.metric = (dm == "L2") ? SPTAG_B200_METRIC_L2
-                             : (dm == "InnerProduct" ? SPTAG_B200_METRIC_INNERPRODUCT : SPTAG_B200_METRIC_COSINE);
+    sh.value_type = enum_value(kValueTypes, vt);
+    if (sh.value_type < 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "unsupported ValueType %s", vt.c_str());
+    const int metric = enum_value(kDistCalcMethods, get("DistCalcMethod", "Cosine"));  // reference default is Cosine
+    sh.metric = metric < 0 ? SPTAG_B200_METRIC_COSINE : metric;
     FileCloser fc;
     FILE* fv = fc.open(dir + "/" + get("VectorFilePath", "vectors.bin"));
     FILE* fg = fc.open(dir + "/" + get("GraphFilePath", "graph.bin"));
@@ -1311,27 +1393,25 @@ int sptag_b200_load(const char* folder, int32_t device, int32_t id_offset, sptag
     t.offset = nodes_off;
     sptag_b200_handle h = nullptr;
     if (int rc = build_handle(sh, v, g, starts.data(), t, d, &h)) return rc;
-    {
-        auto it = kv.find("QuantizerFilePath");  // [Quantizer] section (VectorIndex.cpp:188-192)
-        if (it != kv.end() && !it->second.empty()) {
-            std::vector<char> qb;
-            if (!read_file(dir + "/" + it->second, qb)) {
-                sptag_b200_destroy(h);
-                return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot read quantizer file %s", it->second.c_str());
-            }
-            if (int rc = sptag_b200_set_quantizer(h, qb.data(), (int64_t)qb.size())) {
-                sptag_b200_destroy(h);
-                return rc;
-            }
+    const std::string qpath = ini_get(ini, "Quantizer", "QuantizerFilePath", "");
+    if (!qpath.empty()) {
+        std::vector<char> qb;
+        if (!read_file(dir + "/" + qpath, qb)) {
+            sptag_b200_destroy(h);
+            return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot read quantizer file %s", qpath.c_str());
+        }
+        if (int rc = sptag_b200_set_quantizer(h, qb.data(), (int64_t)qb.size())) {
+            sptag_b200_destroy(h);
+            return rc;
         }
     }
     static const char* names[] = {"MaxCheck", "MaxCheckForRefineGraph", "NumberOfInitialDynamicPivots",
                                   "NumberOfOtherDynamicPivots", "ThresholdOfNumberOfContinuousNoBetterPropagation",
                                   "AddCEF", "CEF", "RNGFactor", "EnableBfs"};
     for (const char* nm : names) {
-        auto it = kv.find(nm);
+        const std::string v = get(nm, "");
         // (EnableBfs is a BKT parameter: set_param refuses it on a KDT handle, and the KDT loader ignores the key)
-        if (it != kv.end()) sptag_b200_set_param(h, nm, it->second.c_str());
+        if (!v.empty()) sptag_b200_set_param(h, nm, v.c_str());
     }
     *out = h;
     return SPTAG_B200_SUCCESS;
@@ -1518,21 +1598,8 @@ namespace {
 int search_host_impl(sptag_b200_handle h, const void* queries, int32_t num_queries, int32_t k, CallOpts opts,
                      const uint8_t* allowed, bool refine, int32_t* out_ids, float* out_dists, int32_t* out_stats) {
     if (num_queries == 0) return SPTAG_B200_SUCCESS;
-    // a staging set of our own for the whole call: the one that is free, else wait for the next in turn
-    sptag_b200_index::Staging* st = nullptr;
     std::unique_lock<std::mutex> slock;
-    for (auto& cand : h->staging) {
-        std::unique_lock<std::mutex> l(cand.mu, std::try_to_lock);
-        if (l.owns_lock()) {
-            st = &cand;
-            slock = std::move(l);
-            break;
-        }
-    }
-    if (!st) {
-        st = &h->staging[h->staging_rr.fetch_add(1) & 1u];
-        slock = std::unique_lock<std::mutex>(st->mu);
-    }
+    auto* st = h->staging.acquire(slock);
     DeviceGuard guard(h->device);
     const size_t qbytes = (size_t)num_queries * query_bytes(h);
     const size_t rn = (size_t)num_queries * k;
@@ -1908,9 +1975,7 @@ int sptag_b200_iterator_next(sptag_b200_iter it, int32_t batch, int32_t* out_ids
     DeviceGuard guard(h->device);
     SearchLaunch L;
     if (int rc = plan_iterator_step(it, batch, L)) return rc;
-    const bool cosine = h->metric != SPTAG_B200_METRIC_L2;
-    IterateKernelFn kern = L.p.bfs ? pick_iterate_bfs_kernel_for(h->value_type, cosine, L.p.mres_cap)
-                                   : pick_iterate_kernel_for(h->value_type, cosine, L.p.mres_cap);
+    IterateKernelFn kern = pick_iter_step_kernel<IterateKernelFn>(h, L.p);
     if (!kern) return fail(SPTAG_B200_LACK_OF_INPUTS, "max(MaxCheck/16, batch) = %d exceeds the supported 1024", L.p.mres_cap);
     if (!it->stepped && it->nearest_k == 0 && it->hashed && L.p.bfs > 0)
         if (int rc = fit_bfs_seeding(it, L.p.bfs)) return rc;
@@ -1938,11 +2003,8 @@ int sptag_b200_iterator_next_from_nearest(sptag_b200_iter it, int32_t k, int32_t
     DeviceGuard guard(h->device);
     SearchLaunch L;
     if (int rc = plan_iterator_step(it, k, L)) return rc;
-    const bool cosine = h->metric != SPTAG_B200_METRIC_L2;
-    NearestFirstKernelFn kfirst = L.p.bfs ? pick_nearest_first_bfs_kernel_for(h->value_type, cosine, L.p.mres_cap)
-                                          : pick_nearest_first_kernel_for(h->value_type, cosine, L.p.mres_cap);
-    IterateKernelFn knext = L.p.bfs ? pick_iterate_bfs_kernel_for(h->value_type, cosine, L.p.mres_cap)
-                                    : pick_iterate_kernel_for(h->value_type, cosine, L.p.mres_cap);
+    NearestFirstKernelFn kfirst = pick_iter_step_kernel<NearestFirstKernelFn>(h, L.p);
+    IterateKernelFn knext = pick_iter_step_kernel<IterateKernelFn>(h, L.p);
     if (!kfirst || !knext)
         return fail(SPTAG_B200_LACK_OF_INPUTS, "max(MaxCheck/16, k) = %d exceeds the supported 1024", L.p.mres_cap);
     if (first && it->hashed) {
@@ -1950,15 +2012,7 @@ int sptag_b200_iterator_next_from_nearest(sptag_b200_iter it, int32_t k, int32_t
         // holds that below its limit (the tables are still empty)
         int need = 6;
         while (((size_t)1 << (need - 1)) < (size_t)k * (h->degree + 1)) ++need;
-        std::vector<unsigned> qs;
-        std::vector<int> bits;
-        for (int q = 0; q < it->nq; ++q)
-            if (it->q_bits[q] != 0 && it->q_bits[q] < need) {
-                qs.push_back((unsigned)q);
-                bits.push_back(need);
-            }
-        if (!qs.empty())
-            if (int rc = grow_iter_visited(it, qs, bits, false, nullptr)) return rc;
+        if (int rc = fit_iter_tables(it, need)) return rc;
     }
     const int rc = run_iterator_step(
         it, k, "k", L, out_ids, out_dists, nullptr, nullptr, first,
@@ -2266,15 +2320,6 @@ int value_base(int vt) {  // COMMON::Utils::GetBase<T> (CommonUtils.h:54-59)
 
 bool write_all(FILE* f, const void* p, size_t bytes) { return bytes == 0 || std::fwrite(p, 1, bytes, f) == bytes; }
 
-const char* value_type_name(int vt) {
-    switch (vt) {
-    case SPTAG_B200_VT_INT8: return "Int8";
-    case SPTAG_B200_VT_UINT8: return "UInt8";
-    case SPTAG_B200_VT_INT16: return "Int16";
-    }
-    return "Float";
-}
-
 }  // namespace
 
 extern "C" {
@@ -2493,15 +2538,15 @@ int sptag_b200_save(sptag_b200_handle h, const char* folder) {
     // indexloader.ini as VectorIndex::SaveIndexConfig writes it (VectorIndex.cpp:197-222): [Index] with the algorithm and
     // value type, then the parameters; the reference's LoadIndex and sptag_b200_load both read it
     if (FILE* f = open_w("indexloader.ini")) {
-        const char* metric = h->metric == SPTAG_B200_METRIC_L2 ? "L2" : (h->metric == SPTAG_B200_METRIC_COSINE ? "Cosine" : "InnerProduct");
         const int w = std::fprintf(
             f,
             "[Index]\nIndexAlgoType=%s\nValueType=%s\n\nTreeFilePath=tree.bin\nGraphFilePath=graph.bin\nVectorFilePath=vectors.bin\n"
             "DeleteVectorFilePath=deletes.bin\nNeighborhoodSize=%d\nCEF=%d\nAddCEF=%d\nMaxCheckForRefineGraph=%d\nRNGFactor=%f\n"
             "DistCalcMethod=%s\nMaxCheck=%d\nThresholdOfNumberOfContinuousNoBetterPropagation=%d\nNumberOfInitialDynamicPivots=%d\n"
             "NumberOfOtherDynamicPivots=%d\n",
-            bkt ? "BKT" : "KDT", value_type_name(h->value_type), h->degree, h->cef, h->add_cef, h->max_check_refine,
-            h->rng_factor, metric, h->max_check, h->no_better_threshold, h->initial_pivots, h->other_pivots);
+            enum_name(kIndexAlgoTypes, h->algo), enum_name(kValueTypes, h->value_type), h->degree, h->cef, h->add_cef,
+            h->max_check_refine, h->rng_factor, enum_name(kDistCalcMethods, h->metric), h->max_check,
+            h->no_better_threshold, h->initial_pivots, h->other_pivots);
         // written only when set, so that the folders of handles without it stay as they were
         const int wb = (bkt && h->bfs != 0) ? std::fprintf(f, "EnableBfs=%d\n", h->bfs) : 1;
         ok = w > 0 && wb > 0 && std::fclose(f) == 0 && ok;
@@ -2540,12 +2585,10 @@ struct sptag_b200_spann {
     DeviceBuffer d_translate, d_off, d_cnt, d_pages, d_ids, d_rows;
     // Host-buffer calls run on one of two staging sets, each with its own stream, head results, dedup tables and outputs,
     // so that two callers overlap; the head search kernels are ordered by the head handle (search_device_impl)
-    struct Staging {
-        std::mutex mu;
-        cudaStream_t stream = nullptr;
+    struct StagingBuffers {
         DeviceBuffer d_q, d_qpad, d_hids, d_hdists, d_ids, d_dists, d_stats, d_tables;
-    } staging[2];
-    std::atomic<unsigned> staging_rr{0};
+    };
+    StagingPool<StagingBuffers> staging;
     std::mutex mu;  // the search parameters
 };
 
@@ -2559,44 +2602,6 @@ int spann_page_limit(const sptag_b200_spann* s) { return std::max(s->page_limit,
 int spann_searched(const sptag_b200_spann* s, int l, int limit) {
     return (int)std::min<long long>(s->cnt[l], ((long long)std::min(s->pages[l], limit) << 12) / s->vis);
 }
-
-// indexloader.ini as Helper::IniReader reads it (SimpleIniReader.cpp:40-135): [Section] headers and Name=Value lines,
-// section and parameter names trimmed and lower-cased; values trimmed here too
-typedef std::map<std::string, std::map<std::string, std::string>> IniSections;
-std::string trim(const std::string& v) {
-    const size_t a = v.find_first_not_of(" \t\r");
-    if (a == std::string::npos) return std::string();
-    return v.substr(a, v.find_last_not_of(" \t\r") + 1 - a);
-}
-std::string lower(std::string v) {
-    for (char& c : v) c = (char)std::tolower((unsigned char)c);
-    return v;
-}
-bool read_ini(const std::string& path, IniSections& out) {
-    std::ifstream ini(path);
-    if (!ini) return false;
-    std::string line, section;
-    while (std::getline(ini, line)) {
-        line = trim(line);
-        if (line.empty() || line[0] == ';' || line[0] == '#') continue;
-        if (line[0] == '[') {
-            const size_t close = line.find(']');
-            section = lower(trim(line.substr(1, close == std::string::npos ? std::string::npos : close - 1)));
-            continue;
-        }
-        const size_t eq = line.find('=');
-        if (eq != std::string::npos) out[section][lower(trim(line.substr(0, eq)))] = trim(line.substr(eq + 1));
-    }
-    return true;
-}
-std::string ini_get(const IniSections& ini, const char* section, const char* name, const std::string& def) {
-    auto s = ini.find(lower(section));
-    if (s == ini.end()) return def;
-    auto it = s->second.find(lower(name));
-    return it == s->second.end() ? def : it->second;
-}
-
-bool ini_true(const std::string& v) { return lower(v) == "true" || v == "1"; }
 
 // The longest list a search reads at the page limit in force, and whether that limit truncates any list (recomputed when
 // the limit changes).  Caller holds s->mu.
@@ -2671,9 +2676,8 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
     const long long vector_limit = atoll(get("BuildSSDIndex", "PostingVectorLimit", "118").c_str());
     s->vector_limit_pages = (int)((vector_limit * s->vis + 4095) / 4096);
     DeviceGuard guard(head->device);
-    for (auto& st : s->staging)
-        if (cudaStreamCreate(&st.stream) != cudaSuccess) return fail(SPTAG_B200_FAIL, "cudaStreamCreate failed");
-    cudaStream_t up = s->staging[0].stream;
+    if (!s->staging.create_streams()) return fail(SPTAG_B200_FAIL, "cudaStreamCreate failed");
+    cudaStream_t up = s->staging.sets[0].stream;
     // m_vectorTranslateMap: one uint64 per head (SPANNIndex.cpp:133-134), kept as the SizeType the search casts it to
     {
         FileCloser fc;
@@ -2790,8 +2794,6 @@ void sptag_b200_spann_destroy(sptag_b200_spann_handle s) {
     {
         DeviceGuard guard(s->head ? s->head->device : 0);
         cudaDeviceSynchronize();
-        for (auto& st : s->staging)
-            if (st.stream) cudaStreamDestroy(st.stream);
         sptag_b200_handle head = s->head;
         delete s;  // frees the device buffers, with the index's device current
         sptag_b200_destroy(head);
@@ -2814,12 +2816,8 @@ int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_h
     if (ini_true(get("BuildSSDIndex", "EnableDeltaEncoding", "false")))
         return fail(SPTAG_B200_LACK_OF_INPUTS, "EnableDeltaEncoding is not supported on the device");
     const std::string vt = get("Base", "ValueType", "Undefined");
-    int value_type = -1;
-    if (vt == "Float") value_type = SPTAG_B200_VT_FLOAT;
-    else if (vt == "Int8") value_type = SPTAG_B200_VT_INT8;
-    else if (vt == "UInt8") value_type = SPTAG_B200_VT_UINT8;
-    else if (vt == "Int16") value_type = SPTAG_B200_VT_INT16;
-    else return fail(SPTAG_B200_LACK_OF_INPUTS, "unsupported ValueType %s", vt.c_str());
+    const int value_type = enum_value(kValueTypes, vt);
+    if (value_type < 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "unsupported ValueType %s", vt.c_str());
 
     sptag_b200_handle head = nullptr;
     const std::string head_dir = dir + "/" + get("Base", "HeadIndexFolder", "HeadIndex");
@@ -2871,20 +2869,8 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     long long entries = 64;
     while (entries < 2 * reads) entries <<= 1;
     if (entries > (1ll << 30)) return fail(SPTAG_B200_MEMORY_OVERFLOW, "dedup table of %lld entries", entries);
-    sptag_b200_spann::Staging* st = nullptr;
     std::unique_lock<std::mutex> slock;
-    for (auto& cand : s->staging) {
-        std::unique_lock<std::mutex> l(cand.mu, std::try_to_lock);
-        if (l.owns_lock()) {
-            st = &cand;
-            slock = std::move(l);
-            break;
-        }
-    }
-    if (!st) {
-        st = &s->staging[s->staging_rr.fetch_add(1) & 1u];
-        slock = std::unique_lock<std::mutex>(st->mu);
-    }
+    auto* st = s->staging.acquire(slock);
     DeviceGuard guard(h->device);
     cudaStream_t stream = st->stream;
     const size_t nq = (size_t)num_queries;
