@@ -392,10 +392,40 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
 
 /* Replaces: SPANN::Index<T>::SetParameter / GetParameter (SPANNIndex.cpp:1033-1073) for SearchInternalResultNum,
  * MaxDistRatio (a float), SearchPostingPageLimit (raised at search time to the pages of PostingVectorLimit vectors, as
- * ExtraFullGraphSearcher::LoadIndex does, :167) and MaxCheck (the head's).  Read-only: PostingBytes (device bytes of the
- * posting lists and the translate map). */
+ * ExtraFullGraphSearcher::LoadIndex does, :167), MaxCheck (the head's) and IterativeSearchHeadBatch ([BuildSSDIndex],
+ * default 32, in [1, 1024]; sampled when an iterator opens).  B200.IteratorVisitedSet and B200.IteratorVisitedHashEntries
+ * are the head handle's (sptag_b200_set_param): they choose the visited sets of the head iterators SPANN iterators open.
+ * B200.SpannDedupEntries: the first dedup table size of an iterator's queries, 0 (default: room for one head batch of
+ * the longest list, at most 2^14) or a power of two >= 64; tables double as they fill.  Read-only: PostingBytes (device
+ * bytes of the posting lists and the translate map), B200.LastIteratorRounds (head refill rounds of the last
+ * sptag_b200_spann_iterator_next on this handle) and B200.LastIteratorDedupBytes (that iterator's dedup table bytes). */
 int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, const char* value);
 int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char* value_out, int32_t capacity);
+
+/* Replaces: SPANN::Index<T>::GetIterator(p_target) (SPANNIndex.cpp:299-314) and SPANNResultIterator::Next(batch)
+ * (SPANNResultIterator.h:37-63, SPANNIndex.cpp:261-296, :416-446, ExtraFullGraphSearcher.h:131-147, :492-525) for every
+ * query of a HOST batch, one iterator per query.
+ *   open:  opens a head iterator per query (p_searchDeleted = false) and an empty ExtraWorkSpace; the head batch is
+ *          IterativeSearchHeadBatch as set now.  The SPANN handle must outlive its iterators.
+ *   next:  up to `batch` further results per query, a resumable, deduplicated stream of posting elements.  The first call
+ *          runs the head's SearchIndexIterativeFromNeareast(first); then each query reads its chosen lists from where it
+ *          stopped, and when they run out asks the head for its next batch, until the call has `batch` results or the
+ *          head finds nothing.  As in the reference, a call's batch is capped by the previous call's result count, the
+ *          deduper spans every head batch and call, an element found as the last element of the last list is added to
+ *          the result but not counted, and RelaxedMono turns on once SearchInternalResultNum lists were loaded before a
+ *          load.  out_ids / out_dists: HOST [num_queries x batch], sorted, unfilled slots (-1, MaxDist); out_counts[q] =
+ *          resultCount; out_relaxed_mono[q] = GetRelaxedMono().  Results equal the reference's bit for bit.
+ *          sptag_b200_spann_search on the same handle may run between calls; it does not change their results.
+ *   close: frees the iterators.
+ * LackOfInputs: null arguments, batch outside [1, 1024], IterativeSearchHeadBatch outside [1, 1024] (open) or above
+ * SearchInternalResultNum (next: the reference has only that many page buffers, IExtraSearcher.h:114-122), and a page
+ * limit that truncates lists of the rearranged layout (as sptag_b200_spann_search). */
+typedef struct sptag_b200_spann_iterator* sptag_b200_spann_iter;
+int sptag_b200_spann_iterator_open(sptag_b200_spann_handle s, const void* queries, int32_t num_queries,
+                                   sptag_b200_spann_iter* out);
+int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int32_t* out_ids, float* out_dists,
+                                   int32_t* out_counts, uint8_t* out_relaxed_mono);
+void sptag_b200_spann_iterator_close(sptag_b200_spann_iter it);
 
 /* Labelset::Count(): tombstones set so far. */
 int32_t sptag_b200_num_deleted(sptag_b200_handle h);

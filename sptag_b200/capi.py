@@ -31,7 +31,8 @@ EXPORTS = [
     "sptag_b200_refine_search", "sptag_b200_refine_schedule", "sptag_b200_rebuild_graph", "sptag_b200_group_create", "sptag_b200_group_search",
     "sptag_b200_group_destroy", "sptag_b200_add", "sptag_b200_delete", "sptag_b200_delete_vectors", "sptag_b200_save",
     "sptag_b200_num_deleted", "sptag_b200_spann_load", "sptag_b200_spann_destroy", "sptag_b200_spann_search",
-    "sptag_b200_spann_set_param", "sptag_b200_spann_get_param",
+    "sptag_b200_spann_set_param", "sptag_b200_spann_get_param", "sptag_b200_spann_iterator_open",
+    "sptag_b200_spann_iterator_next", "sptag_b200_spann_iterator_close",
 ]
 
 
@@ -114,6 +115,11 @@ def lib():
         L.sptag_b200_spann_search.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.sptag_b200_spann_set_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p]
         L.sptag_b200_spann_get_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_int32]
+        L.sptag_b200_spann_iterator_open.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]
+        L.sptag_b200_spann_iterator_next.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                     C.c_void_p]
+        L.sptag_b200_spann_iterator_close.argtypes = [C.c_void_p]
+        L.sptag_b200_spann_iterator_close.restype = None
         for f in ("num_vectors", "dim", "value_type", "metric", "algo"):
             getattr(L, "sptag_b200_" + f).argtypes = [C.c_void_p]
         L.sptag_b200_last_error.restype = C.c_char_p
@@ -486,3 +492,41 @@ class B200SpannIndex:
         _check(lib().sptag_b200_spann_search(self._h, queries.ctypes.data, nq, k, ids.ctypes.data, dists.ctypes.data,
                                              stats.ctypes.data if want_stats else None))
         return (ids, dists, stats) if want_stats else (ids, dists)
+
+    def iterators(self, queries):
+        """SPANN::Index::GetIterator for a batch of HOST queries, one iterator per query."""
+        return B200SpannIterators(self, queries)
+
+
+class B200SpannIterators:
+    """A batch of SPANN ResultIterators (SPANNResultIterator.h): one resumable, deduplicated stream of posting elements per
+    query, state resident in HBM."""
+
+    def __init__(self, index, queries):
+        queries = np.ascontiguousarray(queries)
+        self.index = index           # the handle must outlive the iterators
+        self.nq = queries.shape[0]
+        h = C.c_void_p()
+        _check(lib().sptag_b200_spann_iterator_open(index._h, queries.ctypes.data, self.nq, C.byref(h)))
+        self._it = h
+
+    def next(self, batch):
+        """Next(batch) for every query -> (counts [nq], ids [nq, batch], dists [nq, batch], relaxed [nq] bool)."""
+        ids = np.empty((self.nq, batch), np.int32)
+        dists = np.empty((self.nq, batch), np.float32)
+        counts = np.empty(self.nq, np.int32)
+        relaxed = np.empty(self.nq, np.uint8)
+        _check(lib().sptag_b200_spann_iterator_next(self._it, batch, ids.ctypes.data, dists.ctypes.data,
+                                                    counts.ctypes.data, relaxed.ctypes.data))
+        return counts, ids, dists, relaxed.astype(bool)
+
+    def close(self):
+        if self._it:
+            lib().sptag_b200_spann_iterator_close(self._it)
+            self._it = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -6,6 +6,8 @@
 
 namespace sptag_b200 {
 
+struct IterState;  // search_kernels.cuh
+
 struct SpannScanParams {
     // head search results of every query, W per query, ascending, head-local ids (the head's m_results after SortResult)
     const int* head_ids;
@@ -44,5 +46,56 @@ cudaError_t launch_spann_scan(const SpannScanParams& p, bool cosine, int elem, i
 // Single-warp blocks of the scan kernel that fit on one SM with W results per query.
 int spann_scan_blocks_per_sm(bool cosine, int elem, int w);
 size_t spann_scan_smem(int w);
+
+// What a SPANN iterator keeps per query between launches (SPANNResultIterator's ExtraWorkSpace and the call in progress)
+struct SpannIterState {
+    int np, pi, offset;  // m_postingIDs.size(), m_pi, m_offset
+    int loaded;          // m_loadedPostingNum
+    int relaxed;         // m_relaxedMono
+    int load;            // m_loadPosting
+    int count, batch;    // the call in progress: resultCount and its batch (capped by slots)
+    int slots;           // the QueryResult's result count after the last call (SetResultNum); -1 before the first
+    int await_head;      // on the refill list: the head iterator was asked for its next batch since the last launch
+    int pad[2];
+};
+static_assert(sizeof(SpannIterState) == 48, "SpannIterState is 12 ints");
+
+// One launch of the posting step of SPANN iterators (SPANNIndex.cpp:261-296, :416-446; ExtraFullGraphSearcher.h:131-147,
+// :492-525).  A query runs until its call has `batch` results, its postings run out (it joins `refill`: the host asks the
+// head iterator for its next batch and launches again over that list), its head iterator found nothing (the call ends),
+// or its dedup table would pass half its capacity within the next chunk (it joins `susp`: the host doubles the table and
+// launches again over that list).  A query whose call ends writes its outputs.
+struct SpannIterParams {
+    const int* head_ids;  // [nq x hb] the head iterator's latest results, head-local ids
+    int nq, hb;
+    const unsigned int* list;  // the queries of this launch (kIterListHeader layout), or nullptr: all nq
+    int batch;                 // Next(batch) as the caller asked
+    int fresh;                 // the first launch of a Next: cap the batch by slots and Reset() the QueryResult
+    const unsigned char* queries;
+    size_t row_stride;
+    int dim, simd_width;
+    const long long* off;
+    const int* cnt;
+    const int* pages;
+    const int* ids;
+    const unsigned char* rows;
+    int vector_info_size;
+    int internal, page_limit;  // SearchInternalResultNum, the page limit in force
+    SpannIterState* st;
+    int* posts;                // [nq x hb] m_postingIDs
+    float* heap_d;             // [nq x cap] the call's QueryResult between launches
+    int* heap_v;
+    int cap;
+    unsigned int* const* tables;  // per query: its dedup table (the hashed visited-set format, vhash_home)
+    IterState* dedup;             // per query: vbits = log2 of its table's entries, vfill = ids in it
+    unsigned int* refill;         // kIterListHeader layout
+    unsigned int* susp;
+    int* out_ids;                 // [nq x batch]
+    float* out_dists;
+    int* out_counts;
+    unsigned char* out_relaxed;
+};
+cudaError_t launch_spann_iter_step(const SpannIterParams& p, bool cosine, int elem, int grid, cudaStream_t stream);
+int spann_iter_step_blocks_per_sm(bool cosine, int elem, int cap);
 
 }  // namespace sptag_b200

@@ -838,10 +838,13 @@ int fit_bfs_seeding(sptag_b200_iterator* it, int bfs) {
 // The grid stays the search kernel's.  launch(p, grid, smem, stream, iv) enqueues the iterate or nearest-first kernel;
 // `what` names k in the refusal.  On hashed visited sets the kernel leaves the queries that reached their table's limit
 // on a list: their tables grow (restart: they are replaced by empty ones) and the kernel runs again over that list,
-// until the list is empty.  Caller holds h->mu.
+// until the list is empty.  d_list (device, kIterListHeader layout, or nullptr for every query): the queries of the
+// first launch.  out_ids nullptr: the results stay in it->d_ids and the call returns without waiting for the last
+// launch.  Caller holds h->mu.
 template <typename LaunchFn>
 int run_iterator_step(sptag_b200_iterator* it, int k, const char* what, SearchLaunch& L, int32_t* out_ids,
-                      float* out_dists, int32_t* out_counts, uint8_t* out_relaxed_mono, bool restart, LaunchFn&& launch) {
+                      float* out_dists, int32_t* out_counts, uint8_t* out_relaxed_mono, bool restart, LaunchFn&& launch,
+                      const unsigned int* d_list = nullptr) {
     sptag_b200_index* h = it->h;
     if (it->topk_pad == 0) {  // the first Next creates the QueryResult: its size bounds every later batch
         it->topk_pad = topk_pad_for(k);
@@ -883,6 +886,7 @@ int run_iterator_step(sptag_b200_iterator* it, int k, const char* what, SearchLa
     cudaStream_t stream = nullptr;
     IterVisited iv = {};
     iv.margin = it->margin;
+    iv.list = d_list;
     if (it->hashed) {
         iv.tables = (unsigned int* const*)it->d_tables.ptr;
         iv.resume = (float*)it->d_resume.ptr;
@@ -924,13 +928,14 @@ int run_iterator_step(sptag_b200_iterator* it, int k, const char* what, SearchLa
     CUDA_OK(cudaEventRecord(h->ev_stop, stream));
     h->timed = true;
     if (int rc = scratch_release(h, stream)) return rc;
+    it->stepped = true;
+    if (!out_ids) return SPTAG_B200_SUCCESS;
     CUDA_OK(cudaMemcpyAsync(out_ids, it->d_ids.ptr, rn * 4, cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaMemcpyAsync(out_dists, it->d_dists.ptr, rn * 4, cudaMemcpyDeviceToHost, stream));
     if (out_counts) CUDA_OK(cudaMemcpyAsync(out_counts, it->d_counts.ptr, (size_t)it->nq * 4, cudaMemcpyDeviceToHost, stream));
     if (out_relaxed_mono)
         CUDA_OK(cudaMemcpyAsync(out_relaxed_mono, it->d_relaxed.ptr, (size_t)it->nq, cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaStreamSynchronize(stream));
-    it->stepped = true;
     return SPTAG_B200_SUCCESS;
 }
 
@@ -1988,11 +1993,13 @@ int sptag_b200_iterator_next(sptag_b200_iter it, int32_t batch, int32_t* out_ids
                              });
 }
 
-int sptag_b200_iterator_next_from_nearest(sptag_b200_iter it, int32_t k, int32_t* out_ids, float* out_dists,
-                                          uint8_t* out_found) {
-    if (!it || !it->h) return fail(SPTAG_B200_EMPTY_INDEX, "null iterator");
-    if (!out_ids || !out_dists) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
-    if (k < 1 || k > 1024) return fail(SPTAG_B200_LACK_OF_INPUTS, "k = %d outside [1, 1024]", k);
+}  // extern "C"
+
+namespace {
+
+// SearchIndexIterativeFromNeareast at k for the queries on d_list (nullptr: every query); k is checked by the caller.
+// The results are copied to out_ids / out_dists, or (nullptr) stay in it->d_ids / it->d_dists.
+int nearest_step(sptag_b200_iterator* it, int k, int32_t* out_ids, float* out_dists, const unsigned int* d_list) {
     const bool first = (it->nearest_k == 0);
     if (first && it->stepped)
         return fail(SPTAG_B200_LACK_OF_INPUTS, "the first SearchIndexIterativeFromNeareast call needs a freshly opened iterator");
@@ -2014,6 +2021,7 @@ int sptag_b200_iterator_next_from_nearest(sptag_b200_iter it, int32_t k, int32_t
         while (((size_t)1 << (need - 1)) < (size_t)k * (h->degree + 1)) ++need;
         if (int rc = fit_iter_tables(it, need)) return rc;
     }
+    bool reset_slots = !first;
     const int rc = run_iterator_step(
         it, k, "k", L, out_ids, out_dists, nullptr, nullptr, first,
         [&](const SearchParams& p, int grid, size_t smem, cudaStream_t stream, const IterVisited& iv) {
@@ -2022,19 +2030,35 @@ int sptag_b200_iterator_next_from_nearest(sptag_b200_iter it, int32_t k, int32_t
                 kfirst<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, iv);
             } else {
                 // the caller Reset()s a QueryResult that keeps its k slots (SPANNIndex.cpp:284): no cap from the previous
-                // count (once per call: a resume launch must not undo what its completed queries set)
-                if (!iv.list)
+                // count (once per call: a resume launch must not undo what its completed queries set).  Every query's
+                // cap is reset, listed or not: each of these calls resets it before the kernel reads it.
+                if (reset_slots)
                     CUDA_OK(cudaMemset2DAsync((char*)it->d_state.ptr + offsetof(IterState, slots), sizeof(IterState), 0xFF,
                                               sizeof(int), (size_t)it->nq, stream));
+                reset_slots = false;
                 CUDA_OK(cudaFuncSetAttribute((const void*)knext, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                 knext<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, (int*)it->d_counts.ptr, (unsigned char*)it->d_relaxed.ptr, iv);
             }
             return 0;
-        });
+        },
+        d_list);
     if (rc) return rc;
+    it->nearest_k = k;
+    return SPTAG_B200_SUCCESS;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sptag_b200_iterator_next_from_nearest(sptag_b200_iter it, int32_t k, int32_t* out_ids, float* out_dists,
+                                          uint8_t* out_found) {
+    if (!it || !it->h) return fail(SPTAG_B200_EMPTY_INDEX, "null iterator");
+    if (!out_ids || !out_dists) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    if (k < 1 || k > 1024) return fail(SPTAG_B200_LACK_OF_INPUTS, "k = %d outside [1, 1024]", k);
+    if (int rc = nearest_step(it, k, out_ids, out_dists, nullptr)) return rc;
     if (out_found)  // the reference's return value: is the first result slot a real vector
         for (int q = 0; q < it->nq; ++q) out_found[q] = out_ids[(size_t)q * k] >= 0 ? 1 : 0;
-    it->nearest_k = k;
     return SPTAG_B200_SUCCESS;
 }
 
@@ -2582,6 +2606,11 @@ struct sptag_b200_spann {
     int vector_limit_pages = 0;  // ceil(PostingVectorLimit * vis / PageSize): the least page limit in force
     int longest = 0;          // spann_update_shape
     bool truncated = false;
+    // iterators: IterativeSearchHeadBatch (ParameterDefinitionList.h:125), the first dedup table size (0 = from the
+    // lists), and what the last Next on this handle did
+    int head_batch = 32;
+    int dedup_entries = 0;
+    long last_iter_rounds = 0, last_iter_dedup_bytes = 0;
     DeviceBuffer d_translate, d_off, d_cnt, d_pages, d_ids, d_rows;
     // Host-buffer calls run on one of two staging sets, each with its own stream, head results, dedup tables and outputs,
     // so that two callers overlap; the head search kernels are ordered by the head handle (search_device_impl)
@@ -2673,6 +2702,7 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
     s->internal = atoi(get("BuildSSDIndex", "SearchInternalResultNum", "64").c_str());
     s->max_dist_ratio = strtof(get("BuildSSDIndex", "MaxDistRatio", "10000").c_str(), nullptr);
     s->page_limit = atoi(get("BuildSSDIndex", "SearchPostingPageLimit", "3").c_str());
+    s->head_batch = atoi(get("BuildSSDIndex", "IterativeSearchHeadBatch", "32").c_str());
     const long long vector_limit = atoll(get("BuildSSDIndex", "PostingVectorLimit", "118").c_str());
     s->vector_limit_pages = (int)((vector_limit * s->vis + 4095) / 4096);
     DeviceGuard guard(head->device);
@@ -2942,9 +2972,26 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
 int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, const char* value) {
     if (!s || !name || !value) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
     const std::string n(name);
-    if (n == "MaxCheck") return sptag_b200_set_param(s->head, name, value);  // the head's (SPANNIndex.cpp:901)
+    // the head's (SPANNIndex.cpp:901); the visited sets of the head iterators that SPANN iterators open
+    if (n == "MaxCheck" || n == "B200.IteratorVisitedSet" || n == "B200.IteratorVisitedHashEntries")
+        return sptag_b200_set_param(s->head, name, value);
     char* end = nullptr;
     std::lock_guard<std::mutex> lock(s->mu);
+    if (n == "IterativeSearchHeadBatch" || n == "B200.SpannDedupEntries") {
+        const long v = strtol(value, &end, 10);
+        if (end == value) return fail(SPTAG_B200_FAILED_PARSE_VALUE, "cannot parse '%s' for %s", value, name);
+        if (n == "IterativeSearchHeadBatch") {
+            if (v < 1 || v > 1024) return fail(SPTAG_B200_LACK_OF_INPUTS, "%s %ld outside [1, 1024]", name, v);
+            s->head_batch = (int)v;
+        } else {
+            if (v != 0 && (v < 64 || v > (1l << 30) || (v & (v - 1))))
+                return fail(SPTAG_B200_LACK_OF_INPUTS, "%s %ld is neither 0 nor a power of two in [64, 2^30]", name, v);
+            s->dedup_entries = (int)v;
+        }
+        return SPTAG_B200_SUCCESS;
+    }
+    if (n == "B200.LastIteratorRounds" || n == "B200.LastIteratorDedupBytes")
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "%s is read-only", name);
     if (n == "MaxDistRatio") {
         const float v = strtof(value, &end);
         if (end == value) return fail(SPTAG_B200_FAILED_PARSE_VALUE, "cannot parse '%s' for %s", value, name);
@@ -2966,9 +3013,14 @@ int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, cons
 int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char* value_out, int32_t capacity) {
     if (!s || !name || !value_out || capacity <= 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
     const std::string n(name);
-    if (n == "MaxCheck") return sptag_b200_get_param(s->head, name, value_out, capacity);
+    if (n == "MaxCheck" || n == "B200.IteratorVisitedSet" || n == "B200.IteratorVisitedHashEntries")
+        return sptag_b200_get_param(s->head, name, value_out, capacity);
     std::lock_guard<std::mutex> lock(s->mu);
     if (n == "MaxDistRatio") snprintf(value_out, (size_t)capacity, "%f", s->max_dist_ratio);
+    else if (n == "IterativeSearchHeadBatch") snprintf(value_out, (size_t)capacity, "%d", s->head_batch);
+    else if (n == "B200.SpannDedupEntries") snprintf(value_out, (size_t)capacity, "%d", s->dedup_entries);
+    else if (n == "B200.LastIteratorRounds") snprintf(value_out, (size_t)capacity, "%ld", s->last_iter_rounds);
+    else if (n == "B200.LastIteratorDedupBytes") snprintf(value_out, (size_t)capacity, "%ld", s->last_iter_dedup_bytes);
     else if (n == "SearchInternalResultNum") snprintf(value_out, (size_t)capacity, "%d", s->internal);
     else if (n == "SearchPostingPageLimit") snprintf(value_out, (size_t)capacity, "%d", s->page_limit);
     else if (n == "PostingBytes")
@@ -2976,6 +3028,240 @@ int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char
                                                          s->d_ids.bytes + s->d_rows.bytes);
     else return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
     return SPTAG_B200_SUCCESS;
+}
+
+}  // extern "C"
+
+// SPANN::Index<T>::GetIterator (SPANNIndex.cpp:299-314) for every query of a batch: the SPANNResultIterator's head
+// ResultIterator (an iterator on the head handle), its ExtraWorkSpace (SpannIterState, the chosen lists and the deduper)
+// and its QueryResult, kept in HBM between launches.
+struct sptag_b200_spann_iterator {
+    sptag_b200_spann* s = nullptr;
+    sptag_b200_iterator* head = nullptr;
+    int nq = 0, hb = 0;  // hb: IterativeSearchHeadBatch, sampled at open
+    int cap = 0;         // the QueryResult's size: the first Next's batch
+    DeviceBuffer d_queries, d_state, d_posts, d_heap_d, d_heap_v, d_refill[2], d_susp[2], d_ids, d_dists, d_counts,
+        d_relaxed;
+    // The dedup sets (OptHashPosVector, WorkSpace.h:43-165): exact sets that double when they fill, stored and grown as
+    // the head iterators' hashed visited sets are (grow_iter_visited); this iterator object holds only those tables.
+    sptag_b200_iterator dedup;
+};
+
+namespace {
+
+void spann_iterator_free(sptag_b200_spann_iterator* it) {
+    sptag_b200_iterator_close(it->head);
+    DeviceGuard guard(it->s->head->device);
+    delete it;  // frees the device buffers, with the index's device current
+}
+
+}  // namespace
+
+extern "C" {
+
+int sptag_b200_spann_iterator_open(sptag_b200_spann_handle s, const void* queries, int32_t num_queries,
+                                   sptag_b200_spann_iter* out) {
+    if (!s) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (!out || !queries || num_queries <= 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    *out = nullptr;
+    int hb = 0, entries = 0, longest = 0;
+    {
+        std::lock_guard<std::mutex> lock(s->mu);
+        hb = s->head_batch;
+        entries = s->dedup_entries;
+        longest = s->longest;
+    }
+    if (hb < 1 || hb > 1024) return fail(SPTAG_B200_LACK_OF_INPUTS, "IterativeSearchHeadBatch %d outside [1, 1024]", hb);
+    if (entries == 0) {  // the lists of one head batch at half load, at most 2^14 entries to start with
+        entries = 64;
+        while (entries < (1 << 14) && entries < 2ll * hb * longest) entries <<= 1;
+    }
+    int bits = 6;
+    while ((1 << bits) < entries) ++bits;
+    sptag_b200_index* h = s->head;
+    sptag_b200_iter head = nullptr;
+    // the head ResultIterator searches with p_searchDeleted = false (SPANNResultIterator.h:25)
+    if (int rc = sptag_b200_iterator_open_ex(h, queries, num_queries, 0, &head)) return rc;
+    auto* it = new sptag_b200_spann_iterator();
+    it->s = s;
+    it->head = head;
+    it->nq = num_queries;
+    it->hb = hb;
+    DeviceGuard guard(h->device);
+    const size_t nq = (size_t)num_queries, qrow = (size_t)h->dim * value_size(h->value_type);
+    sptag_b200_iterator& d = it->dedup;
+    d.nq = num_queries;
+    d.hashed = true;
+    d.visited_words = SIZE_MAX;  // a table never turns into a bitmap
+    d.vbufs.emplace_back();
+    d.vbuf_refs.push_back(num_queries);
+    int rc = 0;
+    if ((rc = it->d_queries.ensure(nq * h->row_stride)) || (rc = it->d_state.ensure(nq * sizeof(SpannIterState))) ||
+        (rc = it->d_posts.ensure(nq * hb * 4)) || (rc = it->d_refill[0].ensure((kIterListHeader + nq) * 4)) ||
+        (rc = it->d_refill[1].ensure((kIterListHeader + nq) * 4)) || (rc = it->d_susp[0].ensure((kIterListHeader + nq) * 4)) ||
+        (rc = it->d_susp[1].ensure((kIterListHeader + nq) * 4)) || (rc = it->d_counts.ensure(nq * 4)) ||
+        (rc = it->d_relaxed.ensure(nq)) || (rc = d.d_state.ensure(nq * sizeof(IterState))) ||
+        (rc = d.d_tables.ensure(nq * sizeof(unsigned int*))) || (rc = d.vbufs[0].ensure(nq * entries * 4))) {
+        spann_iterator_free(it);
+        return rc;
+    }
+    d.q_bits.assign(nq, bits);
+    d.q_buf.assign(nq, 0);
+    d.q_set.resize(nq);
+    for (size_t q = 0; q < nq; ++q) d.q_set[q] = (unsigned int*)d.vbufs[0].ptr + q * entries;
+    // GetIterator: relaxedMono = false, loadedPostingNum = 0, an empty deduper and posting list; the first head batch
+    // is loaded by the first Next
+    SpannIterState st0 = {};
+    st0.load = 1;
+    st0.slots = -1;
+    IterState ds0 = {};
+    ds0.vbits = bits;
+    const std::vector<SpannIterState> st(nq, st0);
+    const std::vector<IterState> ds(nq, ds0);
+    cudaError_t e = cudaMemset(it->d_queries.ptr, 0, it->d_queries.bytes);  // rows of the head's stride, zero padded
+    if (e == cudaSuccess)
+        e = cudaMemcpy2D(it->d_queries.ptr, h->row_stride, queries, qrow, qrow, nq, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemset(d.vbufs[0].ptr, 0, d.vbufs[0].bytes);
+    if (e == cudaSuccess) e = cudaMemcpy(d.d_tables.ptr, d.q_set.data(), nq * sizeof(unsigned int*), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(d.d_state.ptr, ds.data(), nq * sizeof(IterState), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(it->d_state.ptr, st.data(), nq * sizeof(SpannIterState), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        spann_iterator_free(it);
+        return fail(SPTAG_B200_FAIL, "SPANN iterator set-up failed: %s", cudaGetErrorString(e));
+    }
+    *out = it;
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int32_t* out_ids, float* out_dists,
+                                   int32_t* out_counts, uint8_t* out_relaxed_mono) {
+    if (!it || !it->s) return fail(SPTAG_B200_EMPTY_INDEX, "null iterator");
+    if (!out_ids || !out_dists || !out_counts || !out_relaxed_mono) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    if (batch < 1 || batch > 1024) return fail(SPTAG_B200_LACK_OF_INPUTS, "batch = %d outside [1, 1024]", batch);
+    sptag_b200_spann* s = it->s;
+    sptag_b200_index* h = s->head;
+    SpannIterParams p;
+    memset(&p, 0, sizeof(p));
+    bool truncated = false;
+    {
+        std::lock_guard<std::mutex> lock(s->mu);
+        p.internal = s->internal;
+        p.page_limit = spann_page_limit(s);
+        truncated = s->truncated;
+    }
+    // The reference has SearchInternalResultNum page buffers and indexes them by m_pi (IExtraSearcher.h:114-122,
+    // ExtraFullGraphSearcher.h:405, :500): a load of more lists is undefined there
+    if (it->hb > p.internal)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "IterativeSearchHeadBatch %d exceeds SearchInternalResultNum %d", it->hb,
+                    p.internal);
+    if (truncated && s->rearranged)  // as sptag_b200_spann_search
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchPostingPageLimit %d truncates posting lists of the rearranged layout",
+                    p.page_limit);
+    DeviceGuard guard(h->device);
+    cudaStream_t stream = nullptr;  // the stream of the head iterator's steps
+    const size_t nq = (size_t)it->nq;
+    if (it->cap == 0) {  // the first Next creates the QueryResult: its size bounds every later batch
+        if (int rc = it->d_heap_d.ensure(nq * batch * 4)) return rc;
+        if (int rc = it->d_heap_v.ensure(nq * batch * 4)) return rc;
+        it->cap = batch;
+    }
+    if (int rc = it->d_ids.ensure(nq * batch * 4)) return rc;
+    if (int rc = it->d_dists.ensure(nq * batch * 4)) return rc;
+    const bool cosine = h->metric != SPTAG_B200_METRIC_L2;
+    int elem = 0;
+    with_elem(h, [&](auto el) { elem = el; });
+    const int per_sm = spann_iter_step_blocks_per_sm(cosine, elem, it->cap);
+    if (per_sm < 1) return fail(SPTAG_B200_MEMORY_OVERFLOW, "the posting step kernel does not fit on an SM");
+    const long long max_grid = (long long)h->num_sms * per_sm;
+    // SearchIndexIterative's first call: the head's FromNeareast(first = true) at the head batch (SPANNIndex.cpp:271-275)
+    if (!it->head->stepped)
+        if (int rc = nearest_step(it->head, it->hb, nullptr, nullptr, nullptr)) return rc;
+    sptag_b200_iterator& d = it->dedup;
+    p.head_ids = (const int*)it->head->d_ids.ptr;
+    p.nq = it->nq;
+    p.hb = it->hb;
+    p.batch = batch;
+    p.fresh = 1;
+    p.queries = (const unsigned char*)it->d_queries.ptr;
+    p.row_stride = h->row_stride;
+    p.dim = h->dim;
+    p.simd_width = h->simd_width;
+    p.off = (const long long*)s->d_off.ptr;
+    p.cnt = (const int*)s->d_cnt.ptr;
+    p.pages = (const int*)s->d_pages.ptr;
+    p.ids = (const int*)s->d_ids.ptr;
+    p.rows = (const unsigned char*)s->d_rows.ptr;
+    p.vector_info_size = s->vis;
+    p.st = (SpannIterState*)it->d_state.ptr;
+    p.posts = (int*)it->d_posts.ptr;
+    p.heap_d = (float*)it->d_heap_d.ptr;
+    p.heap_v = (int*)it->d_heap_v.ptr;
+    p.cap = it->cap;
+    p.tables = (unsigned int* const*)d.d_tables.ptr;
+    p.dedup = (IterState*)d.d_state.ptr;
+    p.out_ids = (int*)it->d_ids.ptr;
+    p.out_dists = (float*)it->d_dists.ptr;
+    p.out_counts = (int*)it->d_counts.ptr;
+    p.out_relaxed = (unsigned char*)it->d_relaxed.ptr;
+    auto lists = [&](int refill, int susp, bool clear_refill) -> int {
+        p.refill = (unsigned int*)it->d_refill[refill].ptr;
+        p.susp = (unsigned int*)it->d_susp[susp].ptr;
+        if (clear_refill) CUDA_OK(cudaMemsetAsync(p.refill, 0, kIterListHeader * 4, stream));
+        CUDA_OK(cudaMemsetAsync(p.susp, 0, kIterListHeader * 4, stream));
+        return 0;
+    };
+    auto launch = [&](long long n) -> int {
+        const cudaError_t e = launch_spann_iter_step(p, cosine, elem, (int)std::min(n, max_grid), stream);
+        g_launches++;
+        if (e != cudaSuccess) return fail(SPTAG_B200_FAIL, "posting step launch failed: %s", cudaGetErrorString(e));
+        return 0;
+    };
+    // Rounds: the posting step over the queries of the round; queries whose tables must grow run again (same round);
+    // then the head's FromNeareast(false) for the queries whose postings ran out, and the posting step over those.
+    int cur = 0, scur = 0;
+    if (int rc = lists(cur, scur, true)) return rc;
+    if (int rc = launch(it->nq)) return rc;
+    p.fresh = 0;
+    long rounds = 0;
+    for (;;) {
+        unsigned hdr[2][kIterListHeader];
+        CUDA_OK(cudaMemcpyAsync(hdr[0], p.refill, sizeof(hdr[0]), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaMemcpyAsync(hdr[1], p.susp, sizeof(hdr[1]), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        if (hdr[1][0] > 0) {  // double the listed tables and run those queries on (they append to the same refill list)
+            std::vector<unsigned> qs(hdr[1][0]);
+            CUDA_OK(cudaMemcpy(qs.data(), (unsigned*)p.susp + kIterListHeader, qs.size() * 4, cudaMemcpyDeviceToHost));
+            std::vector<int> bits(qs.size());
+            for (size_t i = 0; i < qs.size(); ++i) bits[i] = d.q_bits[qs[i]] + 1;
+            if (int rc = grow_iter_visited(&d, qs, bits, true, stream)) return rc;
+            p.list = p.susp;
+            scur ^= 1;
+            if (int rc = lists(cur, scur, false)) return rc;
+            if (int rc = launch(hdr[1][0])) return rc;
+            continue;
+        }
+        if (hdr[0][0] == 0) break;
+        // SearchIndexIterativeFromNeareast(head, false) for the queries on the refill list (SPANNIndex.cpp:281-285)
+        if (int rc = nearest_step(it->head, it->hb, nullptr, nullptr, p.refill)) return rc;
+        ++rounds;
+        p.list = p.refill;
+        cur ^= 1;
+        if (int rc = lists(cur, scur, true)) return rc;
+        if (int rc = launch(hdr[0][0])) return rc;
+    }
+    CUDA_OK(cudaMemcpyAsync(out_ids, it->d_ids.ptr, nq * batch * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaMemcpyAsync(out_dists, it->d_dists.ptr, nq * batch * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaMemcpyAsync(out_counts, it->d_counts.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaMemcpyAsync(out_relaxed_mono, it->d_relaxed.ptr, nq, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    std::lock_guard<std::mutex> lock(s->mu);
+    s->last_iter_rounds = rounds;
+    s->last_iter_dedup_bytes = (long)d.visited_bytes();
+    return SPTAG_B200_SUCCESS;
+}
+
+void sptag_b200_spann_iterator_close(sptag_b200_spann_iter it) {
+    if (it) spann_iterator_free(it);
 }
 
 }  // extern "C"
