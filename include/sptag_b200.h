@@ -427,6 +427,40 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
                                    int32_t* out_counts, uint8_t* out_relaxed_mono);
 void sptag_b200_spann_iterator_close(sptag_b200_spann_iter it);
 
+/* ---- Multi-index scan ----
+ * Replaces: MultiIndexScan::Init(indexes, targets, weight, k, useTimer = false, termCondVal, searchLimit), Next until it
+ * returns false, and Close (inc/Core/MultiIndexScan.h, src/Core/MultiIndexScan.cpp:51-183) for every query of a HOST
+ * batch: the k ids with the smallest weighted sum of per-index distances, over indexes that hold the same ids (for example
+ * an image and a text embedding of each item).  Per query, an iterator with p_searchDeleted = true is opened on every
+ * index; each round asks every index in order for Next(1) and scores an id not seen before as
+ * sum_i weight[i] * dist_i(target_i, id), with GetDistance for the indexes that did not return it; the score enters the
+ * top-k unless the queue is full and its largest score is <= it, which counts a consecutive drop.  The round that finds an
+ * iterator empty ends the query at that index.  After a round the query ends when the consecutive drops reach term_cond
+ * (compared unsigned: a negative value never ends by drops), or else when the ids seen reach search_limit (compared as
+ * size_t: a negative value never ends by size).  Results equal the reference's bit for bit, including which of equal
+ * scores is kept and their output order (libstdc++'s heap), and the score's rounding as GCC compiles WeightedRankFunc
+ * for x86-64-v3 (rounded products added one after another in blocks of 8 and 4, the last num_indexes % 4 terms fused).
+ *   queries[i]: HOST, num_queries rows of index i's dimension and value type; the indexes may differ in dimension, value
+ *               type and metric.
+ *   weights:    num_indexes floats, or NULL for the plain sum (rankFunc, MultiIndexScan.cpp:37-39), which equals unit
+ *               weights bit for bit.
+ *   out_ids / out_scores: HOST [num_queries x k] in the order Next returns them (smallest score first, Dist = score);
+ *               unfilled slots (-1, MaxDist).  out_counts[q]: the number of results.
+ *   out_stats:  HOST [num_queries x 4] int32 or NULL: rounds run, seenSet.size(), consecutive_drops at the end, and why the
+ *               query ended (SPTAG_B200_MS_END_*; SPTAG_B200_MS_END_EXHAUSTED + i: iterator i returned nothing).
+ * The timer form (useTimer = true) is not offered: a wall-clock limit does not give reproducible results.  A user rank
+ * function cannot run on the device either.  The handles are not changed: their iterators are opened and closed inside
+ * the call, so they can be mutated again when it returns.
+ * LackOfInputs: null arguments, num_indexes outside [1, 16], k outside [1, 1024], handles that differ in device, vector
+ * count or id offset, and quantized handles.  Fail: a KDT handle (GetIterator on KDT).  Blocking. */
+#define SPTAG_B200_MS_STATS_PER_QUERY 4
+#define SPTAG_B200_MS_END_DROPS 0
+#define SPTAG_B200_MS_END_LIMIT 1
+#define SPTAG_B200_MS_END_EXHAUSTED 2
+int sptag_b200_multi_scan(const sptag_b200_handle* indexes, int32_t num_indexes, const void* const* queries,
+                          const float* weights, int32_t num_queries, int32_t k, int32_t term_cond, int32_t search_limit,
+                          int32_t* out_ids, float* out_scores, int32_t* out_counts, int32_t* out_stats);
+
 /* Labelset::Count(): tombstones set so far. */
 int32_t sptag_b200_num_deleted(sptag_b200_handle h);
 

@@ -13,6 +13,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SPTAG_B200_LIB", os.path.join(_HERE, "lib", "libsptag_b200.so"))
 
 STATS_PER_QUERY = 8
+# multi_scan stats per query: rounds, ids seen, consecutive drops at the end, why it ended (MS_END_EXHAUSTED + i: index i)
+MS_ROUNDS, MS_SEEN, MS_DROPS, MS_END = range(4)
+MS_END_DROPS, MS_END_LIMIT, MS_END_EXHAUSTED = 0, 1, 2
 ST_CHECKED, ST_TREE_CHECKED, ST_NG_LEFT, ST_SPT_LEFT, ST_NDIST, ST_NEXPAND, ST_NTREE, ST_FLAGS = range(8)
 
 VT_INT8, VT_UINT8, VT_INT16, VT_FLOAT = 0, 1, 2, 3
@@ -32,7 +35,7 @@ EXPORTS = [
     "sptag_b200_group_destroy", "sptag_b200_add", "sptag_b200_delete", "sptag_b200_delete_vectors", "sptag_b200_save",
     "sptag_b200_num_deleted", "sptag_b200_spann_load", "sptag_b200_spann_destroy", "sptag_b200_spann_search",
     "sptag_b200_spann_set_param", "sptag_b200_spann_get_param", "sptag_b200_spann_iterator_open",
-    "sptag_b200_spann_iterator_next", "sptag_b200_spann_iterator_close",
+    "sptag_b200_spann_iterator_next", "sptag_b200_spann_iterator_close", "sptag_b200_multi_scan",
 ]
 
 
@@ -120,6 +123,9 @@ def lib():
                                                      C.c_void_p]
         L.sptag_b200_spann_iterator_close.argtypes = [C.c_void_p]
         L.sptag_b200_spann_iterator_close.restype = None
+        L.sptag_b200_multi_scan.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(C.c_void_p), C.c_void_p, C.c_int32,
+                                            C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]
         for f in ("num_vectors", "dim", "value_type", "metric", "algo"):
             getattr(L, "sptag_b200_" + f).argtypes = [C.c_void_p]
         L.sptag_b200_last_error.restype = C.c_char_p
@@ -530,3 +536,31 @@ class B200SpannIterators:
             self.close()
         except Exception:
             pass
+
+
+def multi_scan(indexes, queries, k, *, term_cond, search_limit, weights=None, want_stats=False):
+    """MultiIndexScan (Init + Next until false) for a batch: the k ids with the smallest weighted sum of per-index
+    distances over B200Index handles that hold the same ids.  queries[i]: [nq x dim_i] of index i's value type;
+    weights: one float per index or None for the plain sum.  term_cond / search_limit as the reference's termCondVal /
+    searchLimit, required as the reference has no defaults (negative: never ends that way; with both negative every
+    query runs until an iterator is exhausted).  -> (ids [nq x k], scores [nq x k], counts [nq][, stats [nq x 4]])"""
+    n = len(indexes)
+    qs = [np.ascontiguousarray(q) for q in queries]
+    if len(qs) != n or n == 0:
+        raise ValueError("one query array per index")
+    nq = qs[0].shape[0]
+    if any(q.shape[0] != nq for q in qs):
+        raise ValueError("every query array needs the same number of rows")
+    hs = (C.c_void_p * n)(*[ix._h.value for ix in indexes])
+    qp = (C.c_void_p * n)(*[q.ctypes.data for q in qs])
+    w = None if weights is None else np.ascontiguousarray(weights, np.float32)
+    if w is not None and w.shape != (n,):
+        raise ValueError("one weight per index")
+    ids = np.empty((nq, k), np.int32)
+    scores = np.empty((nq, k), np.float32)
+    counts = np.empty(nq, np.int32)
+    stats = np.empty((nq, 4), np.int32) if want_stats else None
+    _check(lib().sptag_b200_multi_scan(hs, n, qp, None if w is None else w.ctypes.data, nq, k, term_cond, search_limit,
+                                       ids.ctypes.data, scores.ctypes.data, counts.ctypes.data,
+                                       None if stats is None else stats.ctypes.data))
+    return (ids, scores, counts, stats) if want_stats else (ids, scores, counts)

@@ -8,6 +8,7 @@
 #include "../../include/sptag_b200.h"
 #include "aux_kernels.cuh"
 #include "kernel_select.h"
+#include "multi_scan.h"
 #include "spann_scan.h"
 
 #include <algorithm>
@@ -1970,11 +1971,14 @@ int sptag_b200_iterator_open_ex(sptag_b200_handle h, const void* queries, int32_
     return SPTAG_B200_SUCCESS;
 }
 
-int sptag_b200_iterator_next(sptag_b200_iter it, int32_t batch, int32_t* out_ids, float* out_dists, int32_t* out_counts,
-                             uint8_t* out_relaxed_mono) {
-    if (!it || !it->h) return fail(SPTAG_B200_EMPTY_INDEX, "null iterator");
-    if (!out_ids || !out_dists) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
-    if (batch < 1 || batch > 1024) return fail(SPTAG_B200_LACK_OF_INPUTS, "batch = %d outside [1, 1024]", batch);
+}  // extern "C"
+
+namespace {
+
+// ResultIterator::Next(batch) for the queries on d_list (nullptr: every query); batch is checked by the caller.
+// out_ids nullptr: the results stay in it->d_ids / d_dists / d_counts, and the call does not wait for the last launch.
+int next_step(sptag_b200_iterator* it, int batch, int32_t* out_ids, float* out_dists, int32_t* out_counts,
+              uint8_t* out_relaxed_mono, const unsigned int* d_list) {
     sptag_b200_index* h = it->h;
     std::lock_guard<std::mutex> lock(h->mu);
     DeviceGuard guard(h->device);
@@ -1990,7 +1994,20 @@ int sptag_b200_iterator_next(sptag_b200_iter it, int32_t batch, int32_t* out_ids
                                  kern<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, (int*)it->d_counts.ptr,
                                                                   (unsigned char*)it->d_relaxed.ptr, iv);
                                  return 0;
-                             });
+                             },
+                             d_list);
+}
+
+}  // namespace
+
+extern "C" {
+
+int sptag_b200_iterator_next(sptag_b200_iter it, int32_t batch, int32_t* out_ids, float* out_dists, int32_t* out_counts,
+                             uint8_t* out_relaxed_mono) {
+    if (!it || !it->h) return fail(SPTAG_B200_EMPTY_INDEX, "null iterator");
+    if (!out_ids || !out_dists) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    if (batch < 1 || batch > 1024) return fail(SPTAG_B200_LACK_OF_INPUTS, "batch = %d outside [1, 1024]", batch);
+    return next_step(it, batch, out_ids, out_dists, out_counts, out_relaxed_mono, nullptr);
 }
 
 }  // extern "C"
@@ -3262,6 +3279,191 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
 
 void sptag_b200_spann_iterator_close(sptag_b200_spann_iter it) {
     if (it) spann_iterator_free(it);
+}
+
+}  // extern "C"
+
+// ---- Multi-index scan ----
+
+namespace {
+
+// The per-index iterators of one multi-index scan, closed when the call returns however it returns
+struct ScanIterators {
+    std::vector<sptag_b200_iter> its;
+    ~ScanIterators() {
+        for (sptag_b200_iter it : its) sptag_b200_iterator_close(it);
+    }
+};
+
+}  // namespace
+
+extern "C" {
+
+int sptag_b200_multi_scan(const sptag_b200_handle* indexes, int32_t num_indexes, const void* const* queries,
+                          const float* weights, int32_t num_queries, int32_t k, int32_t term_cond, int32_t search_limit,
+                          int32_t* out_ids, float* out_scores, int32_t* out_counts, int32_t* out_stats) {
+    if (!indexes || !queries || !out_ids || !out_scores || !out_counts || num_queries <= 0)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    if (num_indexes < 1 || num_indexes > kMultiScanMaxIndexes)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "num_indexes = %d outside [1, %d]", num_indexes, kMultiScanMaxIndexes);
+    if (k < 1 || k > 1024) return fail(SPTAG_B200_LACK_OF_INPUTS, "k = %d outside [1, 1024]", k);
+    const int n = num_indexes;
+    for (int i = 0; i < n; ++i)
+        if (!indexes[i] || !queries[i]) return fail(SPTAG_B200_LACK_OF_INPUTS, "null handle or query buffer of index %d", i);
+    sptag_b200_index* h0 = indexes[0];
+    for (int i = 0; i < n; ++i) {
+        sptag_b200_index* h = indexes[i];
+        if (h->algo != SPTAG_B200_ALGO_BKT) return fail(SPTAG_B200_FAIL, "ITERATIVE NOT SUPPORT FOR KDT");
+        if (h->q_type != 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "iterators on quantized indexes are not built");
+        std::lock_guard<std::mutex> lock(h->mu);
+        // GetDistance(target_j, vid) reads row vid of every index: they must hold the same ids
+        if (h->device != h0->device || h->n != h0->n || h->id_offset != h0->id_offset)
+            return fail(SPTAG_B200_LACK_OF_INPUTS, "index %d differs from index 0 in device, vector count or id offset", i);
+    }
+    // Init: GetIterator(target_i, true) on every index
+    ScanIterators iters;
+    for (int i = 0; i < n; ++i) {
+        sptag_b200_iter it = nullptr;
+        if (int rc = sptag_b200_iterator_open_ex(indexes[i], queries[i], num_queries, 1, &it)) return rc;
+        iters.its.push_back(it);
+    }
+    DeviceGuard guard(h0->device);
+    cudaStream_t stream = nullptr;  // the stream of the iterator steps
+    const size_t nq = (size_t)num_queries;
+    std::vector<DeviceBuffer> d_q(n);
+    DeviceBuffer d_cross, d_state, d_heap_s, d_heap_v, d_list[2], d_ids, d_scores, d_counts, d_stats;
+    // seenSet: one table per query in the hashed visited-set format, doubled with grow_iter_visited; this object holds
+    // only those tables
+    sptag_b200_iterator seen;
+    seen.nq = num_queries;
+    seen.hashed = true;
+    seen.visited_words = SIZE_MAX;  // a table never turns into a bitmap
+    seen.vbufs.emplace_back();
+    seen.vbuf_refs.push_back(num_queries);
+    int bits = 7;
+    int rc = 0;
+    for (int i = 0; i < n && !rc; ++i) rc = d_q[i].ensure(nq * indexes[i]->row_stride);
+    if (rc || (rc = d_cross.ensure(nq * n * n * 4)) || (rc = d_state.ensure(nq * sizeof(MultiScanState))) ||
+        (rc = d_heap_s.ensure(nq * k * 4)) || (rc = d_heap_v.ensure(nq * k * 4)) ||
+        (rc = d_list[0].ensure((kIterListHeader + nq) * 4)) || (rc = d_list[1].ensure((kIterListHeader + nq) * 4)) ||
+        (rc = d_ids.ensure(nq * k * 4)) || (rc = d_scores.ensure(nq * k * 4)) || (rc = d_counts.ensure(nq * 4)) ||
+        (rc = d_stats.ensure(nq * 16)) || (rc = seen.d_state.ensure(nq * sizeof(IterState))) ||
+        (rc = seen.d_tables.ensure(nq * sizeof(unsigned int*))) || (rc = seen.vbufs[0].ensure(nq * (4u << bits))))
+        return rc;
+    seen.q_bits.assign(nq, bits);
+    seen.q_buf.assign(nq, 0);
+    seen.q_set.resize(nq);
+    for (size_t q = 0; q < nq; ++q) seen.q_set[q] = (unsigned int*)seen.vbufs[0].ptr + (q << bits);
+    IterState ss0 = {};
+    ss0.vbits = bits;
+    const std::vector<IterState> ss(nq, ss0);
+    const std::vector<MultiScanState> st(nq, MultiScanState{0, 0, -1, 0});
+    std::vector<unsigned> list0(kIterListHeader + nq, 0);
+    list0[0] = (unsigned)nq;
+    for (size_t q = 0; q < nq; ++q) list0[kIterListHeader + q] = (unsigned)q;
+    for (int i = 0; i < n; ++i) {  // rows of the index's stride, zero padded, as the distance reads them
+        const sptag_b200_index* h = indexes[i];
+        const size_t qrow = (size_t)h->dim * value_size(h->value_type);
+        CUDA_OK(cudaMemset(d_q[i].ptr, 0, d_q[i].bytes));
+        CUDA_OK(cudaMemcpy2D(d_q[i].ptr, h->row_stride, queries[i], qrow, qrow, nq, cudaMemcpyHostToDevice));
+    }
+    CUDA_OK(cudaMemset(seen.vbufs[0].ptr, 0, seen.vbufs[0].bytes));
+    CUDA_OK(cudaMemcpy(seen.d_tables.ptr, seen.q_set.data(), nq * sizeof(unsigned int*), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(seen.d_state.ptr, ss.data(), nq * sizeof(IterState), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(d_state.ptr, st.data(), nq * sizeof(MultiScanState), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(d_list[0].ptr, list0.data(), list0.size() * 4, cudaMemcpyHostToDevice));
+
+    MultiScanRound c;
+    memset(&c, 0, sizeof(c));
+    MultiScanMergeParams mp;
+    memset(&mp, 0, sizeof(mp));
+    mp.n = n;
+    mp.k = k;
+    mp.id_offset = h0->id_offset;
+    mp.term_cond = (unsigned int)term_cond;
+    mp.search_limit = (unsigned long long)(long long)search_limit;
+    for (int i = 0; i < n; ++i) mp.weight[i] = weights ? weights[i] : 1.0f;  // rankFunc's sum equals unit weights
+    mp.cross = (const float*)d_cross.ptr;
+    mp.st = (MultiScanState*)d_state.ptr;
+    mp.heap_s = (float*)d_heap_s.ptr;
+    mp.heap_v = (int*)d_heap_v.ptr;
+    mp.tables = (unsigned int* const*)seen.d_tables.ptr;
+    mp.seen = (IterState*)seen.d_state.ptr;
+    const int max_grid = std::max(1, h0->num_sms) * 32;
+    long long rounds = 0;
+    unsigned active = (unsigned)nq;
+    for (int cur = 0; active > 0; cur ^= 1, ++rounds) {
+        // every running query has run `rounds` rounds and this one inserts at most n ids, and no table holds more than the
+        // index's ids: keep every table below half load
+        const long long fill_bound = std::min<long long>((long long)n * (rounds + 1), (long long)h0->n);
+        if (fill_bound > (1ll << (bits - 1))) {
+            std::vector<unsigned> qs(active);
+            CUDA_OK(cudaMemcpy(qs.data(), (unsigned*)d_list[cur].ptr + kIterListHeader, active * 4, cudaMemcpyDeviceToHost));
+            while (fill_bound > (1ll << (bits - 1))) ++bits;
+            if (bits > 30) return fail(SPTAG_B200_MEMORY_OVERFLOW, "seen-set table of 2^%d entries", bits);
+            const std::vector<int> nb(active, bits);
+            if (int rc2 = grow_iter_visited(&seen, qs, nb, true, stream)) return rc2;
+        }
+        const unsigned* list = (const unsigned*)d_list[cur].ptr;
+        for (int i = 0; i < n; ++i)  // Next(1) on every index
+            if (int rc2 = next_step(iters.its[i], 1, nullptr, nullptr, nullptr, nullptr, list)) return rc2;
+        const int grid = (int)std::min<long long>(active, max_grid);
+        for (int i = 0; i < n; ++i) {  // the step's results: [nq x 1], allocated by the first step
+            c.ids[i] = (const int*)iters.its[i]->d_ids.ptr;
+            c.dists[i] = (const float*)iters.its[i]->d_dists.ptr;
+            c.counts[i] = (const int*)iters.its[i]->d_counts.ptr;
+        }
+        for (int j = 0; j < n && n > 1; ++j) {  // GetDistance(target_j, vid) for the other indexes' candidates
+            const sptag_b200_index* h = indexes[j];
+            MultiScanDistParams dp;
+            dp.list = list;
+            dp.n = n;
+            dp.target = j;
+            dp.id_offset = h0->id_offset;
+            dp.c = c;
+            dp.queries = (const unsigned char*)d_q[j].ptr;
+            dp.rows = (const unsigned char*)h->d_vectors.ptr;
+            dp.row_stride = h->row_stride;
+            dp.dim = h->dim;
+            dp.simd_width = h->simd_width;
+            dp.cross = (float*)d_cross.ptr;
+            int elem = 0;
+            with_elem(h, [&](auto el) { elem = el; });
+            const cudaError_t e = launch_multi_scan_distance(dp, h->metric != SPTAG_B200_METRIC_L2, elem, grid, stream);
+            g_launches++;
+            if (e != cudaSuccess) return fail(SPTAG_B200_FAIL, "multi-scan distance launch failed: %s", cudaGetErrorString(e));
+        }
+        mp.c = c;
+        mp.list = list;
+        mp.next = (unsigned*)d_list[cur ^ 1].ptr;
+        CUDA_OK(cudaMemsetAsync(mp.next, 0, kIterListHeader * 4, stream));
+        const cudaError_t e = launch_multi_scan_merge(mp, grid, stream);
+        g_launches++;
+        if (e != cudaSuccess) return fail(SPTAG_B200_FAIL, "multi-scan merge launch failed: %s", cudaGetErrorString(e));
+        CUDA_OK(cudaMemcpyAsync(&active, mp.next, 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+    }
+    MultiScanDrainParams dr;
+    dr.nq = num_queries;
+    dr.k = k;
+    dr.id_offset = h0->id_offset;
+    dr.st = (MultiScanState*)d_state.ptr;
+    dr.seen = (const IterState*)seen.d_state.ptr;
+    dr.heap_s = (float*)d_heap_s.ptr;
+    dr.heap_v = (int*)d_heap_v.ptr;
+    dr.out_ids = (int*)d_ids.ptr;
+    dr.out_scores = (float*)d_scores.ptr;
+    dr.out_counts = (int*)d_counts.ptr;
+    dr.out_stats = (int*)d_stats.ptr;
+    const cudaError_t e = launch_multi_scan_drain(dr, (int)std::min<long long>((long long)nq, max_grid), stream);
+    g_launches++;
+    if (e != cudaSuccess) return fail(SPTAG_B200_FAIL, "multi-scan drain launch failed: %s", cudaGetErrorString(e));
+    CUDA_OK(cudaMemcpyAsync(out_ids, d_ids.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaMemcpyAsync(out_scores, d_scores.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaMemcpyAsync(out_counts, d_counts.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
+    if (out_stats) CUDA_OK(cudaMemcpyAsync(out_stats, d_stats.ptr, nq * 16, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    return SPTAG_B200_SUCCESS;
 }
 
 }  // extern "C"
