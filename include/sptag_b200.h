@@ -136,13 +136,19 @@ void sptag_b200_destroy(sptag_b200_handle h);
  * MaxCheckForRefineGraph)) + 2) entries per query slot, at least 64, independent of the number of vectors; a query that fills half of
  * it is searched again on a bitmap by a second launch on the same stream; results are identical in every mode),
  * B200.VisitedHashEntries (table entries per slot: 0 = the default above, otherwise a power of two in [64, 2^30]).
+ * B200.RowSketch (-1 auto, 0 off, 1 on: a 1-byte-per-dimension copy of the rows of a float BKT index, dim + 16 bytes per
+ * vector of device memory, built on the device from the rows before the next search; BKT search reads it to prove that
+ * m_Results rejects a graph neighbour and then does not fetch that neighbour's row; results and per-query counters are
+ * identical in every mode; auto = on for rows of 2 KB or more unless the array does not fit; off with EnableBfs; 1 returns
+ * LackOfInputs on KDT, integer and quantized indexes).
  * B200.VisitedSet governs search only.  Iterators: B200.IteratorVisitedSet (-1 auto: a bitmap over the index per open
  * iterator query unless the iterator's bitmaps fail to allocate for lack of device memory, then hashed; 0 bitmap;
  * 1 hashed: per query a hash table that grows as the scan proceeds and becomes a bitmap when it would outgrow one;
  * results are identical in every mode; an open iterator keeps the mode it was opened with),
  * B200.IteratorVisitedHashEntries (initial table entries per query: 0 = the default above, otherwise a power of two in
  * [64, 2^30]; raised to what one search step needs).
- * Read-only: B200.LastVisitedOverflows (queries the hashed set handed to the bitmap re-run in the last blocking search
+ * Read-only: B200.RowsSkipped (graph neighbours whose row the finished searches of this handle did not fetch, summed
+ * since the handle was made), B200.LastVisitedOverflows (queries the hashed set handed to the bitmap re-run in the last blocking search
  * call of this handle; 0 on the bitmap), B200.ScratchBytes (device bytes held by the handle's search scratch sets),
  * B200.LastIteratorSuspensions ("step,trees": how often the last iterator call suspended a query at the top of a step /
  * before a tree pop to grow its table), B200.LastIteratorGrowths (tables grown or restarted by that call),

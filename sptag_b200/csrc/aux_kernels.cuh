@@ -145,6 +145,17 @@ __global__ void normalize_rows_kernel(unsigned char* vectors, unsigned long long
     }
 }
 
+// The row sketches of float rows [first, first + num) (search_kernels.cuh warp_sketch): one warp per row, four per block
+__global__ void __launch_bounds__(128) row_sketch_kernel(const unsigned char* __restrict__ vectors, unsigned long long row_stride_bytes,
+                                                         int first, int num, int dim, unsigned char* __restrict__ sketch) {
+    const int r = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (r >= num) return;
+    unsigned char* out = sketch + (size_t)(first + r) * sketch_stride(dim);
+    const RowSketchTail t = warp_sketch(reinterpret_cast<const float*>(vectors + (size_t)(first + r) * row_stride_bytes), dim,
+                                        reinterpret_cast<signed char*>(out), lane);
+    if (lane == 0) *reinterpret_cast<RowSketchTail*>(out + sketch_elems(dim)) = t;
+}
+
 // DeleteIndex(id) for a batch (Labelset::Insert, Labelset.h:59-76) in call order: an id that is out of range, already
 // tombstoned, or repeated earlier in the same batch gets VectorNotFound; the first occurrence of a live id tombstones it.
 // Three launches: first[id] = INT_MAX, first[id] = min(batch position), then the winners flip the byte and count.

@@ -21,6 +21,10 @@ typedef void (*NearestFirstKernelFn)(const SearchParams, int*, const IterVisited
 // slots: query slots per SM the host aims at (512-byte rows: register-capped variants above 16)
 template <bool BFS, bool COSINE>
 SearchKernelFn pick_float_kernel(int dim, int mres_cap, bool kdt, int slots);
+// float rows, BKT: the sketch:: kernels, which test a graph candidate's row sketch before they fetch its row
+// (SearchParams::sketch must be bound); dim 768 selects the unrolled variant
+template <bool COSINE>
+SearchKernelFn pick_sketch_kernel(int dim, int mres_cap);
 // ELEM 1 int8, 2 uint8, 3 int16
 template <bool BFS, int ELEM>
 SearchKernelFn pick_int_kernel(bool cosine, int mres_cap, bool kdt);

@@ -61,6 +61,20 @@ SearchKernelFn pick_float_kernel(int dim, int mres_cap, bool kdt, int slots) {
     return pick_rpl<BFS, 0, COSINE>(mres_cap, kdt, slots);
 }
 
+// 12 slots per SM (168 registers, no spills with the 16- and 32-register m_Results files): what lay_out runs rows of
+// 2 KB or more at.  (A 128-register form of the 768-d kernel spills 330 bytes and was 19 % slower at 13 to 16 slots.)
+template <int DIM, bool COSINE>
+static SearchKernelFn pick_sketch_rpl(int mres_cap) {
+    if (mres_cap <= 32 * 16) return sketch::search_kernel<DIM, COSINE, 16, false, false, 0, 12>;
+    if (mres_cap <= 32 * 32) return sketch::search_kernel<DIM, COSINE, 32, false, false, 0, 12>;
+    if (mres_cap <= 32 * 64) return sketch::search_kernel<DIM, COSINE, 64, false, false, 0, 8>;
+    return nullptr;
+}
+template <bool COSINE>
+SearchKernelFn pick_sketch_kernel(int dim, int mres_cap) {
+    return dim == 768 ? pick_sketch_rpl<768, COSINE>(mres_cap) : pick_sketch_rpl<0, COSINE>(mres_cap);
+}
+
 template <bool BFS, bool COSINE, int ELEM>
 static SearchKernelFn pick_int_rpl(int mres_cap, bool kdt) {
     if constexpr (!BFS) {

@@ -11,7 +11,7 @@ template <int DIM, bool COSINE, int RPL, bool KDT, bool PQ = false, int ELEM = 0
 __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) {
     extern __shared__ __align__(128) unsigned char smem[];
     const int lane = threadIdx.x;
-    WarpSearch<DIM, COSINE, RPL, PQ, ELEM, true, false, SPTAG_B200_BFS> w(p, lane);
+    WarpSearch<DIM, COSINE, RPL, PQ, ELEM, true, false, SPTAG_B200_BFS, SPTAG_B200_SKETCH> w(p, lane);
     w.visited = p.vhash ? p.vhash + (size_t)blockIdx.x * (p.vhash_mask + 1ull) : p.visited + (size_t)blockIdx.x * p.visited_words;
     w.vlog = p.vlog ? p.vlog + (size_t)blockIdx.x * p.vlog_entries : nullptr;
     w.tk = p.topk ? p.topk + (size_t)blockIdx.x * p.topk_pad : nullptr;
@@ -80,6 +80,12 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
                 for (int c = 0; c < DIM / 16; ++c) w.qr.q[c] = __ldg(qg + 16 * c + (lane & 15));
             }
         }
+        if constexpr (SPTAG_B200_SKETCH) {
+            signed char* tq = reinterpret_cast<signed char*>(smem + p.off_sketch);
+            w.tq = reinterpret_cast<const unsigned*>(tq);
+            w.tq_tail = warp_sketch(reinterpret_cast<const float*>(p.queries + (size_t)q * p.query_stride_bytes), p.dim, tq, lane);
+            w.nskipped = 0;
+        }
         __syncwarp();
 
         if (KDT)
@@ -127,6 +133,9 @@ __global__ void __launch_bounds__(32, MINB) search_kernel(const SearchParams p) 
             s[5] = w.nexpand;
             s[6] = w.ntree;
             s[7] = 0;
+        }
+        if constexpr (SPTAG_B200_SKETCH) {
+            if (lane == 0 && w.nskipped) atomicAdd(p.rows_skipped, (unsigned long long)w.nskipped);
         }
         __syncwarp();
     }

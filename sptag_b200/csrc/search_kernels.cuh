@@ -72,6 +72,7 @@ struct SearchParams {
     unsigned long long row_stride_bytes;   // bytes between rows (multiple of 16)
     int row_bytes;                         // bytes copied per row (multiple of 16)
     int n, dim;
+    int off_sketch;                        // sketch:: kernels: the query's int8 sketch in shared memory (fills the padding)
     const int* graph;
     int degree;
     // EnableBfs (BKTree::m_bfs, the bfs:: kernels only): != 0 seeds each tree breadth-first.  (Here it fills the padding
@@ -120,12 +121,20 @@ struct SearchParams {
     int off_ng, off_spt, off_cand, off_bar, off_query;
     // PQ / OPQ quantized index (PQQuantizer.h:110-128, ADC off): rows are M code bytes, the query is M code
     // bytes too and distance = sum_i sdc[(i*Ks + x_i)*Ks + y_i]
-    const float* sdc;
+    // (float rows are never PQ codes, so the row sketches of the sketch:: kernels share the PQ tables' slots: a longer
+    //  struct would move the iterator kernels' later arguments and change their code)
+    union {
+        const float* sdc;
+        const unsigned char* sketch;       // sketch:: kernels: per row round_up(dim, 16) int8 then a RowSketchTail
+    };
     int pq_m, pq_ks;
     // ADC mode (IQuantizer::SetEnableADC, PQQuantizer.h:114-119, :141-157): the query is a rotated float vector,
     // each warp builds its M*Ks distance table in its slot of `adc_tables` and sums table[i*Ks + y_i]
     int pq_adc, pq_dsub;
-    const float* codebooks;
+    union {
+        const float* codebooks;
+        unsigned long long* rows_skipped;  // sketch:: kernels: candidates whose row was not fetched, summed over queries
+    };
     float* adc_tables;                     // per slot, pq_m * pq_ks floats
     // which DistanceUtils summation tree to reproduce: 16 = AVX-512 (all specialised paths), 8 = AVX / AVX2, 4 = SSE
     // (DistanceUtils.h:118-163 picks one by cpuid; a reference host without AVX-512 rounds differently)
@@ -880,6 +889,100 @@ struct MResults {
 };
 
 // ------------------------------------------------------------------------------------------
+// Row sketches (the sketch:: kernels): a 1-byte-per-dimension copy of every float row that decides, exactly, which
+// graph candidates m_Results must reject, so that their 4-byte-per-dimension rows are never fetched.
+// A vector v is sketched as  scale = max|v_i| / 127,  s_i = clamp(rint(v_i / scale), -127, 127)  (all zero when scale
+// is 0) plus three bounds: err >= ||v - scale s||, norm >= ||v||, nsq <= ||v||^2.  A vector with a NaN or an infinity is
+// sketched as zeros with err = +inf, which no test passes.  For a query q (t, e_q) and a row x (s, e_x), I = sum t_i s_i
+// is an exact integer and, by Cauchy-Schwarz,
+//     q.x <= scale_q scale_x I + norm_q err_x + err_q norm_x + err_q err_x.
+// sketch_lower_bound turns that into a value the reference's fp32 distance cannot fall below: every step rounds to the
+// safe side, and `rel` (sketch_rel_margin) times the operands' size covers the reference's own rounding in any of its
+// three summation trees.  tools/row_sketch_model.py restates all of this in numpy, operation by operation, and
+// tests/test_row_sketch_bound.py holds that restatement against the reference's distance function.
+// ------------------------------------------------------------------------------------------
+struct RowSketchTail {
+    float scale, err, norm, nsq;
+};
+static_assert(sizeof(RowSketchTail) == 16, "a sketch row ends in 16 bytes");
+__host__ __device__ __forceinline__ int sketch_elems(int dim) { return (dim + 15) & ~15; }
+__host__ __device__ __forceinline__ size_t sketch_stride(int dim) { return (size_t)sketch_elems(dim) + sizeof(RowSketchTail); }
+// dim/4 additions per accumulator in the narrowest (SSE) tree, the folds, the tail, the product and the last subtraction,
+// 2^-24 each, doubled
+__host__ __device__ __forceinline__ float sketch_rel_margin(int dim) { return (float)(dim / 4 + 24) * 1.1920928955078125e-07f; }
+constexpr float kSketchNormLimit = 1e15f;  // beyond it the reference's own sum may overflow into a NaN: no statement
+
+// the next float above / below a non-negative finite one
+__device__ __forceinline__ float f32_above(float f) { return f < INFINITY ? __uint_as_float(__float_as_uint(f) + 1u) : f; }
+__device__ __forceinline__ float f32_below(float f) { return f > 0.0f ? __uint_as_float(__float_as_uint(f) - 1u) : 0.0f; }
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
+    return v;
+}
+
+// The sketch of v[0..dim) by one warp: the int8 elements (zero padded to sketch_elems) to `out`, the tail returned in
+// every lane.  `out` may be shared or global memory.
+__device__ __forceinline__ RowSketchTail warp_sketch(const float* __restrict__ v, int dim, signed char* out, int lane) {
+    float amax = 0.0f;
+    double n2 = 0.0;
+    bool finite = true;
+    for (int i = lane; i < dim; i += 32) {
+        const float x = v[i];
+        finite = finite && (fabsf(x) < INFINITY);
+        amax = fmaxf(amax, fabsf(x));
+        n2 += (double)x * (double)x;
+    }
+    finite = __all_sync(kFull, finite);
+    amax = finite ? __uint_as_float(__reduce_max_sync(kFull, __float_as_uint(amax))) : 0.0f;
+    n2 = finite ? warp_sum(n2) : 0.0;
+    const float scale = __fdiv_rn(amax, 127.0f);
+    double r2 = 0.0;
+    const int de = sketch_elems(dim);
+    for (int i = lane; i < de; i += 32) {
+        int s = 0;
+        if (i < dim && finite) {
+            const float x = v[i];
+            if (scale > 0.0f) s = (int)fminf(fmaxf(rintf(__fdiv_rn(x, scale)), -127.0f), 127.0f);
+            const double res = (double)x - (double)scale * (double)s;
+            r2 += res * res;
+        }
+        out[i] = (signed char)s;
+    }
+    r2 = warp_sum(r2);
+    RowSketchTail t;
+    t.scale = scale;
+    t.err = finite ? f32_above((float)sqrt(r2)) : INFINITY;
+    t.norm = f32_above((float)sqrt(n2));
+    t.nsq = f32_below(f32_below((float)n2));
+    return t;
+}
+
+// A value the reference's distance of the query (tail q) to a row (tail x) with integer product I never falls below;
+// -inf where nothing can be said
+template <bool COSINE>
+__device__ __forceinline__ float sketch_lower_bound(int I, const RowSketchTail& q, const RowSketchTail& x, float rel) {
+    const float fi = __int2float_ru(I);
+    const float ss = (I >= 0) ? __fmul_ru(q.scale, x.scale) : __fmul_rd(q.scale, x.scale);
+    float ub = __fmul_ru(ss, fi);
+    ub = __fadd_ru(ub, __fmul_ru(q.norm, x.err));
+    ub = __fadd_ru(ub, __fmul_ru(q.err, x.norm));
+    ub = __fadd_ru(ub, __fmul_ru(q.err, x.err));
+    float lb;
+    if (COSINE) {
+        const float margin = __fmul_ru(rel, __fadd_ru(1.0f, __fmul_ru(q.norm, x.norm)));
+        lb = __fsub_rd(__fsub_rd(1.0f, ub), margin);
+    } else {
+        const float nsum = __fadd_ru(q.norm, x.norm);
+        const float margin = __fadd_ru(__fmul_ru(rel, __fmul_ru(nsum, nsum)), 1e-30f);
+        lb = __fsub_rd(__fsub_rd(__fadd_rd(q.nsq, x.nsq), __fmul_ru(2.0f, ub)), margin);
+    }
+    const bool safe = __fmul_ru(q.norm, x.norm) < kSketchNormLimit && q.norm < kSketchNormLimit && x.norm < kSketchNormLimit &&
+                      x.err < INFINITY && q.err < INFINITY;
+    return (safe && lb == lb) ? lb : -INFINITY;
+}
+
+// ------------------------------------------------------------------------------------------
 // The per-query state of one warp
 // ------------------------------------------------------------------------------------------
 struct BktNodeDev {
@@ -889,7 +992,9 @@ struct BktNodeDev {
 // HASH: the hashed visited set can be bound (search_kernel).  QHASH: the visited set is chosen per query (the iterator
 // kernels): a hash table whose capacity the query carries in qmask / qshift / qlimit, or a bitmap (qmask = 0).
 // BFS: the kernel seeds BKT trees breadth-first when p.bfs != 0 (the bfs:: kernels)
-template <int DIM, bool COSINE, int RPL, bool PQ, int ELEM, bool HASH = false, bool QHASH = false, bool BFS = false>
+// SKETCH: BKT search tests a graph candidate's row sketch before it fetches the row (the sketch:: kernels)
+template <int DIM, bool COSINE, int RPL, bool PQ, int ELEM, bool HASH = false, bool QHASH = false, bool BFS = false,
+          bool SKETCH = false>
 struct WarpSearch {
     const SearchParams& p;
     const int lane, half, j;
@@ -923,6 +1028,10 @@ struct WarpSearch {
     int checked, ndist, nexpand, ntree;
     int tree_checked, no_better;  // KDT: m_iNumberOfTreeCheckedLeaves, m_iNumOfContinuousNoBetterPropagation
     unsigned phase_bits;
+    // SKETCH: the query's sketch (its elements in shared memory) and the candidates whose rows were not fetched
+    const unsigned* tq;
+    RowSketchTail tq_tail;
+    int nskipped;
 
     __device__ __forceinline__ WarpSearch(const SearchParams& p_, int lane_)
         : p(p_), lane(lane_), half(lane_ >> 4), j(lane_ & 15) {}
@@ -1562,6 +1671,9 @@ struct WarpSearch {
     // One graph-row chunk after issue_mark: its fresh ids compacted into cand_id in neighbour order (and logged), and their
     // distances in cand_dist.  Returns how many there are.  The iterator kernels bind no clear log (vlog = nullptr: their
     // sets persist across calls), so the log store compiles away there; binding one would add it to every chunk.
+    // GATED: the caller drops every candidate whose distance is above mres.worst (BKT Search), so the sketch may stand in
+    // for the row of such a candidate
+    template <bool GATED = false>
     __device__ __forceinline__ int expand_chunk(RowMark& mark, int nn) {
         const bool fresh = mark_fresh(mark, nn);
         const unsigned freshmask = __ballot_sync(kFull, fresh);
@@ -1573,8 +1685,70 @@ struct WarpSearch {
             if (vlog != nullptr && vlog_count + rank < (int)p.vlog_entries) vlog[vlog_count + rank] = mark_word(mark, nn);
         }
         vlog_count += cnt;
-        compute_dists(cnt);
+        if constexpr (GATED && SKETCH)
+            compute_dists_gated(cnt);
+        else
+            compute_dists(cnt);
         return cnt;
+    }
+
+    // compute_dists for candidates that only matter while their distance is <= mres.worst.  Pass 1 reads the candidates'
+    // sketches (lane l the 4-byte words l, l + 32, ... of a row: coalesced, 1/4 of the row's bytes) and lane r bounds
+    // candidate r's distance from below.  Pass 2 fetches the rows of the others only, compacted in neighbour order, and
+    // their distances are the reference's bits; a candidate that was proven above worst gets its bound as its distance.
+    // worst never increases, so the caller drops it wherever the true distance would have been dropped, and every
+    // counter advances as if the row had been read.  Until m_Results is full its worst is MaxDist and nothing is skipped.
+    __device__ __forceinline__ void compute_dists_gated(int cnt) {
+        if (cnt <= 0) return;
+        __syncwarp();
+        const int myid = (lane < cnt) ? cand_id[lane] : 0;
+        const float worst = mres.worst;
+        float lb = -INFINITY;
+        if (worst < SPTAG_B200_MAXDIST) {  // (warp-uniform)
+            const size_t stride = sketch_stride(p.dim);
+            const int nwords = ((DIM > 0) ? sketch_elems(DIM) : sketch_elems(p.dim)) >> 2;
+            RowSketchTail xt = {0.0f, INFINITY, 0.0f, 0.0f};
+            if (lane < cnt) xt = *reinterpret_cast<const RowSketchTail*>(p.sketch + (size_t)myid * stride + 4 * nwords);
+            int myI = 0;
+            for (int c0 = 0; c0 < cnt; c0 += 4) {
+                const unsigned* rw[4];
+                int acc[4];
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    const int id = __shfl_sync(kFull, myid, min(c0 + u, cnt - 1));
+                    rw[u] = reinterpret_cast<const unsigned*>(p.sketch + (size_t)id * stride);
+                    acc[u] = 0;
+                }
+#pragma unroll
+                for (int w = lane; w < nwords; w += 32) {
+                    const int t = (int)tq[w];
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) acc[u] = __dp4a((int)__ldg(rw[u] + w), t, acc[u]);
+                }
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    const int I = __reduce_add_sync(kFull, acc[u]);
+                    if (lane == c0 + u) myI = I;
+                }
+            }
+            if (lane < cnt) lb = sketch_lower_bound<COSINE>(myI, tq_tail, xt, sketch_rel_margin(p.dim));
+        }
+        const bool keep = (lane < cnt) && !(lb > worst);
+        const unsigned keepmask = __ballot_sync(kFull, keep);
+        const int nkeep = __popc(keepmask);
+        const int rank = __popc(keepmask & ((1u << lane) - 1u));
+        __syncwarp();
+        if (keep) cand_id[rank] = myid;
+        compute_dists(nkeep);
+        const float d = keep ? cand_dist[rank] : lb;
+        __syncwarp();
+        if (lane < cnt) {
+            cand_id[lane] = myid;
+            cand_dist[lane] = d;
+        }
+        __syncwarp();
+        ndist += cnt - nkeep;
+        nskipped += cnt - nkeep;
     }
 
     // BKT Search's accept of the popped node (BKTIndex.cpp:292-320): a node whose last graph entry `checkNode` points back
@@ -1706,7 +1880,7 @@ struct WarpSearch {
                 // the scan stops at the first negative entry (BKTIndex.cpp:333-336); a repeated id inside the row is
                 // "visited" by the time its second copy is reached
                 RowMark mark = issue_mark(nn, cbase + lane <= checkPos);
-                const int cnt = expand_chunk(mark, nn);
+                const int cnt = expand_chunk<true>(mark, nn);
                 // m_Results.worst() never increases, so a candidate above the current worst is rejected
                 // whenever its turn comes; only the others are replayed in neighbour order (BKTIndex.cpp:338-344)
                 const float myd = (lane < cnt) ? cand_dist[lane] : SPTAG_B200_MAXDIST;
@@ -2023,6 +2197,8 @@ __device__ __forceinline__ void suspend_iter_query(const IterVisited& iv, int q,
 
 // The kernels: search_kernel, iterate_kernel and nearest_first_kernel as they are, and the same text in namespace bfs with
 // breadth-first tree seeding (EnableBfs != 0), instantiated for the generic-dimension, integer and PQ rows only
+// and once more in namespace sketch with the row-sketch test in BKT search's graph step (search_kernel only is instantiated)
+#define SPTAG_B200_SKETCH false
 #define SPTAG_B200_BFS false
 #include "search_kernel_defs.cuh"
 #undef SPTAG_B200_BFS
@@ -2031,5 +2207,13 @@ namespace bfs {
 #include "search_kernel_defs.cuh"
 #undef SPTAG_B200_BFS
 }  // namespace bfs
+#undef SPTAG_B200_SKETCH
+namespace sketch {
+#define SPTAG_B200_SKETCH true
+#define SPTAG_B200_BFS false
+#include "search_kernel_defs.cuh"
+#undef SPTAG_B200_BFS
+#undef SPTAG_B200_SKETCH
+}  // namespace sketch
 
 }  // namespace sptag_b200

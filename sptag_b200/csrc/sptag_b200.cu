@@ -174,6 +174,13 @@ struct sptag_b200_index {
     // -1 auto (the bitmap unless its per-slot allocation fails), 0 bitmap, 1 hashed set per slot
     int visited_set = -1;
     int visited_hash_entries = 0;  // table entries per slot, 0 = 2^(bits(max(MaxCheck, MaxCheckForRefineGraph)) + 2)
+    // B200.RowSketch: -1 auto (float BKT rows of 2 KB or more, unless the sketches do not fit in HBM), 0 off, 1 on.
+    // d_sketch holds the sketches of rows [0, sketch_n) (search_kernels.cuh warp_sketch); it is a function of the rows, so
+    // it is rebuilt, never saved.  d_skipped: the candidates whose rows the searches of this handle did not fetch.
+    int row_sketch = -1;
+    DeviceBuffer d_sketch, d_skipped;
+    int sketch_n = 0;
+    bool sketch_unfit = false;  // auto: the allocation failed for lack of memory; cleared by setting B200.RowSketch
     std::atomic<int> last_visited_overflows{0};  // queries the hashed set handed to the re-run, last blocking search
     // iterators: -1 auto (the bitmaps unless their allocation fails), 0 bitmap, 1 a growing hash table per query
     int iter_visited_set = -1;
@@ -283,7 +290,11 @@ SearchKernelFn pick_kernel_seeded(const sptag_b200_index* h, int mres_cap, int s
 
 // The kernel instantiation for this index / parameter set (nullptr: unsupported m_Results capacity); the
 // instantiations live in kern_*.cu (kernel_select.h)
-SearchKernelFn pick_kernel(const sptag_b200_index* h, int mres_cap, int slots = 0) {
+SearchKernelFn pick_kernel(const sptag_b200_index* h, int mres_cap, int slots = 0, bool sketch = false) {
+    if (sketch) {
+        const int kdim = (h->simd_width == 16) ? h->dim : 0;
+        return h->metric != SPTAG_B200_METRIC_L2 ? pick_sketch_kernel<true>(kdim, mres_cap) : pick_sketch_kernel<false>(kdim, mres_cap);
+    }
     return bfs_seeding(h) ? pick_kernel_seeded<true>(h, mres_cap, slots) : pick_kernel_seeded<false>(h, mres_cap, slots);
 }
 
@@ -308,6 +319,7 @@ struct CallOpts {
     // of its searches (an all-zero map rejects nothing, so this equals the reference's Count() == 0 dispatch)
     bool tombstones_live = false;
     int* d_overflows = nullptr;  // device int: receives how many queries the hashed set handed to the re-run (bitmap: 0)
+    bool sketch = false;         // the handle's row sketches cover every row: take the sketch:: kernel (search_device_impl)
 };
 
 // Slots of a result heap kept in HBM for k results: a power of two (the final sort is bitonic), at least 64
@@ -415,6 +427,10 @@ void fill_params(const sptag_b200_index* h, int k, const CallOpts& opts, SearchP
     p.pq_adc = (pq && h->q_adc) ? 1 : 0;
     p.pq_dsub = h->q_dsub;
     p.codebooks = (const float*)h->d_codebooks.ptr;
+    if (opts.sketch) {  // float rows: the PQ tables' slots are free (SearchParams)
+        p.sketch = (const unsigned char*)h->d_sketch.ptr;
+        p.rows_skipped = (unsigned long long*)h->d_skipped.ptr;
+    }
 
     // ---- per-slot arena sizes ----
     p.visited_words = round_up(((size_t)h->n + 1 + 31) / 32, 4);
@@ -462,7 +478,8 @@ int lay_out(const sptag_b200_index* h, int nq, SearchLaunch& L) {
     }
     // 512-byte float rows run the fixed-shape fast path (search_kernels.cuh kFast): 2 stages x 8 rows, slots 576 B apart;
     // must mirror WarpSearch::kFast (BFS seeding runs the generic-dimension kernels)
-    const bool fast128 = !p.bfs && !pq && h->value_type == SPTAG_B200_VT_FLOAT && h->dim == 128 && h->simd_width == 16;
+    const bool sketch = !pq && p.sketch != nullptr;  // the sketch:: kernels have no 128- or 768-d row path of their own
+    const bool fast128 = !sketch && !p.bfs && !pq && h->value_type == SPTAG_B200_VT_FLOAT && h->dim == 128 && h->simd_width == 16;
     // ... with register-capped kernel variants for more than 16 query slots per SM (B200.QueriesPerSM); those run a
     // one-stage ring (B200.Stages = 1 selects it at any residency) so that the slot's shared memory still fits
     // Default residency for 512-byte rows: all warps start together and a query costs about the same for every warp,
@@ -519,11 +536,15 @@ int lay_out(const sptag_b200_index* h, int nq, SearchLaunch& L) {
         const bool query_in_regs_only = !p.bfs && !pq && h->value_type == SPTAG_B200_VT_FLOAT && h->algo == SPTAG_B200_ALGO_BKT &&
                                         h->dim == 768 && h->simd_width == 16;  // must mirror kRegsOnly in search_kernel
         off += query_in_regs_only ? 16 : round_up((size_t)h->dim * 4 + 16, 16);  // float query, or M row offsets for PQ
+        if (sketch) {  // the query's sketch elements
+            p.off_sketch = (int)off;
+            off += sketch_elems(h->dim);
+        }
         L.smem = round_up(off, 128);
         if (L.smem > h->smem_optin)
             return fail(SPTAG_B200_MEMORY_OVERFLOW, "shared memory per query slot %zu exceeds %zu", L.smem, h->smem_optin);
 
-        L.kern = pick_kernel(h, p.mres_cap, want_slots);
+        L.kern = pick_kernel(h, p.mres_cap, want_slots, sketch);
         if (!L.kern)
             return fail(SPTAG_B200_LACK_OF_INPUTS, "max(MaxCheck/16, K) = %d exceeds what this index type supports (2048; quantized: 1024)", p.mres_cap);
         CUDA_OK(cudaFuncSetAttribute((const void*)L.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
@@ -676,13 +697,51 @@ int pick_scratch(sptag_b200_index* h, cudaStream_t stream) {
     return 0;  // both busy elsewhere: queue behind set 0
 }
 
+// B200.RowSketch applies to this handle: float rows searched by the BKT kernels without breadth-first seeding
+bool sketch_applies(const sptag_b200_index* h) {
+    return h->value_type == SPTAG_B200_VT_FLOAT && h->q_type == 0 && h->algo == SPTAG_B200_ALGO_BKT && !bfs_seeding(h);
+}
+// Whether this handle's searches take the sketch:: kernels, with the sketches of the rows that have none yet (a new
+// handle's, or the rows sptag_b200_add appended) built first.  Blocks until they are built: a search on another stream
+// may follow.  Auto turns itself off when the array does not fit.  Caller holds h->mu.
+int ensure_sketch(sptag_b200_index* h, cudaStream_t stream, bool& on) {
+    on = false;
+    if (!sketch_applies(h) || h->row_sketch == 0 || (h->row_sketch < 0 && (h->row_stride < 2048 || h->sketch_unfit))) return 0;
+    const size_t stride = sketch_stride(h->dim), need = ((size_t)h->n + 1) * stride;
+    if (need > h->d_sketch.bytes) {
+        h->sketch_n = 0;
+        if (int rc = h->d_sketch.ensure(std::max(need, h->d_sketch.bytes + h->d_sketch.bytes / 2))) {
+            if (h->row_sketch > 0 || cudaGetLastError() != cudaErrorMemoryAllocation) return rc;
+            h->sketch_unfit = true;
+            return 0;
+        }
+    }
+    if (!h->d_skipped.ptr) {
+        if (int rc = h->d_skipped.ensure(8)) return rc;
+        CUDA_OK(cudaMemset(h->d_skipped.ptr, 0, 8));
+    }
+    h->sketch_n = std::min(h->sketch_n, h->n);
+    if (h->sketch_n < h->n) {
+        const int num = h->n - h->sketch_n;
+        row_sketch_kernel<<<(unsigned)((num + 3) / 4), 128, 0, stream>>>((const unsigned char*)h->d_vectors.ptr, h->row_stride,
+                                                                        h->sketch_n, num, h->dim, (unsigned char*)h->d_sketch.ptr);
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+        CUDA_OK(cudaStreamSynchronize(stream));
+        h->sketch_n = h->n;
+    }
+    on = true;
+    return 0;
+}
+
 // refine = true: the RefineSearchIndex flavour (BKTIndex.cpp:698-711) -- queries are base rows of the index itself
 // (stride = the padded row stride), duplicate groups are not expanded, ids come back local (no shard offset); the
 // caller passes MaxCheckForRefineGraph as opts.max_check.  Caller holds h->mu.
 int search_device_impl(sptag_b200_index* h, const void* d_queries, int nq, int k, int* d_ids, float* d_dists,
-                       int* d_stats, cudaStream_t stream, bool refine = false, const CallOpts& opts = CallOpts()) {
+                       int* d_stats, cudaStream_t stream, bool refine = false, CallOpts opts = CallOpts()) {
     if (nq <= 0) return SPTAG_B200_SUCCESS;
     int set = refine ? 0 : pick_scratch(h, stream);
+    if (int rc = ensure_sketch(h, stream, opts.sketch)) return rc;
     SearchLaunch L;
     if (int rc = plan_search(h, k, nq, opts, L)) return rc;
     if (int rc = bind_scratch(h, L, set)) {
@@ -1536,6 +1595,17 @@ int sptag_b200_set_param(sptag_b200_handle h, const char* name, const char* valu
         h->iter_hash_entries = (int)v;
     }
     else if (n == "B200.SlotScheme") h->slot_scheme = (int)v;
+    else if (n == "B200.RowSketch") {
+        if (v < -1 || v > 1) return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.RowSketch %ld: -1 (auto), 0 (off) or 1 (on)", v);
+        if (v == 1 && !(h->value_type == SPTAG_B200_VT_FLOAT && h->q_type == 0 && h->algo == SPTAG_B200_ALGO_BKT))
+            return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.RowSketch 1: row sketches exist for float BKT indexes only");
+        h->row_sketch = (int)v;
+        h->sketch_unfit = false;  // auto tries the allocation again
+        if (v == 0) {
+            h->d_sketch.release();
+            h->sketch_n = 0;
+        }
+    }
     else if (n == "EnableADC") h->q_adc = (v != 0);  // VectorIndex::SetQuantizerADC (VectorIndex.h:136-138)
     else return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
     return SPTAG_B200_SUCCESS;
@@ -1580,6 +1650,16 @@ int sptag_b200_get_param(sptag_b200_handle h, const char* name, char* value_out,
     else if (n == "B200.LastIteratorGrowths") v = h->last_iter_growths;                // read-only
     else if (n == "B200.LastIteratorVisitedBytes") v = h->last_iter_visited_bytes;     // read-only
     else if (n == "B200.SlotScheme") v = h->slot_scheme;
+    else if (n == "B200.RowSketch") v = h->row_sketch;
+    else if (n == "B200.RowsSkipped") {  // read-only: since the handle was made, over the searches that have finished
+        unsigned long long c = 0;
+        if (h->d_skipped.ptr) {
+            DeviceGuard guard(h->device);
+            CUDA_OK(cudaDeviceSynchronize());
+            CUDA_OK(cudaMemcpy(&c, h->d_skipped.ptr, 8, cudaMemcpyDeviceToHost));
+        }
+        v = (long)c;
+    }
     else if (n == "EnableADC") v = h->q_adc;
     else if (n == "B200.LastRefineSearchUs") v = (long)(h->refine_search_ms * 1000.0);    // read-only: device time
     else if (n == "B200.LastRefineRebuildUs") v = (long)(h->refine_rebuild_ms * 1000.0);  // of the last refine pass
