@@ -173,21 +173,11 @@ __global__ void __launch_bounds__(32) multi_scan_drain_kernel(const MultiScanDra
     }
 }
 
-template <typename F>
-auto with_distance_kernel(bool cosine, int elem, F&& f) {
-    switch (elem) {
-    case 1: return cosine ? f(multi_scan_distance_kernel<true, 1>) : f(multi_scan_distance_kernel<false, 1>);
-    case 2: return cosine ? f(multi_scan_distance_kernel<true, 2>) : f(multi_scan_distance_kernel<false, 2>);
-    case 3: return cosine ? f(multi_scan_distance_kernel<true, 3>) : f(multi_scan_distance_kernel<false, 3>);
-    default: return cosine ? f(multi_scan_distance_kernel<true, 0>) : f(multi_scan_distance_kernel<false, 0>);
-    }
-}
-
 }  // namespace
 
 cudaError_t launch_multi_scan_distance(const MultiScanDistParams& p, bool cosine, int elem, int grid, cudaStream_t stream) {
-    return with_distance_kernel(cosine, elem, [&](void (*k)(const MultiScanDistParams)) {
-        k<<<grid, 32, 0, stream>>>(p);
+    return with_cosine_elem(cosine, elem, [&](auto cos, auto el) {
+        multi_scan_distance_kernel<cos, el><<<grid, 32, 0, stream>>>(p);
         return cudaGetLastError();
     });
 }

@@ -163,34 +163,20 @@ __global__ void __launch_bounds__(32) spann_scan_kernel(const SpannScanParams p)
     }
 }
 
-template <typename F>
-auto with_kernel(bool cosine, int elem, F&& f) {
-    switch (elem) {
-    case 1: return cosine ? f(spann_scan_kernel<true, 1>) : f(spann_scan_kernel<false, 1>);
-    case 2: return cosine ? f(spann_scan_kernel<true, 2>) : f(spann_scan_kernel<false, 2>);
-    case 3: return cosine ? f(spann_scan_kernel<true, 3>) : f(spann_scan_kernel<false, 3>);
-    default: return cosine ? f(spann_scan_kernel<true, 0>) : f(spann_scan_kernel<false, 0>);
-    }
-}
-
 }  // namespace
 
 size_t spann_scan_smem(int w) { return (size_t)w * 12 + 3 * 32 * 4 + 16; }
 
 int spann_scan_blocks_per_sm(bool cosine, int elem, int w) {
-    const size_t smem = spann_scan_smem(w);
-    return with_kernel(cosine, elem, [&](void (*k)(const SpannScanParams)) {
-        int fit = 0;
-        if (smem > 48 * 1024 && cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-            return 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, (const void*)k, 32, smem) != cudaSuccess) return 0;
-        return fit;
+    return with_cosine_elem(cosine, elem, [&](auto cos, auto el) {
+        return warp_blocks_per_sm((const void*)spann_scan_kernel<cos, el>, spann_scan_smem(w));
     });
 }
 
 cudaError_t launch_spann_scan(const SpannScanParams& p, bool cosine, int elem, int grid, cudaStream_t stream) {
     const size_t smem = spann_scan_smem(p.w);
-    return with_kernel(cosine, elem, [&](void (*k)(const SpannScanParams)) {
+    return with_cosine_elem(cosine, elem, [&](auto cos, auto el) {
+        void (*k)(const SpannScanParams) = spann_scan_kernel<cos, el>;
         if (smem > 48 * 1024) {
             cudaError_t e = cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (e != cudaSuccess) return e;

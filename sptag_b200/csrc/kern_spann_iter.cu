@@ -217,31 +217,18 @@ __global__ void __launch_bounds__(32) spann_iter_step_kernel(const SpannIterPara
     }
 }
 
-template <typename F>
-auto with_iter_kernel(bool cosine, int elem, F&& f) {
-    switch (elem) {
-    case 1: return cosine ? f(spann_iter_step_kernel<true, 1>) : f(spann_iter_step_kernel<false, 1>);
-    case 2: return cosine ? f(spann_iter_step_kernel<true, 2>) : f(spann_iter_step_kernel<false, 2>);
-    case 3: return cosine ? f(spann_iter_step_kernel<true, 3>) : f(spann_iter_step_kernel<false, 3>);
-    default: return cosine ? f(spann_iter_step_kernel<true, 0>) : f(spann_iter_step_kernel<false, 0>);
-    }
-}
-
 size_t spann_iter_step_smem(int cap) { return (size_t)cap * 8 + 3 * 32 * 4 + 16; }
 
 }  // namespace
 int spann_iter_step_blocks_per_sm(bool cosine, int elem, int cap) {
-    return with_iter_kernel(cosine, elem, [&](void (*k)(const SpannIterParams)) {
-        int fit = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, (const void*)k, 32, spann_iter_step_smem(cap)) != cudaSuccess)
-            return 0;
-        return fit;
+    return with_cosine_elem(cosine, elem, [&](auto cos, auto el) {
+        return warp_blocks_per_sm((const void*)spann_iter_step_kernel<cos, el>, spann_iter_step_smem(cap));
     });
 }
 
 cudaError_t launch_spann_iter_step(const SpannIterParams& p, bool cosine, int elem, int grid, cudaStream_t stream) {
-    return with_iter_kernel(cosine, elem, [&](void (*k)(const SpannIterParams)) {
-        k<<<grid, 32, spann_iter_step_smem(p.cap), stream>>>(p);
+    return with_cosine_elem(cosine, elem, [&](auto cos, auto el) {
+        spann_iter_step_kernel<cos, el><<<grid, 32, spann_iter_step_smem(p.cap), stream>>>(p);
         return cudaGetLastError();
     });
 }

@@ -1,10 +1,38 @@
-// spann_device.cuh -- device pieces shared by the SPANN posting scan (kern_spann.cu) and the posting step of SPANN
-// iterators (kern_spann_iter.cu): QueryResultSet's comparator and Heapify, the distance, LoadingHeadInfo's truncation.
+// spann_device.cuh -- pieces shared by the posting-side kernels: the SPANN posting scan (kern_spann.cu), the posting
+// step of SPANN iterators (kern_spann_iter.cu) and the multi-index scan's cross distances (kern_multi_scan.cu).
+// QueryResultSet's comparator and Heapify, the distance, LoadingHeadInfo's truncation, and the launchers' dispatch.
 #pragma once
 #include "search_kernels.cuh"
 
+#include <type_traits>
+
 namespace sptag_b200 {
 namespace {
+
+// Calls f(cos, el) with the runtime metric flag and element code (0 float, 1 int8, 2 uint8, 3 int16) as compile-time
+// constants (std::bool_constant, std::integral_constant<int, ELEM>), so that f can name its kernel's <COSINE, ELEM>
+// instantiation
+template <typename F>
+auto with_cosine_elem(bool cosine, int elem, F&& f) {
+    using T = std::true_type;
+    using N = std::false_type;
+    switch (elem) {
+    case 1: return cosine ? f(T(), std::integral_constant<int, 1>()) : f(N(), std::integral_constant<int, 1>());
+    case 2: return cosine ? f(T(), std::integral_constant<int, 2>()) : f(N(), std::integral_constant<int, 2>());
+    case 3: return cosine ? f(T(), std::integral_constant<int, 3>()) : f(N(), std::integral_constant<int, 3>());
+    default: return cosine ? f(T(), std::integral_constant<int, 0>()) : f(N(), std::integral_constant<int, 0>());
+    }
+}
+
+// Blocks of one warp of kernel k with smem bytes of dynamic shared memory that fit on one SM (0: none, or the query
+// failed)
+inline int warp_blocks_per_sm(const void* k, size_t smem) {
+    int fit = 0;
+    if (smem > 48 * 1024 && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+        return 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, k, 32, smem) != cudaSuccess) return 0;
+    return fit;
+}
 
 // BasicResult operator< (QueryResultSet.h:17-20)
 __device__ __forceinline__ bool res_less(float da, int va, float db, int vb) {

@@ -140,6 +140,107 @@ struct StagingPool {
     }
 };
 
+// One set per query in the hashed visited-set format (vhash_home), grown while its owner runs: the visited sets of
+// iterators on hash tables, the SPANN iterators' dedupers and the multi-index scan's seen sets.  The kernels find query
+// q's set at d_tables[q] and its size and fill in vbits / vfill of q's IterState in the owner's array.  A set is a table
+// of 2^bits[q] entries, or (bits 0) a bitmap of bitmap_words words once a table would be larger.  The sets live in bufs:
+// one buffer at open, one per growth round; a buffer is freed when no query's set lives in it any more.
+struct QueryTables {
+    static constexpr size_t kNoBitmap = 0;  // bitmap_words of sets that stay tables however large they grow
+    size_t bitmap_words = kNoBitmap;
+    IterState* state = nullptr;  // the owner's per-query IterState array (device)
+    std::vector<int> bits, buf;  // per query: log2 of its table's entries (0: a bitmap), the index of its buffer
+    std::vector<unsigned int*> set;
+    std::vector<DeviceBuffer> bufs;
+    std::vector<int> refs;  // per buffer: the queries whose sets live in it
+    DeviceBuffer d_tables, d_jobs;
+
+    // nq empty tables of 2^bits0 entries, and st0 with vbits = bits0 written to each of the nq IterStates at st.  Blocks
+    // until done.
+    int open(size_t nq, int bits0, size_t bitmap_words_, IterState* st, IterState st0 = IterState()) {
+        const size_t entries = (size_t)1 << bits0;
+        bitmap_words = bitmap_words_;
+        state = st;
+        bufs.emplace_back();
+        refs.push_back((int)nq);
+        if (int rc = bufs[0].ensure(nq * entries * 4)) return rc;
+        if (int rc = d_tables.ensure(nq * sizeof(unsigned int*))) return rc;
+        bits.assign(nq, bits0);
+        buf.assign(nq, 0);
+        set.resize(nq);
+        for (size_t q = 0; q < nq; ++q) set[q] = (unsigned int*)bufs[0].ptr + q * entries;
+        st0.vbits = bits0;
+        const std::vector<IterState> sts(nq, st0);
+        CUDA_OK(cudaMemset(bufs[0].ptr, 0, bufs[0].bytes));
+        CUDA_OK(cudaMemcpy(d_tables.ptr, set.data(), nq * sizeof(unsigned int*), cudaMemcpyHostToDevice));
+        CUDA_OK(cudaMemcpy(state, sts.data(), nq * sizeof(IterState), cudaMemcpyHostToDevice));
+        return 0;
+    }
+
+    // Move the sets of queries qs[i] to one new, zeroed buffer: tables of 2^new_bits[i] entries, or bitmaps where such a
+    // table would be larger than one.  keep: the ids are carried over; otherwise the sets start empty (the query's call
+    // runs again from the start).  Blocks until the move is done.
+    int grow(const std::vector<unsigned>& qs, const std::vector<int>& new_bits, bool keep, cudaStream_t stream) {
+        std::vector<IterGrowJob> jobs(qs.size());
+        size_t words = 0;
+        for (size_t i = 0; i < qs.size(); ++i) {
+            int b = new_bits[i];
+            if (b && bitmap_words != kNoBitmap && ((size_t)1 << b) > bitmap_words) b = 0;  // a bitmap, and stays one
+            jobs[i].new_bits = b;
+            jobs[i].new_set = (unsigned int*)(words * 4);  // offset until the buffer exists
+            words += b ? ((size_t)1 << b) : bitmap_words;
+        }
+        DeviceBuffer nbuf;
+        if (int rc = nbuf.ensure(words * 4)) return rc;
+        CUDA_OK(cudaMemsetAsync(nbuf.ptr, 0, nbuf.bytes, stream));
+        for (size_t i = 0; i < qs.size(); ++i) {
+            const unsigned q = qs[i];
+            jobs[i].new_set = (unsigned int*)((char*)nbuf.ptr + (size_t)jobs[i].new_set);
+            jobs[i].old_set = set[q];
+            jobs[i].q = (int)q;
+            jobs[i].old_bits = bits[q];
+            jobs[i].keep = keep ? 1 : 0;
+        }
+        if (int rc = d_jobs.ensure(jobs.size() * sizeof(IterGrowJob))) return rc;
+        CUDA_OK(cudaMemcpyAsync(d_jobs.ptr, jobs.data(), jobs.size() * sizeof(IterGrowJob), cudaMemcpyHostToDevice, stream));
+        iter_grow_kernel<<<(unsigned)jobs.size(), 32, 0, stream>>>((const IterGrowJob*)d_jobs.ptr, (unsigned int**)d_tables.ptr,
+                                                                   (int*)state);
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+        CUDA_OK(cudaStreamSynchronize(stream));
+        const int nb = (int)bufs.size();
+        for (size_t i = 0; i < qs.size(); ++i) {
+            const unsigned q = qs[i];
+            if (--refs[buf[q]] == 0) bufs[buf[q]].release();
+            buf[q] = nb;
+            bits[q] = jobs[i].new_bits;
+            set[q] = jobs[i].new_set;
+        }
+        bufs.push_back(std::move(nbuf));
+        refs.push_back((int)qs.size());
+        return 0;
+    }
+
+    // Read the header of the device list d_list (kIterListHeader layout) into hdr, and double the sets of the hdr[0]
+    // queries it lists.  Blocks.
+    int double_listed(const unsigned int* d_list, unsigned* hdr, bool keep, cudaStream_t stream) {
+        CUDA_OK(cudaMemcpyAsync(hdr, d_list, kIterListHeader * 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        if (hdr[0] == 0) return 0;
+        std::vector<unsigned> qs(hdr[0]);
+        CUDA_OK(cudaMemcpy(qs.data(), d_list + kIterListHeader, qs.size() * 4, cudaMemcpyDeviceToHost));
+        std::vector<int> nb(qs.size());
+        for (size_t i = 0; i < qs.size(); ++i) nb[i] = bits[qs[i]] + 1;
+        return grow(qs, nb, keep, stream);
+    }
+
+    size_t bytes() const {
+        size_t b = 0;
+        for (const DeviceBuffer& v : bufs) b += v.bytes;
+        return b;
+    }
+};
+
 }  // namespace
 
 struct sptag_b200_index {
@@ -248,21 +349,13 @@ struct sptag_b200_iterator {
     int nearest_k = 0;       // > 0 once sptag_b200_iterator_next_from_nearest ran: the head QueryResult's size
     bool stepped = false;    // a Next of either kind has run
     DeviceBuffer d_queries, d_visited, d_ng, d_spt, d_state, d_topk, d_ids, d_dists, d_counts, d_relaxed;
-    // Hashed visited sets (B200.IteratorVisitedSet): each query's set is a table of 2^bits entries, or a bitmap (bits 0)
-    // once a table would outgrow one.  The sets live in vbufs: one buffer at open, one per growth round; a buffer is
-    // freed when no query's set lives in it any more.
+    // Hashed visited sets (B200.IteratorVisitedSet): tables that grow, each turning into a bitmap of visited_words words
+    // once it would outgrow one
     bool hashed = false;
     int margin = 0;  // degree + largest duplicate group + 1 (IterVisited::margin)
-    std::vector<int> q_bits, q_buf;
-    std::vector<unsigned int*> q_set;
-    std::vector<DeviceBuffer> vbufs;
-    std::vector<int> vbuf_refs;
-    DeviceBuffer d_tables, d_resume, d_susp[2], d_jobs;
-    size_t visited_bytes() const {
-        size_t b = d_visited.bytes;
-        for (const DeviceBuffer& v : vbufs) b += v.bytes;
-        return b;
-    }
+    QueryTables tables;
+    DeviceBuffer d_resume, d_susp[2];
+    size_t visited_bytes() const { return d_visited.bytes + tables.bytes(); }
 };
 
 namespace {
@@ -825,51 +918,6 @@ int plan_iterator_step(const sptag_b200_iterator* it, int k, SearchLaunch& L) {
     return plan_search(it->h, k, it->nq, iopts, L);
 }
 
-// Move the visited sets of queries qs[i] to one new, zeroed buffer: tables of 2^bits[i] entries, or bitmaps where such a
-// table would be larger than the query's bitmap.  keep: the ids are carried over; otherwise the sets start empty (the
-// query's call runs again from the start).  Blocks until the move is done.  Caller holds h->mu.
-int grow_iter_visited(sptag_b200_iterator* it, const std::vector<unsigned>& qs, const std::vector<int>& bits, bool keep,
-                      cudaStream_t stream) {
-    std::vector<IterGrowJob> jobs(qs.size());
-    size_t words = 0;
-    for (size_t i = 0; i < qs.size(); ++i) {
-        int b = bits[i];
-        if (b && ((size_t)1 << b) > it->visited_words) b = 0;  // converts to a bitmap and stays one
-        jobs[i].new_bits = b;
-        jobs[i].new_set = (unsigned int*)(words * 4);  // offset until the buffer exists
-        words += b ? ((size_t)1 << b) : it->visited_words;
-    }
-    DeviceBuffer buf;
-    if (int rc = buf.ensure(words * 4)) return rc;
-    CUDA_OK(cudaMemsetAsync(buf.ptr, 0, buf.bytes, stream));
-    for (size_t i = 0; i < qs.size(); ++i) {
-        const unsigned q = qs[i];
-        jobs[i].new_set = (unsigned int*)((char*)buf.ptr + (size_t)jobs[i].new_set);
-        jobs[i].old_set = it->q_set[q];
-        jobs[i].q = (int)q;
-        jobs[i].old_bits = it->q_bits[q];
-        jobs[i].keep = keep ? 1 : 0;
-    }
-    if (int rc = it->d_jobs.ensure(jobs.size() * sizeof(IterGrowJob))) return rc;
-    CUDA_OK(cudaMemcpyAsync(it->d_jobs.ptr, jobs.data(), jobs.size() * sizeof(IterGrowJob), cudaMemcpyHostToDevice, stream));
-    iter_grow_kernel<<<(unsigned)jobs.size(), 32, 0, stream>>>((const IterGrowJob*)it->d_jobs.ptr,
-                                                               (unsigned int**)it->d_tables.ptr, (int*)it->d_state.ptr);
-    g_launches++;
-    CUDA_OK(cudaGetLastError());
-    CUDA_OK(cudaStreamSynchronize(stream));
-    const int nb = (int)it->vbufs.size();
-    for (size_t i = 0; i < qs.size(); ++i) {
-        const unsigned q = qs[i];
-        if (--it->vbuf_refs[it->q_buf[q]] == 0) it->vbufs[it->q_buf[q]].release();
-        it->q_buf[q] = nb;
-        it->q_bits[q] = jobs[i].new_bits;
-        it->q_set[q] = jobs[i].new_set;
-    }
-    it->vbufs.push_back(std::move(buf));
-    it->vbuf_refs.push_back((int)qs.size());
-    return 0;
-}
-
 // Before an iterator's first call, whose seeding cannot suspend: every hashed table of fewer than 2^need entries is
 // replaced by an empty one of 2^need (the tables are still empty: nothing has run), or by a bitmap where such a table
 // would be larger.  Caller holds h->mu.
@@ -877,11 +925,11 @@ int fit_iter_tables(sptag_b200_iterator* it, int need) {
     std::vector<unsigned> qs;
     std::vector<int> bits;
     for (int q = 0; q < it->nq; ++q)
-        if (it->q_bits[q] != 0 && it->q_bits[q] < need) {
+        if (it->tables.bits[q] != 0 && it->tables.bits[q] < need) {
             qs.push_back((unsigned)q);
             bits.push_back(need);
         }
-    return qs.empty() ? 0 : grow_iter_visited(it, qs, bits, false, nullptr);
+    return qs.empty() ? 0 : it->tables.grow(qs, bits, false, nullptr);
 }
 
 // The first Next of an iterator on hash tables with EnableBfs = bfs > 0: the breadth-first seeding inserts at most
@@ -948,7 +996,7 @@ int run_iterator_step(sptag_b200_iterator* it, int k, const char* what, SearchLa
     iv.margin = it->margin;
     iv.list = d_list;
     if (it->hashed) {
-        iv.tables = (unsigned int* const*)it->d_tables.ptr;
+        iv.tables = (unsigned int* const*)it->tables.d_tables.ptr;
         iv.resume = (float*)it->d_resume.ptr;
         iv.suspended = (unsigned int*)it->d_susp[0].ptr;
     }
@@ -962,22 +1010,16 @@ int run_iterator_step(sptag_b200_iterator* it, int k, const char* what, SearchLa
     long susp_step = 0, susp_trees = 0, growths = 0;
     for (int cur = 0; it->hashed; cur ^= 1) {  // at most ~log2(n) rounds: every round doubles the listed tables
         unsigned hdr[kIterListHeader];
-        CUDA_OK(cudaMemcpyAsync(hdr, it->d_susp[cur].ptr, sizeof(hdr), cudaMemcpyDeviceToHost, stream));
-        CUDA_OK(cudaStreamSynchronize(stream));
+        if (int rc = it->tables.double_listed((const unsigned int*)it->d_susp[cur].ptr, hdr, !restart, stream)) return rc;
         susp_step += hdr[1];
         susp_trees += hdr[2];
         if (hdr[0] == 0) break;
-        std::vector<unsigned> qs(hdr[0]);
-        CUDA_OK(cudaMemcpy(qs.data(), (unsigned*)it->d_susp[cur].ptr + kIterListHeader, qs.size() * 4, cudaMemcpyDeviceToHost));
-        std::vector<int> bits(qs.size());
-        for (size_t i = 0; i < qs.size(); ++i) bits[i] = it->q_bits[qs[i]] + 1;
-        if (int rc = grow_iter_visited(it, qs, bits, !restart, stream)) return rc;
-        growths += (long)qs.size();
+        growths += (long)hdr[0];
         iv.list = (const unsigned int*)it->d_susp[cur].ptr;
         iv.suspended = (unsigned int*)it->d_susp[cur ^ 1].ptr;
         CUDA_OK(cudaMemsetAsync(p.work_counter, 0, 4, stream));
         CUDA_OK(cudaMemsetAsync(iv.suspended, 0, kIterListHeader * 4, stream));
-        if (int rc = launch(p, std::min(L.grid, (int)qs.size()), smem, stream, iv)) return rc;
+        if (int rc = launch(p, std::min(L.grid, (int)hdr[0]), smem, stream, iv)) return rc;
         g_launches++;
         CUDA_OK(cudaGetLastError());
     }
@@ -1026,6 +1068,26 @@ void with_metric_elem(const sptag_b200_index* h, F&& f) {
         else
             f(std::true_type(), el);
     });
+}
+
+// The handle's metric flag (true for every metric but L2) and element code, as the posting kernels' launchers take them
+struct MetricElem {
+    bool cosine;
+    int elem;
+};
+MetricElem metric_elem(const sptag_b200_index* h) {
+    MetricElem m = {h->metric != SPTAG_B200_METRIC_L2, 0};
+    with_elem(h, [&](auto el) { m.elem = el; });
+    return m;
+}
+
+// Writes nq queries (host or device memory) to dst as rows of the handle's row stride, zero padded, as the posting and
+// cross-distance kernels read them
+int upload_query_rows(const sptag_b200_index* h, void* dst, const void* queries, size_t nq, cudaStream_t stream) {
+    const size_t qrow = (size_t)h->dim * value_size(h->value_type);
+    CUDA_OK(cudaMemsetAsync(dst, 0, nq * h->row_stride, stream));
+    CUDA_OK(cudaMemcpy2DAsync(dst, h->row_stride, queries, qrow, qrow, nq, cudaMemcpyDefault, stream));
+    return 0;
 }
 
 // Make d_graph_new, rows of `degree` entries, the index's graph.  BuildGraph re-attaches the duplicate-group
@@ -1995,7 +2057,9 @@ int sptag_b200_iterator_open_ex(sptag_b200_handle h, const void* queries, int32_
         }
         it->hashed = true;  // auto: the bitmaps do not fit (the failed cudaMalloc's error is cleared above)
     }
-    int bits = 0;
+    IterState st0 = {};
+    st0.first = 1;   // first call: InitSearchTrees + SearchTrees
+    st0.slots = -1;  // no QueryResult yet: the first Next sets the slot count
     if (it->hashed) {
         if (h->max_dup < 0) {  // computed once per handle: the tree does not change
             int* d_max = (int*)h->scratch[0].d_counter.ptr + 16;
@@ -2013,35 +2077,22 @@ int sptag_b200_iterator_open_ex(sptag_b200_handle h, const void* queries, int32_
         it->margin = h->degree + h->max_dup + 1;
         // initial entries: B200.IteratorVisitedHashEntries, or the reference's first-block size as for search; raised
         // until one step fits below the limit, so that doubling a table always makes room for the step that suspended
-        bits = vhash_log2_entries(h->iter_hash_entries, std::max(h->max_check, h->max_check_refine));
+        int bits = vhash_log2_entries(h->iter_hash_entries, std::max(h->max_check, h->max_check_refine));
         while (bits < 30 && (1 << (bits - 1)) < it->margin) ++bits;
-        const size_t entries = (size_t)1 << bits;
-        it->vbufs.emplace_back();
-        it->vbuf_refs.push_back(num_queries);
-        if ((rc = it->vbufs[0].ensure((size_t)num_queries * entries * 4)) ||
-            (rc = it->d_tables.ensure((size_t)num_queries * sizeof(unsigned int*))) ||
-            (rc = it->d_resume.ensure((size_t)num_queries * kIterResumeWords * 4)) ||
+        if ((rc = it->d_resume.ensure((size_t)num_queries * kIterResumeWords * 4)) ||
             (rc = it->d_susp[0].ensure((size_t)(kIterListHeader + num_queries) * 4)) ||
-            (rc = it->d_susp[1].ensure((size_t)(kIterListHeader + num_queries) * 4))) {
+            (rc = it->d_susp[1].ensure((size_t)(kIterListHeader + num_queries) * 4)) ||
+            (rc = it->tables.open((size_t)num_queries, bits, it->visited_words, (IterState*)it->d_state.ptr, st0))) {
             delete it;
             return rc;
         }
-        it->q_bits.assign(num_queries, bits);
-        it->q_buf.assign(num_queries, 0);
-        it->q_set.resize(num_queries);
-        for (int q = 0; q < num_queries; ++q) it->q_set[q] = (unsigned int*)it->vbufs[0].ptr + (size_t)q * entries;
     }
-    IterState st0 = {};
-    st0.first = 1;   // first call: InitSearchTrees + SearchTrees
-    st0.slots = -1;  // no QueryResult yet: the first Next sets the slot count
-    st0.vbits = bits;
-    const std::vector<IterState> st(num_queries, st0);
     cudaError_t e = cudaMemcpy(it->d_queries.ptr, queries, qbytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && !it->hashed) e = cudaMemset(it->d_visited.ptr, 0, it->d_visited.bytes);
-    if (e == cudaSuccess && it->hashed) e = cudaMemset(it->vbufs[0].ptr, 0, it->vbufs[0].bytes);
-    if (e == cudaSuccess && it->hashed)
-        e = cudaMemcpy(it->d_tables.ptr, it->q_set.data(), (size_t)num_queries * sizeof(unsigned int*), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(it->d_state.ptr, st.data(), st.size() * sizeof(IterState), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && !it->hashed) {  // (the tables' open wrote the states of hashed sets)
+        const std::vector<IterState> st(num_queries, st0);
+        e = cudaMemset(it->d_visited.ptr, 0, it->d_visited.bytes);
+        if (e == cudaSuccess) e = cudaMemcpy(it->d_state.ptr, st.data(), st.size() * sizeof(IterState), cudaMemcpyHostToDevice);
+    }
     if (e != cudaSuccess) {
         delete it;
         return fail(SPTAG_B200_FAIL, "iterator set-up failed: %s", cudaGetErrorString(e));
@@ -2724,6 +2775,30 @@ namespace {
 // (ExtraFullGraphSearcher.h:167)
 int spann_page_limit(const sptag_b200_spann* s) { return std::max(s->page_limit, s->vector_limit_pages); }
 
+// The parameters a SPANN search or iterator step runs with, read together under s->mu
+struct SpannSnapshot {
+    int internal, page_limit, longest;
+    float max_dist_ratio;
+};
+// Takes the snapshot, and refuses a page limit that truncates lists of the rearranged layout: the reference reads a
+// truncated list's ids from an offset computed with the truncated count (ExtraFullGraphSearcher.h:1186-1190), and its
+// results on such lists are not reproduced
+int spann_snapshot(sptag_b200_spann* s, SpannSnapshot& out) {
+    bool truncated = false;
+    {
+        std::lock_guard<std::mutex> lock(s->mu);
+        out.internal = s->internal;
+        out.max_dist_ratio = s->max_dist_ratio;
+        out.page_limit = spann_page_limit(s);
+        out.longest = s->longest;
+        truncated = s->truncated;
+    }
+    if (truncated && s->rearranged)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchPostingPageLimit %d truncates posting lists of the rearranged layout",
+                    out.page_limit);
+    return 0;
+}
+
 // Elements of list l that a search reads (LoadingHeadInfo, ExtraFullGraphSearcher.h:1093-1097)
 int spann_searched(const sptag_b200_spann* s, int l, int limit) {
     return (int)std::min<long long>(s->cnt[l], ((long long)std::min(s->pages[l], limit) << 12) / s->vis);
@@ -2971,28 +3046,18 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     if (k < 1 || k > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "k = %d outside the supported range [1, 2048]", k);
     if (num_queries == 0) return SPTAG_B200_SUCCESS;
     sptag_b200_handle h = s->head;
+    SpannSnapshot sp;
+    if (int rc = spann_snapshot(s, sp)) return rc;
     SpannScanParams p;
     memset(&p, 0, sizeof(p));
-    int longest = 0;
-    bool truncated = false;
-    {
-        std::lock_guard<std::mutex> lock(s->mu);
-        p.internal = s->internal;
-        p.max_dist_ratio = s->max_dist_ratio;
-        p.page_limit = spann_page_limit(s);
-        longest = s->longest;
-        truncated = s->truncated;
-    }
+    p.internal = sp.internal;
+    p.max_dist_ratio = sp.max_dist_ratio;
+    p.page_limit = sp.page_limit;
     // SPANNIndex.cpp:197-201: the head search runs at K when K >= SearchInternalResultNum, else at SearchInternalResultNum
     const int w = k >= p.internal ? k : p.internal;
     if (w > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchInternalResultNum %d exceeds 2048", p.internal);
-    // With the rearranged layout the reference reads a truncated list's ids from an offset computed with the truncated
-    // count (ExtraFullGraphSearcher.h:1186-1190); its results on such lists are not reproduced, so the search is refused
-    if (truncated && s->rearranged)
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchPostingPageLimit %d truncates posting lists of the rearranged layout",
-                    p.page_limit);
     // the dedup table holds every element a query may read at half load
-    const long long reads = (long long)std::min(std::max(p.internal, 0), w) * longest;
+    const long long reads = (long long)std::min(std::max(p.internal, 0), w) * sp.longest;
     long long entries = 64;
     while (entries < 2 * reads) entries <<= 1;
     if (entries > (1ll << 30)) return fail(SPTAG_B200_MEMORY_OVERFLOW, "dedup table of %lld entries", entries);
@@ -3002,10 +3067,8 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     cudaStream_t stream = st->stream;
     const size_t nq = (size_t)num_queries;
     const size_t qrow = (size_t)h->dim * value_size(h->value_type);
-    const bool cosine = h->metric != SPTAG_B200_METRIC_L2;
-    int elem = 0;
-    with_elem(h, [&](auto el) { elem = el; });
-    int per_sm = spann_scan_blocks_per_sm(cosine, elem, w);
+    const MetricElem me = metric_elem(h);
+    int per_sm = spann_scan_blocks_per_sm(me.cosine, me.elem, w);
     if (per_sm < 1) return fail(SPTAG_B200_MEMORY_OVERFLOW, "the posting scan kernel does not fit on an SM at W = %d", w);
     // resident blocks, but no more dedup-table bytes than kTableBytes unless one block per SM needs more
     const long long kTableBytes = 256ll << 20;
@@ -3020,10 +3083,8 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     if (out_stats)
         if (int rc = st->d_stats.ensure(nq * 3 * 4)) return rc;
     if (int rc = st->d_tables.ensure((size_t)grid * entries * 4)) return rc;
-    CUDA_OK(cudaMemcpyAsync(st->d_q.ptr, queries, nq * qrow, cudaMemcpyHostToDevice, stream));
-    // the scan reads the queries as rows of the head's stride (16-byte aligned, zero padded)
-    CUDA_OK(cudaMemsetAsync(st->d_qpad.ptr, 0, nq * h->row_stride, stream));
-    CUDA_OK(cudaMemcpy2DAsync(st->d_qpad.ptr, h->row_stride, st->d_q.ptr, qrow, qrow, nq, cudaMemcpyDeviceToDevice, stream));
+    CUDA_OK(cudaMemcpyAsync(st->d_q.ptr, queries, nq * qrow, cudaMemcpyHostToDevice, stream));  // as the head search reads them
+    if (int rc = upload_query_rows(h, st->d_qpad.ptr, st->d_q.ptr, nq, stream)) return rc;
     {
         std::lock_guard<std::mutex> lock(h->mu);
         if (int rc = search_device_impl(h, st->d_q.ptr, num_queries, w, (int*)st->d_hids.ptr, (float*)st->d_hdists.ptr,
@@ -3053,7 +3114,7 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     p.out_ids = (int*)st->d_ids.ptr;
     p.out_dists = (float*)st->d_dists.ptr;
     p.out_stats = out_stats ? (int*)st->d_stats.ptr : nullptr;
-    cudaError_t e = launch_spann_scan(p, cosine, elem, grid, stream);
+    cudaError_t e = launch_spann_scan(p, me.cosine, me.elem, grid, stream);
     g_launches++;
     if (e != cudaSuccess) {
         cudaStreamSynchronize(stream);
@@ -3139,9 +3200,10 @@ struct sptag_b200_spann_iterator {
     int cap = 0;         // the QueryResult's size: the first Next's batch
     DeviceBuffer d_queries, d_state, d_posts, d_heap_d, d_heap_v, d_refill[2], d_susp[2], d_ids, d_dists, d_counts,
         d_relaxed;
-    // The dedup sets (OptHashPosVector, WorkSpace.h:43-165): exact sets that double when they fill, stored and grown as
-    // the head iterators' hashed visited sets are (grow_iter_visited); this iterator object holds only those tables.
-    sptag_b200_iterator dedup;
+    // The dedup sets (OptHashPosVector, WorkSpace.h:43-165): exact sets that double when they fill; d_dedup holds their
+    // IterStates
+    QueryTables dedup;
+    DeviceBuffer d_dedup;
 };
 
 namespace {
@@ -3185,43 +3247,25 @@ int sptag_b200_spann_iterator_open(sptag_b200_spann_handle s, const void* querie
     it->nq = num_queries;
     it->hb = hb;
     DeviceGuard guard(h->device);
-    const size_t nq = (size_t)num_queries, qrow = (size_t)h->dim * value_size(h->value_type);
-    sptag_b200_iterator& d = it->dedup;
-    d.nq = num_queries;
-    d.hashed = true;
-    d.visited_words = SIZE_MAX;  // a table never turns into a bitmap
-    d.vbufs.emplace_back();
-    d.vbuf_refs.push_back(num_queries);
+    const size_t nq = (size_t)num_queries;
     int rc = 0;
     if ((rc = it->d_queries.ensure(nq * h->row_stride)) || (rc = it->d_state.ensure(nq * sizeof(SpannIterState))) ||
         (rc = it->d_posts.ensure(nq * hb * 4)) || (rc = it->d_refill[0].ensure((kIterListHeader + nq) * 4)) ||
         (rc = it->d_refill[1].ensure((kIterListHeader + nq) * 4)) || (rc = it->d_susp[0].ensure((kIterListHeader + nq) * 4)) ||
         (rc = it->d_susp[1].ensure((kIterListHeader + nq) * 4)) || (rc = it->d_counts.ensure(nq * 4)) ||
-        (rc = it->d_relaxed.ensure(nq)) || (rc = d.d_state.ensure(nq * sizeof(IterState))) ||
-        (rc = d.d_tables.ensure(nq * sizeof(unsigned int*))) || (rc = d.vbufs[0].ensure(nq * entries * 4))) {
+        (rc = it->d_relaxed.ensure(nq)) || (rc = it->d_dedup.ensure(nq * sizeof(IterState))) ||
+        (rc = upload_query_rows(h, it->d_queries.ptr, queries, nq, nullptr)) ||
+        (rc = it->dedup.open(nq, bits, QueryTables::kNoBitmap, (IterState*)it->d_dedup.ptr))) {
         spann_iterator_free(it);
         return rc;
     }
-    d.q_bits.assign(nq, bits);
-    d.q_buf.assign(nq, 0);
-    d.q_set.resize(nq);
-    for (size_t q = 0; q < nq; ++q) d.q_set[q] = (unsigned int*)d.vbufs[0].ptr + q * entries;
     // GetIterator: relaxedMono = false, loadedPostingNum = 0, an empty deduper and posting list; the first head batch
     // is loaded by the first Next
     SpannIterState st0 = {};
     st0.load = 1;
     st0.slots = -1;
-    IterState ds0 = {};
-    ds0.vbits = bits;
     const std::vector<SpannIterState> st(nq, st0);
-    const std::vector<IterState> ds(nq, ds0);
-    cudaError_t e = cudaMemset(it->d_queries.ptr, 0, it->d_queries.bytes);  // rows of the head's stride, zero padded
-    if (e == cudaSuccess)
-        e = cudaMemcpy2D(it->d_queries.ptr, h->row_stride, queries, qrow, qrow, nq, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemset(d.vbufs[0].ptr, 0, d.vbufs[0].bytes);
-    if (e == cudaSuccess) e = cudaMemcpy(d.d_tables.ptr, d.q_set.data(), nq * sizeof(unsigned int*), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(d.d_state.ptr, ds.data(), nq * sizeof(IterState), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(it->d_state.ptr, st.data(), nq * sizeof(SpannIterState), cudaMemcpyHostToDevice);
+    const cudaError_t e = cudaMemcpy(it->d_state.ptr, st.data(), nq * sizeof(SpannIterState), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
         spann_iterator_free(it);
         return fail(SPTAG_B200_FAIL, "SPANN iterator set-up failed: %s", cudaGetErrorString(e));
@@ -3237,23 +3281,17 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     if (batch < 1 || batch > 1024) return fail(SPTAG_B200_LACK_OF_INPUTS, "batch = %d outside [1, 1024]", batch);
     sptag_b200_spann* s = it->s;
     sptag_b200_index* h = s->head;
+    SpannSnapshot sp;
+    if (int rc = spann_snapshot(s, sp)) return rc;
     SpannIterParams p;
     memset(&p, 0, sizeof(p));
-    bool truncated = false;
-    {
-        std::lock_guard<std::mutex> lock(s->mu);
-        p.internal = s->internal;
-        p.page_limit = spann_page_limit(s);
-        truncated = s->truncated;
-    }
+    p.internal = sp.internal;
+    p.page_limit = sp.page_limit;
     // The reference has SearchInternalResultNum page buffers and indexes them by m_pi (IExtraSearcher.h:114-122,
     // ExtraFullGraphSearcher.h:405, :500): a load of more lists is undefined there
     if (it->hb > p.internal)
         return fail(SPTAG_B200_LACK_OF_INPUTS, "IterativeSearchHeadBatch %d exceeds SearchInternalResultNum %d", it->hb,
                     p.internal);
-    if (truncated && s->rearranged)  // as sptag_b200_spann_search
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchPostingPageLimit %d truncates posting lists of the rearranged layout",
-                    p.page_limit);
     DeviceGuard guard(h->device);
     cudaStream_t stream = nullptr;  // the stream of the head iterator's steps
     const size_t nq = (size_t)it->nq;
@@ -3264,16 +3302,13 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     }
     if (int rc = it->d_ids.ensure(nq * batch * 4)) return rc;
     if (int rc = it->d_dists.ensure(nq * batch * 4)) return rc;
-    const bool cosine = h->metric != SPTAG_B200_METRIC_L2;
-    int elem = 0;
-    with_elem(h, [&](auto el) { elem = el; });
-    const int per_sm = spann_iter_step_blocks_per_sm(cosine, elem, it->cap);
+    const MetricElem me = metric_elem(h);
+    const int per_sm = spann_iter_step_blocks_per_sm(me.cosine, me.elem, it->cap);
     if (per_sm < 1) return fail(SPTAG_B200_MEMORY_OVERFLOW, "the posting step kernel does not fit on an SM");
     const long long max_grid = (long long)h->num_sms * per_sm;
     // SearchIndexIterative's first call: the head's FromNeareast(first = true) at the head batch (SPANNIndex.cpp:271-275)
     if (!it->head->stepped)
         if (int rc = nearest_step(it->head, it->hb, nullptr, nullptr, nullptr)) return rc;
-    sptag_b200_iterator& d = it->dedup;
     p.head_ids = (const int*)it->head->d_ids.ptr;
     p.nq = it->nq;
     p.hb = it->hb;
@@ -3294,8 +3329,8 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     p.heap_d = (float*)it->d_heap_d.ptr;
     p.heap_v = (int*)it->d_heap_v.ptr;
     p.cap = it->cap;
-    p.tables = (unsigned int* const*)d.d_tables.ptr;
-    p.dedup = (IterState*)d.d_state.ptr;
+    p.tables = (unsigned int* const*)it->dedup.d_tables.ptr;
+    p.dedup = it->dedup.state;
     p.out_ids = (int*)it->d_ids.ptr;
     p.out_dists = (float*)it->d_dists.ptr;
     p.out_counts = (int*)it->d_counts.ptr;
@@ -3308,7 +3343,7 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
         return 0;
     };
     auto launch = [&](long long n) -> int {
-        const cudaError_t e = launch_spann_iter_step(p, cosine, elem, (int)std::min(n, max_grid), stream);
+        const cudaError_t e = launch_spann_iter_step(p, me.cosine, me.elem, (int)std::min(n, max_grid), stream);
         g_launches++;
         if (e != cudaSuccess) return fail(SPTAG_B200_FAIL, "posting step launch failed: %s", cudaGetErrorString(e));
         return 0;
@@ -3321,16 +3356,10 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     p.fresh = 0;
     long rounds = 0;
     for (;;) {
-        unsigned hdr[2][kIterListHeader];
+        unsigned hdr[2][kIterListHeader];  // the refill and suspension lists' headers, read with one synchronisation
         CUDA_OK(cudaMemcpyAsync(hdr[0], p.refill, sizeof(hdr[0]), cudaMemcpyDeviceToHost, stream));
-        CUDA_OK(cudaMemcpyAsync(hdr[1], p.susp, sizeof(hdr[1]), cudaMemcpyDeviceToHost, stream));
-        CUDA_OK(cudaStreamSynchronize(stream));
-        if (hdr[1][0] > 0) {  // double the listed tables and run those queries on (they append to the same refill list)
-            std::vector<unsigned> qs(hdr[1][0]);
-            CUDA_OK(cudaMemcpy(qs.data(), (unsigned*)p.susp + kIterListHeader, qs.size() * 4, cudaMemcpyDeviceToHost));
-            std::vector<int> bits(qs.size());
-            for (size_t i = 0; i < qs.size(); ++i) bits[i] = d.q_bits[qs[i]] + 1;
-            if (int rc = grow_iter_visited(&d, qs, bits, true, stream)) return rc;
+        if (int rc = it->dedup.double_listed(p.susp, hdr[1], true, stream)) return rc;
+        if (hdr[1][0] > 0) {  // the listed tables doubled: run those queries on (they append to the same refill list)
             p.list = p.susp;
             scur ^= 1;
             if (int rc = lists(cur, scur, false)) return rc;
@@ -3353,7 +3382,7 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     CUDA_OK(cudaStreamSynchronize(stream));
     std::lock_guard<std::mutex> lock(s->mu);
     s->last_iter_rounds = rounds;
-    s->last_iter_dedup_bytes = (long)d.visited_bytes();
+    s->last_iter_dedup_bytes = (long)it->dedup.bytes();
     return SPTAG_B200_SUCCESS;
 }
 
@@ -3411,15 +3440,8 @@ int sptag_b200_multi_scan(const sptag_b200_handle* indexes, int32_t num_indexes,
     cudaStream_t stream = nullptr;  // the stream of the iterator steps
     const size_t nq = (size_t)num_queries;
     std::vector<DeviceBuffer> d_q(n);
-    DeviceBuffer d_cross, d_state, d_heap_s, d_heap_v, d_list[2], d_ids, d_scores, d_counts, d_stats;
-    // seenSet: one table per query in the hashed visited-set format, doubled with grow_iter_visited; this object holds
-    // only those tables
-    sptag_b200_iterator seen;
-    seen.nq = num_queries;
-    seen.hashed = true;
-    seen.visited_words = SIZE_MAX;  // a table never turns into a bitmap
-    seen.vbufs.emplace_back();
-    seen.vbuf_refs.push_back(num_queries);
+    DeviceBuffer d_cross, d_state, d_heap_s, d_heap_v, d_list[2], d_ids, d_scores, d_counts, d_stats, d_seen;
+    QueryTables seen;  // seenSet, one table per query; d_seen holds their IterStates
     int bits = 7;
     int rc = 0;
     for (int i = 0; i < n && !rc; ++i) rc = d_q[i].ensure(nq * indexes[i]->row_stride);
@@ -3427,29 +3449,15 @@ int sptag_b200_multi_scan(const sptag_b200_handle* indexes, int32_t num_indexes,
         (rc = d_heap_s.ensure(nq * k * 4)) || (rc = d_heap_v.ensure(nq * k * 4)) ||
         (rc = d_list[0].ensure((kIterListHeader + nq) * 4)) || (rc = d_list[1].ensure((kIterListHeader + nq) * 4)) ||
         (rc = d_ids.ensure(nq * k * 4)) || (rc = d_scores.ensure(nq * k * 4)) || (rc = d_counts.ensure(nq * 4)) ||
-        (rc = d_stats.ensure(nq * 16)) || (rc = seen.d_state.ensure(nq * sizeof(IterState))) ||
-        (rc = seen.d_tables.ensure(nq * sizeof(unsigned int*))) || (rc = seen.vbufs[0].ensure(nq * (4u << bits))))
+        (rc = d_stats.ensure(nq * 16)) || (rc = d_seen.ensure(nq * sizeof(IterState))))
         return rc;
-    seen.q_bits.assign(nq, bits);
-    seen.q_buf.assign(nq, 0);
-    seen.q_set.resize(nq);
-    for (size_t q = 0; q < nq; ++q) seen.q_set[q] = (unsigned int*)seen.vbufs[0].ptr + (q << bits);
-    IterState ss0 = {};
-    ss0.vbits = bits;
-    const std::vector<IterState> ss(nq, ss0);
     const std::vector<MultiScanState> st(nq, MultiScanState{0, 0, -1, 0});
     std::vector<unsigned> list0(kIterListHeader + nq, 0);
     list0[0] = (unsigned)nq;
     for (size_t q = 0; q < nq; ++q) list0[kIterListHeader + q] = (unsigned)q;
-    for (int i = 0; i < n; ++i) {  // rows of the index's stride, zero padded, as the distance reads them
-        const sptag_b200_index* h = indexes[i];
-        const size_t qrow = (size_t)h->dim * value_size(h->value_type);
-        CUDA_OK(cudaMemset(d_q[i].ptr, 0, d_q[i].bytes));
-        CUDA_OK(cudaMemcpy2D(d_q[i].ptr, h->row_stride, queries[i], qrow, qrow, nq, cudaMemcpyHostToDevice));
-    }
-    CUDA_OK(cudaMemset(seen.vbufs[0].ptr, 0, seen.vbufs[0].bytes));
-    CUDA_OK(cudaMemcpy(seen.d_tables.ptr, seen.q_set.data(), nq * sizeof(unsigned int*), cudaMemcpyHostToDevice));
-    CUDA_OK(cudaMemcpy(seen.d_state.ptr, ss.data(), nq * sizeof(IterState), cudaMemcpyHostToDevice));
+    for (int i = 0; i < n; ++i)
+        if (int rc2 = upload_query_rows(indexes[i], d_q[i].ptr, queries[i], nq, stream)) return rc2;
+    if (int rc2 = seen.open(nq, bits, QueryTables::kNoBitmap, (IterState*)d_seen.ptr)) return rc2;
     CUDA_OK(cudaMemcpy(d_state.ptr, st.data(), nq * sizeof(MultiScanState), cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(d_list[0].ptr, list0.data(), list0.size() * 4, cudaMemcpyHostToDevice));
 
@@ -3468,7 +3476,7 @@ int sptag_b200_multi_scan(const sptag_b200_handle* indexes, int32_t num_indexes,
     mp.heap_s = (float*)d_heap_s.ptr;
     mp.heap_v = (int*)d_heap_v.ptr;
     mp.tables = (unsigned int* const*)seen.d_tables.ptr;
-    mp.seen = (IterState*)seen.d_state.ptr;
+    mp.seen = seen.state;
     const int max_grid = std::max(1, h0->num_sms) * 32;
     long long rounds = 0;
     unsigned active = (unsigned)nq;
@@ -3482,7 +3490,7 @@ int sptag_b200_multi_scan(const sptag_b200_handle* indexes, int32_t num_indexes,
             while (fill_bound > (1ll << (bits - 1))) ++bits;
             if (bits > 30) return fail(SPTAG_B200_MEMORY_OVERFLOW, "seen-set table of 2^%d entries", bits);
             const std::vector<int> nb(active, bits);
-            if (int rc2 = grow_iter_visited(&seen, qs, nb, true, stream)) return rc2;
+            if (int rc2 = seen.grow(qs, nb, true, stream)) return rc2;
         }
         const unsigned* list = (const unsigned*)d_list[cur].ptr;
         for (int i = 0; i < n; ++i)  // Next(1) on every index
@@ -3507,9 +3515,8 @@ int sptag_b200_multi_scan(const sptag_b200_handle* indexes, int32_t num_indexes,
             dp.dim = h->dim;
             dp.simd_width = h->simd_width;
             dp.cross = (float*)d_cross.ptr;
-            int elem = 0;
-            with_elem(h, [&](auto el) { elem = el; });
-            const cudaError_t e = launch_multi_scan_distance(dp, h->metric != SPTAG_B200_METRIC_L2, elem, grid, stream);
+            const MetricElem me = metric_elem(h);
+            const cudaError_t e = launch_multi_scan_distance(dp, me.cosine, me.elem, grid, stream);
             g_launches++;
             if (e != cudaSuccess) return fail(SPTAG_B200_FAIL, "multi-scan distance launch failed: %s", cudaGetErrorString(e));
         }
@@ -3528,7 +3535,7 @@ int sptag_b200_multi_scan(const sptag_b200_handle* indexes, int32_t num_indexes,
     dr.k = k;
     dr.id_offset = h0->id_offset;
     dr.st = (MultiScanState*)d_state.ptr;
-    dr.seen = (const IterState*)seen.d_state.ptr;
+    dr.seen = seen.state;
     dr.heap_s = (float*)d_heap_s.ptr;
     dr.heap_v = (int*)d_heap_v.ptr;
     dr.out_ids = (int*)d_ids.ptr;
