@@ -152,7 +152,10 @@ void sptag_b200_destroy(sptag_b200_handle h);
  * call of this handle; 0 on the bitmap), B200.ScratchBytes (device bytes held by the handle's search scratch sets),
  * B200.LastIteratorSuspensions ("step,trees": how often the last iterator call suspended a query at the top of a step /
  * before a tree pop to grow its table), B200.LastIteratorGrowths (tables grown or restarted by that call),
- * B200.LastIteratorVisitedBytes (device bytes of that iterator's visited sets after the call). */
+ * B200.LastIteratorVisitedBytes (device bytes of that iterator's visited sets after the call), B200.LastRefineSearchUs
+ * and B200.LastRefineRebuildUs (device microseconds of the last sptag_b200_refine_graph call's search and rebuild).
+ * Names are matched case-insensitively, as the reference's StrEqualIgnoreCase does.  Unknown names are ParamNotFound;
+ * writing a read-only name is LackOfInputs. */
 int sptag_b200_set_param(sptag_b200_handle h, const char* name, const char* value);
 int sptag_b200_get_param(sptag_b200_handle h, const char* name, char* value_out, int32_t capacity);
 
@@ -372,8 +375,8 @@ int sptag_b200_save(sptag_b200_handle h, const char* folder);
  * LoadIndexData, SPANNIndex.cpp:59-140, ExtraFullGraphSearcher::LoadIndex / LoadingHeadInfo, ExtraFullGraphSearcher.h:
  * 163-220, :1030-1120).  Reads indexloader.ini ([Base] ValueType, HeadIndexFolder, HeadVectorIDs; [BuildSSDIndex]
  * SSDIndex, SearchInternalResultNum, MaxDistRatio, SearchPostingPageLimit, PostingVectorLimit,
- * EnablePostingListRearrange), loads the head folder with sptag_b200_load and applies the [BuildHead] search parameters
- * to it as SPANN::Index::SetParameter does (:1033-1038), reads the translate map and every posting file (SSDIndex,
+ * EnablePostingListRearrange), loads the head folder with sptag_b200_load and applies to it the [BuildHead] keys that
+ * sptag_b200_load reads from [Index], as SPANN::Index::SetParameter does (:1033-1038), reads the translate map and every posting file (SSDIndex,
  * SSDIndex_1, ...) in the plain or the rearranged layout, and packs the lists into HBM.  Each list keeps its full element
  * count; SearchPostingPageLimit truncates at search time.  Section and parameter names are read case-insensitively, as
  * Helper::IniReader reads them.  LackOfInputs for EnableDataCompression, EnableDeltaEncoding and quantized SPANN.  Device
@@ -404,7 +407,8 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
  * B200.SpannDedupEntries: the first dedup table size of an iterator's queries, 0 (default: room for one head batch of
  * the longest list, at most 2^14) or a power of two >= 64; tables double as they fill.  Read-only: PostingBytes (device
  * bytes of the posting lists and the translate map), B200.LastIteratorRounds (head refill rounds of the last
- * sptag_b200_spann_iterator_next on this handle) and B200.LastIteratorDedupBytes (that iterator's dedup table bytes). */
+ * sptag_b200_spann_iterator_next on this handle) and B200.LastIteratorDedupBytes (that iterator's dedup table bytes).
+ * Names are matched case-insensitively, and codes are those of sptag_b200_set_param. */
 int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, const char* value);
 int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char* value_out, int32_t capacity);
 

@@ -25,6 +25,7 @@
 #include <fstream>
 #include <map>
 #include <mutex>
+#include <strings.h>
 #include <sys/stat.h>
 #include <sstream>
 #include <string>
@@ -1375,6 +1376,143 @@ const char* enum_name(const EnumName (&names)[N], int value) {
     return "Undefined";
 }
 
+// The parameters of a handle type H, one table per type as the reference's ParameterDefinitionList.h keeps them:
+// set_param, get_param and the ini loaders all read the table.  Names match case-insensitively (StrEqualIgnoreCase,
+// BKTIndex.cpp:980-1025).
+enum : unsigned {
+    kRefKey = 1,   // a key of the reference's ini: read from [Index] by sptag_b200_load, from [BuildHead] for a SPANN head
+    kBktOnly = 2,  // BKT handles only: ParamNotFound on KDT
+    kBool = 4,     // stored as v != 0
+    kPow2 = 8,     // accepted: 0 or a power of two in [64, 2^30]
+    kHead = 16,    // SPANN: the head handle's parameter, set and read there
+};
+template <typename H>
+struct Param {
+    const char* name;
+    unsigned flags = 0;
+    int H::*i = nullptr;                      // an int value (strtol, base 10)
+    float H::*f = nullptr;                    // a float value (strtof)
+    long lo = LONG_MIN, hi = LONG_MAX;        // the int values accepted
+    int (*set)(H*, long) = nullptr;           // stores an accepted int value in place of i, with the side effects
+    int (*get)(H*, char*, size_t) = nullptr;  // prints a read-only value
+    Param(const char* n, int H::*m, unsigned fl = 0, long l = LONG_MIN, long u = LONG_MAX, int (*s)(H*, long) = nullptr)
+        : name(n), flags(fl), i(m), lo(l), hi(u), set(s) {}
+    Param(const char* n, float H::*m, unsigned fl = 0) : name(n), flags(fl), f(m) {}
+    Param(const char* n, int (*g)(H*, char*, size_t)) : name(n), get(g) {}
+    Param(const char* n, unsigned fl) : name(n), flags(fl) {}
+};
+
+template <typename H, size_t N>
+const Param<H>* find_param(const Param<H> (&table)[N], const char* name, bool bkt = true) {
+    for (const Param<H>& p : table)
+        if (strcasecmp(p.name, name) == 0) return (p.flags & kBktOnly) && !bkt ? nullptr : &p;
+    return nullptr;
+}
+
+// p: find_param's result for name.  The caller holds the lock of h's parameters.
+template <typename H>
+int set_param(H* h, const Param<H>* p, const char* name, const char* value) {
+    if (!p) return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
+    if (p->get) return fail(SPTAG_B200_LACK_OF_INPUTS, "%s is read-only", p->name);
+    char* end = nullptr;
+    const float x = p->f ? strtof(value, &end) : 0.0f;
+    const long v = p->f ? 0 : strtol(value, &end, 10);
+    if (end == value) return fail(SPTAG_B200_FAILED_PARSE_VALUE, "cannot parse '%s' for %s", value, p->name);
+    if (p->f) {
+        h->*p->f = x;
+        return SPTAG_B200_SUCCESS;
+    }
+    if ((p->flags & kPow2) && v != 0 && (v < 64 || v > (1l << 30) || (v & (v - 1)) != 0))
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "%s %ld: 0 or a power of two in [64, 2^30]", p->name, v);
+    if (v < p->lo || v > p->hi) return fail(SPTAG_B200_LACK_OF_INPUTS, "%s %ld outside [%ld, %ld]", p->name, v, p->lo, p->hi);
+    if (p->set) return p->set(h, v);
+    h->*p->i = (p->flags & kBool) ? (v != 0) : (int)v;
+    return SPTAG_B200_SUCCESS;
+}
+
+int put(char* out, size_t capacity, const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(out, capacity, fmt, ap);
+    va_end(ap);
+    return SPTAG_B200_SUCCESS;
+}
+
+template <typename H>
+int get_param(H* h, const Param<H>* p, const char* name, char* out, size_t capacity) {
+    if (!p) return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
+    if (p->get) return p->get(h, out, capacity);
+    return p->f ? put(out, capacity, "%f", h->*p->f) : put(out, capacity, "%d", h->*p->i);  // %f: as ConvertToString
+}
+
+using Index = sptag_b200_index;
+const Param<Index> kIndexParams[] = {
+    {"MaxCheck", &Index::max_check, kRefKey},  // search: BKT/ParameterDefinitionList.h:44-49
+    {"MaxCheckForRefineGraph", &Index::max_check_refine, kRefKey},
+    {"NumberOfInitialDynamicPivots", &Index::initial_pivots, kRefKey},
+    {"NumberOfOtherDynamicPivots", &Index::other_pivots, kRefKey},
+    {"ThresholdOfNumberOfContinuousNoBetterPropagation", &Index::no_better_threshold, kRefKey},
+    {"EnableBfs", &Index::bfs, kRefKey | kBktOnly},  // any int, like BKTree::m_bfs
+    {"AddCEF", &Index::add_cef, kRefKey},  // graph updates: BKT/ParameterDefinitionList.h:28-31
+    {"CEF", &Index::cef, kRefKey},
+    {"RNGFactor", &Index::rng_factor, kRefKey},
+    {"SearchDeleted", &Index::search_deleted, kBool},
+    {"EnableADC", &Index::q_adc, kBool},  // VectorIndex::SetQuantizerADC (VectorIndex.h:136-138)
+    {"B200.QueriesPerSM", &Index::queries_per_sm},
+    {"B200.StageRows", &Index::stage_rows},
+    {"B200.Stages", &Index::stages, 0, LONG_MIN, LONG_MAX,
+     [](Index* h, long v) { h->stages = (int)v; h->stages_set = true; return SPTAG_B200_SUCCESS; }},
+    {"B200.NGCacheEntries", &Index::h_ng},
+    {"B200.SPTCacheEntries", &Index::h_spt},
+    {"B200.SimdWidth", &Index::simd_width},
+    {"B200.SlotScheme", &Index::slot_scheme},
+    {"B200.VisitedLog", &Index::visited_log},
+    {"B200.VisitedLogEntries", &Index::visited_log_entries},
+    {"B200.VisitedSet", &Index::visited_set, 0, -1, 1, [](Index* h, long v) {
+         h->visited_set = (int)v;
+         for (auto& sc : h->scratch) sc.bitmap_unfit = 0;  // auto tries the bitmap again
+         return SPTAG_B200_SUCCESS;
+     }},
+    {"B200.VisitedHashEntries", &Index::visited_hash_entries, kPow2},
+    {"B200.IteratorVisitedSet", &Index::iter_visited_set, 0, -1, 1},  // taken by iterators opened afterwards
+    {"B200.IteratorVisitedHashEntries", &Index::iter_hash_entries, kPow2},
+    {"B200.RowSketch", &Index::row_sketch, 0, -1, 1, [](Index* h, long v) {
+         if (v == 1 && !(h->value_type == SPTAG_B200_VT_FLOAT && h->q_type == 0 && h->algo == SPTAG_B200_ALGO_BKT))
+             return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.RowSketch 1: row sketches exist for float BKT indexes only");
+         h->row_sketch = (int)v;
+         h->sketch_unfit = false;  // auto tries the allocation again
+         if (v == 0) { h->d_sketch.release(); h->sketch_n = 0; }
+         return SPTAG_B200_SUCCESS;
+     }},
+    {"B200.RowsSkipped", [](Index* h, char* o, size_t n) {  // since the handle was made, over the searches that have finished
+         unsigned long long c = 0;
+         if (h->d_skipped.ptr) {
+             DeviceGuard guard(h->device);
+             CUDA_OK(cudaDeviceSynchronize());
+             CUDA_OK(cudaMemcpy(&c, h->d_skipped.ptr, 8, cudaMemcpyDeviceToHost));
+         }
+         return put(o, n, "%ld", (long)c);
+     }},
+    {"B200.LastVisitedOverflows", [](Index* h, char* o, size_t n) { return put(o, n, "%d", h->last_visited_overflows.load()); }},
+    {"B200.ScratchBytes", [](Index* h, char* o, size_t n) { return put(o, n, "%zu", h->scratch[0].bytes() + h->scratch[1].bytes()); }},
+    {"B200.LastIteratorSuspensions",  // "step,trees" of the last iterator call
+     [](Index* h, char* o, size_t n) { return put(o, n, "%ld,%ld", h->last_iter_susp_step, h->last_iter_susp_trees); }},
+    {"B200.LastIteratorGrowths", [](Index* h, char* o, size_t n) { return put(o, n, "%ld", h->last_iter_growths); }},
+    {"B200.LastIteratorVisitedBytes", [](Index* h, char* o, size_t n) { return put(o, n, "%ld", h->last_iter_visited_bytes); }},
+    // device time of the last refine pass
+    {"B200.LastRefineSearchUs", [](Index* h, char* o, size_t n) { return put(o, n, "%ld", (long)(h->refine_search_ms * 1e3)); }},
+    {"B200.LastRefineRebuildUs", [](Index* h, char* o, size_t n) { return put(o, n, "%ld", (long)(h->refine_rebuild_ms * 1e3)); }},
+};
+
+// The reference keys of kIndexParams present in ini's section, set on h.  Values set_param refuses are ignored, as
+// LoadIndex ignores a failed ConvertStringTo.
+void load_ref_keys(sptag_b200_index* h, const IniSections& ini, const char* section) {
+    for (const Param<Index>& p : kIndexParams) {
+        const std::string v = (p.flags & kRefKey) ? ini_get(ini, section, p.name, "") : "";
+        if (!v.empty()) sptag_b200_set_param(h, p.name, v.c_str());
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -1532,14 +1670,7 @@ int sptag_b200_load(const char* folder, int32_t device, int32_t id_offset, sptag
             return rc;
         }
     }
-    static const char* names[] = {"MaxCheck", "MaxCheckForRefineGraph", "NumberOfInitialDynamicPivots",
-                                  "NumberOfOtherDynamicPivots", "ThresholdOfNumberOfContinuousNoBetterPropagation",
-                                  "AddCEF", "CEF", "RNGFactor", "EnableBfs"};
-    for (const char* nm : names) {
-        const std::string v = get(nm, "");
-        // (EnableBfs is a BKT parameter: set_param refuses it on a KDT handle, and the KDT loader ignores the key)
-        if (!v.empty()) sptag_b200_set_param(h, nm, v.c_str());
-    }
+    load_ref_keys(h, ini, "Index");  // (EnableBfs is BKT-only: the KDT loader ignores the key)
     *out = h;
     return SPTAG_B200_SUCCESS;
 }
@@ -1616,118 +1747,14 @@ int sptag_b200_quantize(sptag_b200_handle h, const void* raw_vectors, int32_t nu
 
 int sptag_b200_set_param(sptag_b200_handle h, const char* name, const char* value) {
     if (!h || !name || !value) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
-    char* end = nullptr;
-    const long v = strtol(value, &end, 10);
-    if (end == value) return fail(SPTAG_B200_FAILED_PARSE_VALUE, "cannot parse '%s' for %s", value, name);
     std::lock_guard<std::mutex> lock(h->mu);
-    const std::string n(name);
-    if (n == "MaxCheck") h->max_check = (int)v;
-    else if (n == "MaxCheckForRefineGraph") h->max_check_refine = (int)v;
-    else if (n == "AddCEF") h->add_cef = (int)v;
-    else if (n == "CEF") h->cef = (int)v;
-    else if (n == "RNGFactor") h->rng_factor = strtof(value, nullptr);
-    else if (n == "SearchDeleted") h->search_deleted = (v != 0) ? 1 : 0;
-    else if (n == "NumberOfInitialDynamicPivots") h->initial_pivots = (int)v;
-    else if (n == "NumberOfOtherDynamicPivots") h->other_pivots = (int)v;
-    else if (n == "ThresholdOfNumberOfContinuousNoBetterPropagation") h->no_better_threshold = (int)v;
-    else if (n == "EnableBfs" && h->algo == SPTAG_B200_ALGO_BKT) h->bfs = (int)v;  // any int, like BKTree::m_bfs
-    else if (n == "B200.QueriesPerSM") h->queries_per_sm = (int)v;
-    else if (n == "B200.StageRows") h->stage_rows = (int)v;
-    else if (n == "B200.Stages") { h->stages = (int)v; h->stages_set = true; }
-    else if (n == "B200.NGCacheEntries") h->h_ng = (int)v;
-    else if (n == "B200.SPTCacheEntries") h->h_spt = (int)v;
-    else if (n == "B200.SimdWidth") h->simd_width = (int)v;
-    else if (n == "B200.VisitedLog") h->visited_log = (int)v;
-    else if (n == "B200.VisitedLogEntries") h->visited_log_entries = (int)v;
-    else if (n == "B200.VisitedSet") {
-        if (v < -1 || v > 1) return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.VisitedSet %ld: -1 (auto), 0 (bitmap) or 1 (hashed)", v);
-        h->visited_set = (int)v;
-        for (auto& sc : h->scratch) sc.bitmap_unfit = 0;  // auto tries the bitmap again
-    } else if (n == "B200.VisitedHashEntries") {
-        if (v != 0 && (v < 64 || v > (1l << 30) || (v & (v - 1)) != 0))
-            return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.VisitedHashEntries %ld: 0 (default) or a power of two in [64, 2^30]", v);
-        h->visited_hash_entries = (int)v;
-    } else if (n == "B200.IteratorVisitedSet") {  // taken by iterators opened afterwards
-        if (v < -1 || v > 1)
-            return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.IteratorVisitedSet %ld: -1 (auto), 0 (bitmap) or 1 (hashed)", v);
-        h->iter_visited_set = (int)v;
-    } else if (n == "B200.IteratorVisitedHashEntries") {
-        if (v != 0 && (v < 64 || v > (1l << 30) || (v & (v - 1)) != 0))
-            return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.IteratorVisitedHashEntries %ld: 0 (default) or a power of two in [64, 2^30]", v);
-        h->iter_hash_entries = (int)v;
-    }
-    else if (n == "B200.SlotScheme") h->slot_scheme = (int)v;
-    else if (n == "B200.RowSketch") {
-        if (v < -1 || v > 1) return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.RowSketch %ld: -1 (auto), 0 (off) or 1 (on)", v);
-        if (v == 1 && !(h->value_type == SPTAG_B200_VT_FLOAT && h->q_type == 0 && h->algo == SPTAG_B200_ALGO_BKT))
-            return fail(SPTAG_B200_LACK_OF_INPUTS, "B200.RowSketch 1: row sketches exist for float BKT indexes only");
-        h->row_sketch = (int)v;
-        h->sketch_unfit = false;  // auto tries the allocation again
-        if (v == 0) {
-            h->d_sketch.release();
-            h->sketch_n = 0;
-        }
-    }
-    else if (n == "EnableADC") h->q_adc = (v != 0);  // VectorIndex::SetQuantizerADC (VectorIndex.h:136-138)
-    else return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
-    return SPTAG_B200_SUCCESS;
+    return set_param(h, find_param(kIndexParams, name, h->algo == SPTAG_B200_ALGO_BKT), name, value);
 }
 
 int sptag_b200_get_param(sptag_b200_handle h, const char* name, char* value_out, int32_t capacity) {
     if (!h || !name || !value_out || capacity <= 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
     std::lock_guard<std::mutex> lock(h->mu);
-    const std::string n(name);
-    long v;
-    if (n == "RNGFactor") {  // float, printed like the reference's ini (ConvertToString)
-        snprintf(value_out, (size_t)capacity, "%f", h->rng_factor);
-        return SPTAG_B200_SUCCESS;
-    }
-    if (n == "B200.LastIteratorSuspensions") {  // read-only: "step,trees" of the last iterator call
-        snprintf(value_out, (size_t)capacity, "%ld,%ld", h->last_iter_susp_step, h->last_iter_susp_trees);
-        return SPTAG_B200_SUCCESS;
-    }
-    if (n == "MaxCheck") v = h->max_check;
-    else if (n == "MaxCheckForRefineGraph") v = h->max_check_refine;
-    else if (n == "AddCEF") v = h->add_cef;
-    else if (n == "CEF") v = h->cef;
-    else if (n == "SearchDeleted") v = h->search_deleted;
-    else if (n == "NumberOfInitialDynamicPivots") v = h->initial_pivots;
-    else if (n == "NumberOfOtherDynamicPivots") v = h->other_pivots;
-    else if (n == "ThresholdOfNumberOfContinuousNoBetterPropagation") v = h->no_better_threshold;
-    else if (n == "EnableBfs" && h->algo == SPTAG_B200_ALGO_BKT) v = h->bfs;
-    else if (n == "B200.QueriesPerSM") v = h->queries_per_sm;
-    else if (n == "B200.StageRows") v = h->stage_rows;
-    else if (n == "B200.Stages") v = h->stages;
-    else if (n == "B200.NGCacheEntries") v = h->h_ng;
-    else if (n == "B200.SPTCacheEntries") v = h->h_spt;
-    else if (n == "B200.SimdWidth") v = h->simd_width;
-    else if (n == "B200.VisitedLog") v = h->visited_log;
-    else if (n == "B200.VisitedLogEntries") v = h->visited_log_entries;
-    else if (n == "B200.VisitedSet") v = h->visited_set;
-    else if (n == "B200.VisitedHashEntries") v = h->visited_hash_entries;
-    else if (n == "B200.LastVisitedOverflows") v = h->last_visited_overflows;       // read-only
-    else if (n == "B200.ScratchBytes") v = (long)(h->scratch[0].bytes() + h->scratch[1].bytes());  // read-only
-    else if (n == "B200.IteratorVisitedSet") v = h->iter_visited_set;
-    else if (n == "B200.IteratorVisitedHashEntries") v = h->iter_hash_entries;
-    else if (n == "B200.LastIteratorGrowths") v = h->last_iter_growths;                // read-only
-    else if (n == "B200.LastIteratorVisitedBytes") v = h->last_iter_visited_bytes;     // read-only
-    else if (n == "B200.SlotScheme") v = h->slot_scheme;
-    else if (n == "B200.RowSketch") v = h->row_sketch;
-    else if (n == "B200.RowsSkipped") {  // read-only: since the handle was made, over the searches that have finished
-        unsigned long long c = 0;
-        if (h->d_skipped.ptr) {
-            DeviceGuard guard(h->device);
-            CUDA_OK(cudaDeviceSynchronize());
-            CUDA_OK(cudaMemcpy(&c, h->d_skipped.ptr, 8, cudaMemcpyDeviceToHost));
-        }
-        v = (long)c;
-    }
-    else if (n == "EnableADC") v = h->q_adc;
-    else if (n == "B200.LastRefineSearchUs") v = (long)(h->refine_search_ms * 1000.0);    // read-only: device time
-    else if (n == "B200.LastRefineRebuildUs") v = (long)(h->refine_rebuild_ms * 1000.0);  // of the last refine pass
-    else return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
-    snprintf(value_out, (size_t)capacity, "%ld", v);
-    return SPTAG_B200_SUCCESS;
+    return get_param(h, find_param(kIndexParams, name, h->algo == SPTAG_B200_ALGO_BKT), name, value_out, (size_t)capacity);
 }
 
 int sptag_b200_search_device(sptag_b200_handle h, const void* d_queries, int32_t num_queries, int32_t k,
@@ -2817,6 +2844,27 @@ void spann_update_shape(sptag_b200_spann* s) {
     }
 }
 
+// Search parameters (SPANN/ParameterDefinitionList.h:110-125), under s->mu; the kHead ones are set and read on the head
+// (SPANNIndex.cpp:901) without it
+using Spann = sptag_b200_spann;
+const Param<Spann> kSpannParams[] = {
+    {"MaxCheck", kHead},
+    {"B200.IteratorVisitedSet", kHead},  // with the next: the visited sets of the head iterators SPANN iterators open
+    {"B200.IteratorVisitedHashEntries", kHead},
+    {"SearchInternalResultNum", &Spann::internal, 0, 0, 2048,
+     [](Spann* s, long v) { s->internal = (int)v; spann_update_shape(s); return SPTAG_B200_SUCCESS; }},
+    {"SearchPostingPageLimit", &Spann::page_limit, 0, 0, 2048,
+     [](Spann* s, long v) { s->page_limit = (int)v; spann_update_shape(s); return SPTAG_B200_SUCCESS; }},
+    {"MaxDistRatio", &Spann::max_dist_ratio},
+    {"IterativeSearchHeadBatch", &Spann::head_batch, 0, 1, 1024},
+    {"B200.SpannDedupEntries", &Spann::dedup_entries, kPow2},
+    {"PostingBytes", [](Spann* s, char* o, size_t n) {
+         return put(o, n, "%zu", s->d_translate.bytes + s->d_off.bytes + s->d_cnt.bytes + s->d_pages.bytes + s->d_ids.bytes + s->d_rows.bytes);
+     }},
+    {"B200.LastIteratorRounds", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_iter_rounds); }},
+    {"B200.LastIteratorDedupBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_iter_dedup_bytes); }},
+};
+
 // One posting file (OutputSSDIndexFile, ExtraFullGraphSearcher.h:1292-1420; read as LoadingHeadInfo does, :1030-1120):
 // int32 listCount, totalDocCount, dim, listPageOffset; per list int32 pageNum, uint16 pageOffset, int32 listEleCount,
 // uint16 listPageCount; list l's bytes start at ((listPageOffset + pageNum) << 12) + pageOffset
@@ -2863,12 +2911,7 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
     auto get = [&](const char* section, const char* name, const char* def) { return ini_get(ini, section, name, def); };
     sptag_b200_handle head = s->head;
     // SPANN::Index::LoadConfig hands every [BuildHead] entry to the head (SPANNIndex.cpp:59-71, :1033-1038)
-    static const char* head_names[] = {"MaxCheck", "NumberOfInitialDynamicPivots", "NumberOfOtherDynamicPivots",
-                                       "ThresholdOfNumberOfContinuousNoBetterPropagation", "EnableBfs"};
-    for (const char* nm : head_names) {
-        const std::string v = get("BuildHead", nm, "");
-        if (!v.empty()) sptag_b200_set_param(head, nm, v.c_str());
-    }
+    load_ref_keys(head, ini, "BuildHead");
     s->vis = head->dim * (int)value_size(head->value_type) + 4;
     s->rearranged = ini_true(get("BuildSSDIndex", "EnablePostingListRearrange", "false")) ? 1 : 0;
     s->internal = atoi(get("BuildSSDIndex", "SearchInternalResultNum", "64").c_str());
@@ -3129,63 +3172,18 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
 
 int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, const char* value) {
     if (!s || !name || !value) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
-    const std::string n(name);
-    // the head's (SPANNIndex.cpp:901); the visited sets of the head iterators that SPANN iterators open
-    if (n == "MaxCheck" || n == "B200.IteratorVisitedSet" || n == "B200.IteratorVisitedHashEntries")
-        return sptag_b200_set_param(s->head, name, value);
-    char* end = nullptr;
+    const Param<Spann>* p = find_param(kSpannParams, name);
+    if (p && (p->flags & kHead)) return sptag_b200_set_param(s->head, name, value);
     std::lock_guard<std::mutex> lock(s->mu);
-    if (n == "IterativeSearchHeadBatch" || n == "B200.SpannDedupEntries") {
-        const long v = strtol(value, &end, 10);
-        if (end == value) return fail(SPTAG_B200_FAILED_PARSE_VALUE, "cannot parse '%s' for %s", value, name);
-        if (n == "IterativeSearchHeadBatch") {
-            if (v < 1 || v > 1024) return fail(SPTAG_B200_LACK_OF_INPUTS, "%s %ld outside [1, 1024]", name, v);
-            s->head_batch = (int)v;
-        } else {
-            if (v != 0 && (v < 64 || v > (1l << 30) || (v & (v - 1))))
-                return fail(SPTAG_B200_LACK_OF_INPUTS, "%s %ld is neither 0 nor a power of two in [64, 2^30]", name, v);
-            s->dedup_entries = (int)v;
-        }
-        return SPTAG_B200_SUCCESS;
-    }
-    if (n == "B200.LastIteratorRounds" || n == "B200.LastIteratorDedupBytes")
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "%s is read-only", name);
-    if (n == "MaxDistRatio") {
-        const float v = strtof(value, &end);
-        if (end == value) return fail(SPTAG_B200_FAILED_PARSE_VALUE, "cannot parse '%s' for %s", value, name);
-        s->max_dist_ratio = v;
-        return SPTAG_B200_SUCCESS;
-    }
-    const long v = strtol(value, &end, 10);
-    if (n == "SearchInternalResultNum" || n == "SearchPostingPageLimit") {
-        if (end == value) return fail(SPTAG_B200_FAILED_PARSE_VALUE, "cannot parse '%s' for %s", value, name);
-        if (v < 0 || v > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "%s %ld outside [0, 2048]", name, v);
-        (n == "SearchInternalResultNum" ? s->internal : s->page_limit) = (int)v;
-        spann_update_shape(s);
-        return SPTAG_B200_SUCCESS;
-    }
-    if (n == "PostingBytes") return fail(SPTAG_B200_LACK_OF_INPUTS, "PostingBytes is read-only");
-    return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
+    return set_param(s, p, name, value);
 }
 
 int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char* value_out, int32_t capacity) {
     if (!s || !name || !value_out || capacity <= 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
-    const std::string n(name);
-    if (n == "MaxCheck" || n == "B200.IteratorVisitedSet" || n == "B200.IteratorVisitedHashEntries")
-        return sptag_b200_get_param(s->head, name, value_out, capacity);
+    const Param<Spann>* p = find_param(kSpannParams, name);
+    if (p && (p->flags & kHead)) return sptag_b200_get_param(s->head, name, value_out, capacity);
     std::lock_guard<std::mutex> lock(s->mu);
-    if (n == "MaxDistRatio") snprintf(value_out, (size_t)capacity, "%f", s->max_dist_ratio);
-    else if (n == "IterativeSearchHeadBatch") snprintf(value_out, (size_t)capacity, "%d", s->head_batch);
-    else if (n == "B200.SpannDedupEntries") snprintf(value_out, (size_t)capacity, "%d", s->dedup_entries);
-    else if (n == "B200.LastIteratorRounds") snprintf(value_out, (size_t)capacity, "%ld", s->last_iter_rounds);
-    else if (n == "B200.LastIteratorDedupBytes") snprintf(value_out, (size_t)capacity, "%ld", s->last_iter_dedup_bytes);
-    else if (n == "SearchInternalResultNum") snprintf(value_out, (size_t)capacity, "%d", s->internal);
-    else if (n == "SearchPostingPageLimit") snprintf(value_out, (size_t)capacity, "%d", s->page_limit);
-    else if (n == "PostingBytes")
-        snprintf(value_out, (size_t)capacity, "%zu", s->d_translate.bytes + s->d_off.bytes + s->d_cnt.bytes + s->d_pages.bytes +
-                                                         s->d_ids.bytes + s->d_rows.bytes);
-    else return fail(SPTAG_B200_PARAM_NOT_FOUND, "unknown parameter %s", name);
-    return SPTAG_B200_SUCCESS;
+    return get_param(s, p, name, value_out, (size_t)capacity);
 }
 
 }  // extern "C"
