@@ -379,9 +379,15 @@ int sptag_b200_save(sptag_b200_handle h, const char* folder);
  * sptag_b200_load reads from [Index], as SPANN::Index::SetParameter does (:1033-1038), reads the translate map and every posting file (SSDIndex,
  * SSDIndex_1, ...) in the plain or the rearranged layout, and packs the lists into HBM.  Each list keeps its full element
  * count; SearchPostingPageLimit truncates at search time.  Section and parameter names are read case-insensitively, as
- * Helper::IniReader reads them.  LackOfInputs for EnableDataCompression, EnableDeltaEncoding and quantized SPANN.  Device
- * memory: the packed lists (rows at the head's row stride, one int32 id each), plus during the load a staging buffer of
- * at most 64 MB (or the largest list, if larger); MemoryOverFlow when that does not fit. */
+ * Helper::IniReader reads them.  LackOfInputs for EnableDataCompression and EnableDeltaEncoding.
+ * Quantized SPANN ([Base] QuantizerFilePath set, as the reference builds it from PQ/OPQ code rows): the head must be a
+ * quantized BKT index (UInt8 code rows and a quantizer), the folder's quantizer (the file its [Quantizer] section names)
+ * is installed on the head as SPANN::Index::SetQuantizer does (SPANNIndex.cpp:39-56), [BuildSSDIndex] EnableADC sets the
+ * head's EnableADC, ValueType must be UInt8 (what the reference writes) or the quantizer's reconstruct type, and the
+ * lists hold M-byte code rows (M + 4 bytes per element).  LackOfInputs when the head holds no quantizer (tested before
+ * the quantizer file is opened) and for Cosine with a quantizer (quantized search is L2 only, PQQuantizer.h:130-136).
+ * Device memory: the packed lists (rows at the head's row stride, one int32 id each), plus during the load a staging
+ * buffer of at most 64 MB (or the largest list, if larger); MemoryOverFlow when that does not fit. */
 typedef struct sptag_b200_spann* sptag_b200_spann_handle;
 int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_handle* out);
 void sptag_b200_spann_destroy(sptag_b200_spann_handle s);
@@ -391,7 +397,10 @@ void sptag_b200_spann_destroy(sptag_b200_spann_handle s);
  * postings are chosen from its results, the result array is reversed, every chosen list is scanned in order with the
  * deduper, the head's distance function and QueryResultSet::AddPoint, and SortResult orders the array
  * (QueryResultSet.h:77-112); the first K entries are returned.  Results equal the reference's bit for bit.
- * queries: HOST, num_queries x dim of the value type.  out_ids / out_dists: HOST [num_queries x k].  out_stats: HOST
+ * queries: HOST, num_queries x dim of the value type; on a quantized index raw vectors of the quantizer's reconstruct type
+ * and dimension, which the head search and the posting scan both score with the quantizer's SDC or (EnableADC) ADC
+ * distance, ExtraFullGraphSearcher<std::uint8_t> (ExtraFullGraphSearcher.h:120-130).
+ * out_ids / out_dists: HOST [num_queries x k].  out_stats: HOST
  * [num_queries x 3] int32 or NULL: postings scanned (m_diskIOCount), list elements read (m_totalListElementsCount),
  * distances computed.  k <= 2048.  Thread-safe; two callers overlap.  LackOfInputs when the page limit truncates lists
  * of the rearranged layout (the reference then reads ids from an offset computed with the truncated count,
@@ -401,7 +410,9 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
 
 /* Replaces: SPANN::Index<T>::SetParameter / GetParameter (SPANNIndex.cpp:1033-1073) for SearchInternalResultNum,
  * MaxDistRatio (a float), SearchPostingPageLimit (raised at search time to the pages of PostingVectorLimit vectors, as
- * ExtraFullGraphSearcher::LoadIndex does, :167), MaxCheck (the head's) and IterativeSearchHeadBatch ([BuildSSDIndex],
+ * ExtraFullGraphSearcher::LoadIndex does, :167), MaxCheck and EnableADC (the head's; on a quantized index EnableADC
+ * switches the head search and the posting scan together, as the shared quantizer does, VectorIndex.h:136-138) and
+ * IterativeSearchHeadBatch ([BuildSSDIndex],
  * default 32, in [1, 1024]; sampled when an iterator opens).  B200.IteratorVisitedSet and B200.IteratorVisitedHashEntries
  * are the head handle's (sptag_b200_set_param): they choose the visited sets of the head iterators SPANN iterators open.
  * B200.SpannDedupEntries: the first dedup table size of an iterator's queries, 0 (default: room for one head batch of
@@ -428,8 +439,9 @@ int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char
  *          sptag_b200_spann_search on the same handle may run between calls; it does not change their results.
  *   close: frees the iterators.
  * LackOfInputs: null arguments, batch outside [1, 1024], IterativeSearchHeadBatch outside [1, 1024] (open) or above
- * SearchInternalResultNum (next: the reference has only that many page buffers, IExtraSearcher.h:114-122), and a page
- * limit that truncates lists of the rearranged layout (as sptag_b200_spann_search). */
+ * SearchInternalResultNum (next: the reference has only that many page buffers, IExtraSearcher.h:114-122), a page
+ * limit that truncates lists of the rearranged layout (as sptag_b200_spann_search), and quantized SPANN handles (open:
+ * head iterators are not built for quantized indexes). */
 typedef struct sptag_b200_spann_iterator* sptag_b200_spann_iter;
 int sptag_b200_spann_iterator_open(sptag_b200_spann_handle s, const void* queries, int32_t num_queries,
                                    sptag_b200_spann_iter* out);

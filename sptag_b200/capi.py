@@ -480,7 +480,7 @@ class B200SpannIndex:
             pass
 
     def set_param(self, name, value):
-        """SearchInternalResultNum, MaxDistRatio, SearchPostingPageLimit, MaxCheck (the head's)."""
+        """SearchInternalResultNum, MaxDistRatio, SearchPostingPageLimit, MaxCheck and EnableADC (the head's)."""
         _check(lib().sptag_b200_spann_set_param(self._h, name.encode(), str(value).encode()))
 
     def get_param(self, name):
@@ -489,7 +489,8 @@ class B200SpannIndex:
         return buf.value.decode()
 
     def search(self, queries, k, want_stats=False):
-        """SPANN::Index::SearchIndex for a batch of HOST queries: ids [nq, k], dists [nq, k] (and stats [nq, 3])."""
+        """SPANN::Index::SearchIndex for a batch of HOST queries: ids [nq, k], dists [nq, k] (and stats [nq, 3]).
+        On a quantized index the queries are raw vectors of the quantizer's reconstruct type and dimension."""
         queries = np.ascontiguousarray(queries)
         nq = queries.shape[0]
         ids = np.empty((nq, k), np.int32)

@@ -1,9 +1,12 @@
-// spann_device.cuh -- pieces shared by the posting-side kernels: the SPANN posting scan (kern_spann.cu), the posting
-// step of SPANN iterators (kern_spann_iter.cu) and the multi-index scan's cross distances (kern_multi_scan.cu).
-// QueryResultSet's comparator and Heapify, the distance, LoadingHeadInfo's truncation, and the launchers' dispatch.
+// spann_device.cuh -- pieces shared by the posting-side kernels: the SPANN posting scans (kern_spann.cu on raw rows,
+// kern_spann_pq.cu on PQ code rows), the posting step of SPANN iterators (kern_spann_iter.cu) and the multi-index scan's
+// cross distances (kern_multi_scan.cu).  QueryResultSet's comparator and Heapify, the distance, LoadingHeadInfo's
+// truncation, the posting scan's body, and the launchers' dispatch.
 #pragma once
 #include "search_kernels.cuh"
+#include "spann_scan.h"
 
+#include <climits>
 #include <type_traits>
 
 namespace sptag_b200 {
@@ -87,6 +90,162 @@ template <typename Params>
 __device__ __forceinline__ int searched_count(const Params& p, int l) {
     const long long lim = (long long)min(p.pages[l], p.page_limit) << 12;
     return (int)min((long long)p.cnt[l], lim / p.vector_info_size);
+}
+
+// The SPANN posting scan (SPANN::Index<T>::SearchIndex after its head search, SPANNIndex.cpp:193-250, and
+// ExtraFullGraphSearcher<T>::SearchIndex, ExtraFullGraphSearcher.h:226-375), one warp per query:
+//   translate the head results and choose the postings (lane 0, in result order), Reverse(), then for every chosen list
+//   and element in order: the deduper, the distance and QueryResultSet::AddPoint, then SortResult (QueryResultSet.h:77-112).
+// AddPoint's Heapify stops at `next < maxidx`, so which entries survive depends on the insertion order: the heap is
+// replayed in element order by one lane.  The lanes only skip work: a candidate that does not beat the current root
+// cannot beat any later root (a replacement never raises the root), so each chunk tests its candidates against the
+// root, applies the first that beats it, and re-tests the rest against the new root.
+// Dist is the distance of one flavour (kern_spann.cu: raw rows, kern_spann_pq.cu: PQ code rows):
+//   dist.begin_query(p, q)           before the first list of query q (the warp is converged)
+//   dist.chunk(p, l, cl, cnt, cd)    cd[r] = distance of the query to element cl[r] of list l, for r < cnt (<= 32); the
+//                                    warp calls it together, cd is read after a __syncwarp
+// smem holds spann_scan_smem(p.w) bytes.  p is taken by value: with a reference the raw-row kernels' instructions
+// differed from those of the scan written out in the kernel, with a copy only the registers of two parameter loads do.
+template <typename Dist>
+__device__ __forceinline__ void spann_scan_body(const SpannScanParams p, unsigned char* smem, Dist& dist) {
+    const int lane = threadIdx.x;
+    float* rd = reinterpret_cast<float*>(smem);            // m_results dists [w]
+    int* rv = reinterpret_cast<int*>(rd + p.w);            // m_results vids [w]
+    int* posts = rv + p.w;                                 // m_postingIDs [w]
+    float* cd = reinterpret_cast<float*>(posts + p.w);     // chunk candidates [32]
+    int* cv = reinterpret_cast<int*>(cd + 32);
+    int* cl = cv + 32;                                     // candidate element index in its list
+    int* shared_int = cl + 32;                             // [0] postings chosen, [1] table entries in use
+    int* table = p.tables + (size_t)blockIdx.x * p.table_entries;
+    for (int q = blockIdx.x; q < p.nq; q += gridDim.x) {
+        const int* hid = p.head_ids + (size_t)q * p.w;
+        const float* hd = p.head_dists + (size_t)q * p.w;
+        for (int i = lane; i < p.w; i += 32) {
+            rv[i] = hid[i];
+            rd[i] = hd[i];
+        }
+        __syncwarp();
+        if (lane == 0) {
+            // SPANNIndex.cpp:213-234: limitDist = result[0].Dist * MaxDistRatio (float), then per result until VID -1
+            const float limit = __fmul_rn(rd[0], p.max_dist_ratio);
+            int np = 0;
+            long long total = 0;
+            for (int i = 0; i < p.w; ++i) {
+                const int pid = rv[i];
+                if (pid == -1) break;
+                const int t = p.translate[pid];
+                if (t == INT_MAX) {
+                    rv[i] = -1;
+                    rd[i] = SPTAG_B200_MAXDIST;
+                } else {
+                    rv[i] = t;
+                }
+                if (np >= p.internal || ((double)limit > 0.1 && rd[i] > limit)) continue;
+                const int tc = searched_count(p, pid);
+                if (tc == 0) continue;  // CheckValidPosting (:931-934)
+                posts[np++] = pid;
+                total += tc;
+            }
+            shared_int[0] = np;
+            // the deduper needs room for every element this query reads; the table keeps at most half its entries used
+            int entries = 64;
+            while (entries < p.table_entries && (long long)entries < 2 * total) entries <<= 1;
+            shared_int[1] = entries;
+        }
+        __syncwarp();
+        const int np = shared_int[0], entries = shared_int[1];
+        for (int i = lane; i < entries; i += 32) table[i] = 0;
+        for (int i = lane; i < p.w / 2; i += 32) {  // Reverse()
+            const int o = p.w - 1 - i;
+            const float td = rd[i];
+            const int tv = rv[i];
+            rd[i] = rd[o];
+            rv[i] = rv[o];
+            rd[o] = td;
+            rv[o] = tv;
+        }
+        __syncwarp();
+        dist.begin_query(p, q);
+        int elements = 0, ndist = 0;
+        for (int pi = 0; pi < np; ++pi) {
+            const int l = posts[pi];
+            const int tc = searched_count(p, l);
+            elements += tc;
+            for (int base = 0; base < tc; base += 32) {
+                const int i = base + lane;
+                const bool in = i < tc;
+                const int vid = in ? p.ids[p.off[l] + i] : 0;
+                // m_deduper.CheckAndSet(vid) in element order (WorkSpace.h:113-117): an id seen earlier is skipped.  Among
+                // equal ids of this chunk only the lowest lane may insert; -1 maps to the empty key and is never "seen".
+                const unsigned same = __match_any_sync(kFull, in ? vid : INT_MIN);
+                bool keep = in && (vid == -1 || (__ffs(same) - 1) == lane);
+                if (keep && vid != -1) {
+                    const unsigned key = (unsigned)vid + 1u;
+                    unsigned h = vhash_home(key, 32 - __ffs(entries) + 1) & (unsigned)(entries - 1);
+                    for (;;) {
+                        const int prev = atomicCAS(&table[h], 0, (int)key);
+                        if (prev == 0) break;
+                        if (prev == (int)key) {
+                            keep = false;
+                            break;
+                        }
+                        h = (h + 1) & (unsigned)(entries - 1);
+                    }
+                }
+                const unsigned km = __ballot_sync(kFull, keep);
+                const int cnt = __popc(km);
+                if (keep) {
+                    const int slot = __popc(km & ((1u << lane) - 1u));
+                    cv[slot] = vid;
+                    cl[slot] = i;
+                }
+                __syncwarp();
+                dist.chunk(p, l, cl, cnt, cd);
+                ndist += cnt;
+                __syncwarp();
+                // AddPoint in element order (QueryResultSet.h:77-87)
+                int from = 0;
+                for (;;) {
+                    const float root_d = rd[0];
+                    const int root_v = rv[0];
+                    const bool beats = lane >= from && lane < cnt && res_less(cd[lane], cv[lane], root_d, root_v);
+                    const unsigned bm = __ballot_sync(kFull, beats);
+                    if (bm == 0) break;
+                    const int first = __ffs(bm) - 1;
+                    if (lane == 0) {
+                        rd[0] = cd[first];
+                        rv[0] = cv[first];
+                        heapify(rd, rv, p.w);
+                    }
+                    __syncwarp();
+                    from = first + 1;
+                }
+                __syncwarp();
+            }
+        }
+        if (lane == 0) {  // SortResult (QueryResultSet.h:89-96)
+            for (int i = p.w - 1; i >= 0; --i) {
+                const float td = rd[0];
+                const int tv = rv[0];
+                rd[0] = rd[i];
+                rv[0] = rv[i];
+                rd[i] = td;
+                rv[i] = tv;
+                heapify(rd, rv, i);
+            }
+        }
+        __syncwarp();
+        for (int i = lane; i < p.k; i += 32) {
+            p.out_ids[(size_t)q * p.k + i] = rv[i];
+            p.out_dists[(size_t)q * p.k + i] = rd[i];
+        }
+        if (p.out_stats && lane == 0) {
+            p.out_stats[(size_t)q * 3 + 0] = np;
+            p.out_stats[(size_t)q * 3 + 1] = elements;
+            p.out_stats[(size_t)q * 3 + 2] = ndist;
+        }
+        __syncwarp();
+    }
 }
 
 }  // namespace

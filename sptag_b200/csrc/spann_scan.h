@@ -45,7 +45,25 @@ struct SpannScanParams {
 cudaError_t launch_spann_scan(const SpannScanParams& p, bool cosine, int elem, int grid, cudaStream_t stream);
 // Single-warp blocks of the scan kernel that fit on one SM with W results per query.
 int spann_scan_blocks_per_sm(bool cosine, int elem, int w);
-size_t spann_scan_smem(int w);
+// Its dynamic shared memory: W result dists, vids and posting ids, three 32-entry chunk arrays and two counters
+__host__ __device__ inline size_t spann_scan_smem(int w) { return (size_t)w * 12 + 3 * 32 * 4 + 16; }
+
+// The posting scan of a PQ/OPQ-quantized SPANN index (ExtraFullGraphSearcher<std::uint8_t>, SPANNIndex.cpp:93-99): the
+// rows are M code bytes and the distance is the quantizer's L2Distance to the quantized query (PQQuantizer.h:110-128).
+// Everything else is the scan above; of `s`, queries, dim and simd_width are not read.
+struct SpannPqScanParams {
+    SpannScanParams s;
+    int m, ks, dsub;
+    int adc;                      // 0: SDC, the query is M codes; 1: ADC, the query is the rotated float vector
+    const unsigned char* qcodes;  // SDC: [nq x m] the quantized queries
+    const float* sdc;             // SDC: [m x ks x ks] InitializeDistanceTables
+    const float* qrot;            // ADC: [nq x m*dsub] the (OPQ-rotated) float queries
+    const float* codebooks;       // ADC: [m x ks x dsub]
+    float* adc_tables;            // ADC: per block, the current query's m x ks table
+};
+cudaError_t launch_spann_pq_scan(const SpannPqScanParams& p, int grid, cudaStream_t stream);
+int spann_pq_scan_blocks_per_sm(int w, int m);
+size_t spann_pq_scan_smem(int w, int m);
 
 // What a SPANN iterator keeps per query between launches (SPANNResultIterator's ExtraWorkSpace and the call in progress)
 struct SpannIterState {

@@ -2766,11 +2766,13 @@ int32_t sptag_b200_num_deleted(sptag_b200_handle h) {
 // SPANN with its posting lists in HBM (SPANN::Index<T>, SPANNIndex.cpp; ExtraFullGraphSearcher.h).  The head is an
 // ordinary handle loaded by sptag_b200_load; the lists are packed into one id array and one array of rows padded to the
 // head's row stride, with one element offset per list.  The search runs the head search kernels at width W, then the
-// posting scan kernel (kern_spann.cu).
+// posting scan kernel (kern_spann.cu; kern_spann_pq.cu on a quantized index, whose head and lists hold M-byte code
+// rows: ExtraFullGraphSearcher<std::uint8_t>, SPANNIndex.cpp:93-99).
 // ---------------------------------------------------------------------------------------------------------------
 struct sptag_b200_spann {
     sptag_b200_index* head = nullptr;
-    int vis = 0;          // m_vectorInfoSize: dim * sizeof(T) + sizeof(int)
+    bool quantized = false;  // [Base] QuantizerFilePath: the head's quantizer scores the postings too
+    int vis = 0;          // m_vectorInfoSize: dim * sizeof(T) + sizeof(int) (quantized: M code bytes + sizeof(int))
     int rearranged = 0;   // EnablePostingListRearrange
     int num_lists = 0;
     std::vector<int> cnt, pages;  // per list: full element count, page count (host copies for the table size)
@@ -2791,6 +2793,7 @@ struct sptag_b200_spann {
     // so that two callers overlap; the head search kernels are ordered by the head handle (search_device_impl)
     struct StagingBuffers {
         DeviceBuffer d_q, d_qpad, d_hids, d_hdists, d_ids, d_dists, d_stats, d_tables;
+        DeviceBuffer d_codes, d_adc;  // quantized: the queries' codes (SDC) or rotated vectors (ADC); ADC tables per block
     };
     StagingPool<StagingBuffers> staging;
     std::mutex mu;  // the search parameters
@@ -2851,6 +2854,8 @@ const Param<Spann> kSpannParams[] = {
     {"MaxCheck", kHead},
     {"B200.IteratorVisitedSet", kHead},  // with the next: the visited sets of the head iterators SPANN iterators open
     {"B200.IteratorVisitedHashEntries", kHead},
+    // the one quantizer of the head and the postings (VectorIndex::SetQuantizerADC, VectorIndex.h:136-138)
+    {"EnableADC", kHead},
     {"SearchInternalResultNum", &Spann::internal, 0, 0, 2048,
      [](Spann* s, long v) { s->internal = (int)v; spann_update_shape(s); return SPTAG_B200_SUCCESS; }},
     {"SearchPostingPageLimit", &Spann::page_limit, 0, 0, 2048,
@@ -3054,8 +3059,9 @@ int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_h
     auto get = [&](const char* section, const char* name, const char* def) { return ini_get(ini, section, name, def); };
     if (get("Index", "IndexAlgoType", "SPANN") != "SPANN") return fail(SPTAG_B200_LACK_OF_INPUTS, "%s is not a SPANN index", folder);
     // Refusals: what the device does not hold or decode (SPANN/ParameterDefinitionList.h:34, :79-81)
-    if (!get("Base", "QuantizerFilePath", "").empty())
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "quantized SPANN indexes are not supported on the device");
+    const bool quantized = !get("Base", "QuantizerFilePath", "").empty();
+    if (quantized && get("Base", "DistCalcMethod", "Cosine") != "L2")  // PQQuantizer::CosineDistance is an error stub
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "quantized SPANN indexes are searched with L2 only");
     if (ini_true(get("BuildSSDIndex", "EnableDataCompression", "false")))
         return fail(SPTAG_B200_LACK_OF_INPUTS, "EnableDataCompression (zstd posting lists) is not supported on the device");
     if (ini_true(get("BuildSSDIndex", "EnableDeltaEncoding", "false")))
@@ -3069,7 +3075,32 @@ int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_h
     if (int rc = sptag_b200_load(head_dir.c_str(), device, 0, &head)) return rc;
     auto* s = new sptag_b200_spann();
     s->head = head;
-    if (head->value_type != value_type || head->q_type != 0) {
+    s->quantized = quantized;
+    if (quantized) {
+        // A quantized index's head is a BKT index over UInt8 code rows (SPANNIndex.cpp:850-855).  The reference loads the
+        // quantizer the folder's [Quantizer] section names and installs it on the head (VectorIndex.cpp:675-677,
+        // SPANNIndex.cpp:39-56); its ValueType is UInt8 (SPANNIndex.cpp:1013, the type of the code rows it was built on)
+        // or the quantizer's reconstruct type.  [BuildSSDIndex] EnableADC switches the one quantizer (SPANNIndex.cpp:73-76).
+        if (head->q_type == 0 || head->value_type != SPTAG_B200_VT_UINT8 || head->algo != SPTAG_B200_ALGO_BKT) {
+            sptag_b200_spann_destroy(s);
+            return fail(SPTAG_B200_LACK_OF_INPUTS, "QuantizerFilePath is set but the head index is not a quantized BKT index");
+        }
+        std::string qname = get("Base", "QuantizerFilePath", "");
+        qname = get("Quantizer", "QuantizerFilePath", qname.substr(qname.find_last_of("/\\") + 1).c_str());
+        std::vector<char> qb;
+        if (!read_file(dir + "/" + qname, qb)) {
+            sptag_b200_spann_destroy(s);
+            return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot read quantizer file %s", qname.c_str());
+        }
+        int rc = sptag_b200_set_quantizer(head, qb.data(), (int64_t)qb.size());
+        if (!rc && value_type != SPTAG_B200_VT_UINT8 && value_type != head->q_rtype)
+            rc = fail(SPTAG_B200_LACK_OF_INPUTS, "ValueType %s is neither UInt8 nor the quantizer's reconstruct type", vt.c_str());
+        if (!rc && ini_true(get("BuildSSDIndex", "EnableADC", "false"))) rc = sptag_b200_set_param(head, "EnableADC", "1");
+        if (rc) {
+            sptag_b200_spann_destroy(s);
+            return rc;
+        }
+    } else if (head->value_type != value_type || head->q_type != 0) {
         sptag_b200_spann_destroy(s);
         return fail(SPTAG_B200_LACK_OF_INPUTS, "head index value type %d does not match ValueType %s", head->value_type, vt.c_str());
     }
@@ -3109,9 +3140,9 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     DeviceGuard guard(h->device);
     cudaStream_t stream = st->stream;
     const size_t nq = (size_t)num_queries;
-    const size_t qrow = (size_t)h->dim * value_size(h->value_type);
+    const size_t qrow = query_bytes(h);  // quantized: raw vectors of the quantizer's reconstruct type
     const MetricElem me = metric_elem(h);
-    int per_sm = spann_scan_blocks_per_sm(me.cosine, me.elem, w);
+    int per_sm = s->quantized ? spann_pq_scan_blocks_per_sm(w, h->q_m) : spann_scan_blocks_per_sm(me.cosine, me.elem, w);
     if (per_sm < 1) return fail(SPTAG_B200_MEMORY_OVERFLOW, "the posting scan kernel does not fit on an SM at W = %d", w);
     // resident blocks, but no more dedup-table bytes than kTableBytes unless one block per SM needs more
     const long long kTableBytes = 256ll << 20;
@@ -3127,13 +3158,42 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
         if (int rc = st->d_stats.ensure(nq * 3 * 4)) return rc;
     if (int rc = st->d_tables.ensure((size_t)grid * entries * 4)) return rc;
     CUDA_OK(cudaMemcpyAsync(st->d_q.ptr, queries, nq * qrow, cudaMemcpyHostToDevice, stream));  // as the head search reads them
-    if (int rc = upload_query_rows(h, st->d_qpad.ptr, st->d_q.ptr, nq, stream)) return rc;
+    if (!s->quantized)
+        if (int rc = upload_query_rows(h, st->d_qpad.ptr, st->d_q.ptr, nq, stream)) return rc;
+    SpannPqScanParams pq;
+    memset(&pq, 0, sizeof(pq));
     {
         std::lock_guard<std::mutex> lock(h->mu);
         if (int rc = search_device_impl(h, st->d_q.ptr, num_queries, w, (int*)st->d_hids.ptr, (float*)st->d_hdists.ptr,
                                         nullptr, stream)) {
             cudaStreamSynchronize(stream);
             return rc;
+        }
+        if (s->quantized) {
+            // QueryResultSet::GetQuantizedTarget, as the head search quantized it (SDC: M codes; ADC: the rotated vector
+            // the scan builds the query's table from), under the same lock, so that both see one EnableADC
+            pq.m = h->q_m;
+            pq.ks = h->q_ks;
+            pq.dsub = h->q_dsub;
+            pq.adc = h->q_adc ? 1 : 0;
+            int rc = 0;
+            if (pq.adc) {
+                const size_t dimq = (size_t)h->q_m * h->q_dsub;
+                if (!(rc = st->d_codes.ensure(nq * dimq * 4)) && !(rc = st->d_adc.ensure((size_t)grid * h->q_m * h->q_ks * 4)))
+                    rc = quantize_device(h, st->d_q.ptr, num_queries, nullptr, stream, (float*)st->d_codes.ptr);
+                pq.qrot = (const float*)st->d_codes.ptr;
+                pq.codebooks = (const float*)h->d_codebooks.ptr;
+                pq.adc_tables = (float*)st->d_adc.ptr;
+            } else {
+                if (!(rc = st->d_codes.ensure(nq * h->q_m)))
+                    rc = quantize_device(h, st->d_q.ptr, num_queries, (unsigned char*)st->d_codes.ptr, stream);
+                pq.qcodes = (const unsigned char*)st->d_codes.ptr;
+                pq.sdc = (const float*)h->d_sdc.ptr;
+            }
+            if (rc) {
+                cudaStreamSynchronize(stream);
+                return rc;
+            }
         }
     }
     p.head_ids = (const int*)st->d_hids.ptr;
@@ -3157,7 +3217,8 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     p.out_ids = (int*)st->d_ids.ptr;
     p.out_dists = (float*)st->d_dists.ptr;
     p.out_stats = out_stats ? (int*)st->d_stats.ptr : nullptr;
-    cudaError_t e = launch_spann_scan(p, me.cosine, me.elem, grid, stream);
+    pq.s = p;
+    cudaError_t e = s->quantized ? launch_spann_pq_scan(pq, grid, stream) : launch_spann_scan(p, me.cosine, me.elem, grid, stream);
     g_launches++;
     if (e != cudaSuccess) {
         cudaStreamSynchronize(stream);
@@ -3221,6 +3282,8 @@ int sptag_b200_spann_iterator_open(sptag_b200_spann_handle s, const void* querie
     if (!s) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
     if (!out || !queries || num_queries <= 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
     *out = nullptr;
+    // the head iterators are not built for quantized indexes (sptag_b200_iterator_open)
+    if (s->quantized) return fail(SPTAG_B200_LACK_OF_INPUTS, "SPANN iterators on quantized indexes are not supported");
     int hb = 0, entries = 0, longest = 0;
     {
         std::lock_guard<std::mutex> lock(s->mu);
