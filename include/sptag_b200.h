@@ -392,6 +392,34 @@ typedef struct sptag_b200_spann* sptag_b200_spann_handle;
 int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_handle* out);
 void sptag_b200_spann_destroy(sptag_b200_spann_handle s);
 
+/* Replaces: the SSD stage of SPANN::Index<T>::BuildIndex with SelectHead and BuildHead off (SPANNIndex.cpp:889-951):
+ * ExtraFullGraphSearcher::BuildIndex (ExtraFullGraphSearcher.h:587-922) with VectorIndex::ApproximateRNG
+ * (VectorIndex.cpp:884-986, its CPU form), SortSelections (EdgeCompare, SearchResult.h:29-63), the posting cut (:722-760),
+ * SelectPostingOffset (:1206-1290) and OutputSSDIndexFile (:1292-1568), for a folder that already holds its head.
+ * folder: indexloader.ini (names read case-insensitively), the head index folder and the head-id file.  Keys read, with
+ * the reference's defaults (SPANN/ParameterDefinitionList.h): [Base] ValueType, DistCalcMethod, Dim, HeadIndexFolder,
+ * HeadVectorIDs, SSDIndex, SSDIndexFileNum, QuantizerFilePath; [BuildSSDIndex] ReplicaCount (<= 64), InternalResultNum
+ * (<= 2048), RNGFactor, PostingPageLimit, PostingVectorLimit, ExcludeHead, EnablePostingListRearrange, MaxCheck (the
+ * head's, as SPANNIndex.cpp:901 sets it), EnableDataCompression, EnableDeltaEncoding, OutputEmptyReplicaID.
+ * vectors: HOST, num x dim of ValueType, row i is vector id i.  Cosine rows are normalised first unless `normalized`.
+ * Every vector that is not a head (the head-id file's uint64s cast to SizeType) is searched on the head at K =
+ * InternalResultNum; the RNG test (RNGFactor * ComputeDistance(head_i, head_j) < dist_i rejects candidate i) keeps at
+ * most ReplicaCount heads; the lists are sorted by (distance, vector id), cut to PostingPageLimit pages, split over
+ * SSDIndexFileNum files (SSDIndex, SSDIndex_1, ...) and written byte for byte as the reference writes them, in the plain
+ * or the rearranged layout.  With ExcludeHead false the head-id file is first rewritten with MaxSize for every head, so
+ * every vector is searched.  indexloader.ini is not rewritten.  device: CUDA ordinal of the head.
+ * out_stats: HOST int64[8] or NULL: vectors searched, RNG rejections, edges before the cut, edges after it, then device
+ * microseconds of the head searches, the RNG selection and the sort, and host microseconds of writing the files.
+ * Device memory: the head index, the rows (num x dim, tightly packed), 24 bytes per edge (num x ReplicaCount edges, the
+ * radix sort's two key / vector-id buffers) plus the sort's scratch, one search batch of 65536 rows x InternalResultNum
+ * results, and a 64 MB window of the file being written.
+ * Codes: EmptyData (null input, num <= 0), DimensionSizeMismatch (dim differs from [Base] Dim or the head's),
+ * MemoryOverFlow (the rows and edges do not fit, or more than 2^31 - 1 edges), LackOfInputs (QuantizerFilePath,
+ * EnableDataCompression, EnableDeltaEncoding, OutputEmptyReplicaID, a head whose type or distance differs from the
+ * folder's, a NaN or infinity in a float row or a distance, parameters outside the ranges above). */
+int sptag_b200_spann_build(const char* folder, const void* vectors, int32_t num, int32_t dim, int32_t normalized,
+                           int32_t device, int64_t* out_stats);
+
 /* Replaces: SPANN::Index<T>::SearchIndex(QueryResult&) (SPANNIndex.cpp:193-250) with ExtraFullGraphSearcher::SearchIndex
  * (ExtraFullGraphSearcher.h:226-375) for a batch.  The head search runs at W = max(K, SearchInternalResultNum); the
  * postings are chosen from its results, the result array is reversed, every chosen list is scanned in order with the

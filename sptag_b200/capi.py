@@ -36,6 +36,7 @@ EXPORTS = [
     "sptag_b200_num_deleted", "sptag_b200_spann_load", "sptag_b200_spann_destroy", "sptag_b200_spann_search",
     "sptag_b200_spann_set_param", "sptag_b200_spann_get_param", "sptag_b200_spann_iterator_open",
     "sptag_b200_spann_iterator_next", "sptag_b200_spann_iterator_close", "sptag_b200_multi_scan",
+    "sptag_b200_spann_build",
 ]
 
 
@@ -115,6 +116,8 @@ def lib():
         L.sptag_b200_spann_load.argtypes = [C.c_char_p, C.c_int32, C.POINTER(C.c_void_p)]
         L.sptag_b200_spann_destroy.argtypes = [C.c_void_p]
         L.sptag_b200_spann_destroy.restype = None
+        L.sptag_b200_spann_build.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                             C.c_void_p]
         L.sptag_b200_spann_search.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.sptag_b200_spann_set_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p]
         L.sptag_b200_spann_get_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_int32]
@@ -467,6 +470,23 @@ class B200SpannIndex:
         h = C.c_void_p()
         _check(lib().sptag_b200_spann_load(os.fsencode(folder), device, C.byref(h)))
         return cls(h.value)
+
+    BUILD_STATS = ("searched", "rng_rejected", "edges_before_cut", "edges_after_cut", "search_us", "rng_us", "sort_us",
+                   "write_us")
+
+    @classmethod
+    def build(cls, folder, vectors, normalized=False, device=-1, stats=None):
+        """The SSD stage of SPANN::Index::BuildIndex (SelectHead and BuildHead off) on the device: writes the posting
+        files of `folder`, whose head is already built, from HOST vectors (row i is vector id i), and returns
+        load(folder, device).  If `stats` is a dict it receives BUILD_STATS."""
+        vectors = np.ascontiguousarray(vectors)
+        out = np.zeros(len(cls.BUILD_STATS), np.int64)
+        _check(lib().sptag_b200_spann_build(os.fsencode(folder), vectors.ctypes.data, vectors.shape[0],
+                                            vectors.shape[1] if vectors.ndim == 2 else 0, int(bool(normalized)), device,
+                                            out.ctypes.data))
+        if stats is not None:
+            stats.update(zip(cls.BUILD_STATS, out.tolist()))
+        return cls.load(folder, device)
 
     def close(self):
         if self._h:

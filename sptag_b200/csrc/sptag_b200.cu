@@ -9,12 +9,14 @@
 #include "aux_kernels.cuh"
 #include "kernel_select.h"
 #include "multi_scan.h"
+#include "spann_build.h"
 #include "spann_scan.h"
 
 #include <algorithm>
 #include <atomic>
 #include <cctype>
 #include <cfloat>
+#include <chrono>
 #include <climits>
 #include <cmath>
 #include <cstdarg>
@@ -24,7 +26,9 @@
 #include <cstring>
 #include <fstream>
 #include <map>
+#include <memory>
 #include <mutex>
+#include <set>
 #include <strings.h>
 #include <sys/stat.h>
 #include <sstream>
@@ -414,6 +418,8 @@ struct CallOpts {
     bool tombstones_live = false;
     int* d_overflows = nullptr;  // device int: receives how many queries the hashed set handed to the re-run (bitmap: 0)
     bool sketch = false;         // the handle's row sketches cover every row: take the sketch:: kernel (search_device_impl)
+    // device {count, query indices}: search only the listed queries of the batch (their results land at their own rows)
+    const unsigned int* d_query_list = nullptr;
 };
 
 // Slots of a result heap kept in HBM for k results: a power of two (the final sort is bitonic), at least 64
@@ -872,6 +878,7 @@ int search_device_impl(sptag_b200_index* h, const void* d_queries, int nq, int k
         p.id_offset = 0;
     }
     p.nq = nq;
+    p.rerun = opts.d_query_list;
     p.out_ids = d_ids;
     p.out_dists = d_dists;
     p.out_stats = d_stats;
@@ -3035,6 +3042,183 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
     spann_update_shape(s);
     return 0;
 }
+
+// ---------------------------------------------------------------------------------------------------------------
+// SPANN posting-list build (the SSD stage of SPANN::Index<T>::BuildIndexInternal, SPANNIndex.cpp:889-951, with
+// ExtraFullGraphSearcher::BuildIndex, ExtraFullGraphSearcher.h:587-922) from a head that is already built
+// ---------------------------------------------------------------------------------------------------------------
+
+// SelectPostingOffset (ExtraFullGraphSearcher.h:1206-1290): lists are placed greedily, each time the one with the largest
+// bytes % PageSize that still fits in the current page (the lower id among equals); a page that nothing fits is left
+// with its rest as padding.  page_num / page_off: where list i starts in the list area; order: the placement order.
+void select_posting_offset(const std::vector<long long>& bytes, std::vector<int>& page_num, std::vector<int>& page_off,
+                           std::vector<int>& order) {
+    page_num.assign(bytes.size(), 0);
+    page_off.assign(bytes.size(), 0);
+    order.clear();
+    std::set<std::pair<int, int>> rest;  // (-(bytes % 4096), id): largest rest first, then the lower id
+    for (size_t i = 0; i < bytes.size(); ++i)
+        if (bytes[i] != 0) rest.insert({-(int)(bytes[i] % 4096), (int)i});
+    int page = 0, off = 0;
+    while (!rest.empty()) {
+        const int room = 4096 - off;
+        auto it = rest.lower_bound({-room, -1});
+        if (it == rest.end() || (room != 4096 && it->first == 0)) {
+            ++page;
+            off = 0;
+            continue;
+        }
+        const int id = it->second;
+        page_num[id] = page;
+        page_off[id] = off;
+        order.push_back(id);
+        off -= it->first;
+        if (off == 4096) {
+            ++page;
+            off = 0;
+        }
+        page += (int)(bytes[id] / 4096);
+        rest.erase(it);
+    }
+}
+
+// One posting file (OutputSSDIndexFile, ExtraFullGraphSearcher.h:1292-1568) of lists [first, first + nl): the header on
+// the host, the list area from the device in windows of kWindow bytes, each copied into one of two pinned buffers so
+// that the fwrite of one window overlaps the image and copy of the next.
+struct SpannBuildFile {
+    const int* d_tonode;          // the sorted edges' tonode
+    const unsigned char* d_rows;  // the full rows, row_bytes apart
+    int row_bytes, rearranged, num_vectors, dim;
+    const std::vector<long long>* edge_off;  // per list: its first sorted edge
+    const std::vector<int>* count;           // per list: its elements after the cut
+};
+int write_posting_file(const SpannBuildFile& b, const std::string& path, int first, int nl, cudaStream_t stream) {
+    const long long vis = b.row_bytes + 4;
+    std::vector<long long> bytes((size_t)nl);
+    for (int i = 0; i < nl; ++i) bytes[i] = (long long)(*b.count)[first + i] * vis;
+    std::vector<int> page_num, page_off, order;
+    select_posting_offset(bytes, page_num, page_off, order);
+    // header: list count, vector count, dimension, the list area's first page; per list page, offset, count, pages
+    const size_t meta = 16 + 12 * (size_t)nl;
+    std::vector<unsigned char> hdr(round_up(meta, 4096), 0);
+    const int32_t h4[4] = {nl, b.num_vectors, b.dim, (int32_t)(hdr.size() / 4096)};
+    memcpy(hdr.data(), h4, 16);
+    for (int i = 0; i < nl; ++i) {
+        unsigned char* e = hdr.data() + 16 + 12 * (size_t)i;
+        const int32_t pn = bytes[i] ? page_num[i] : 0, ele = (*b.count)[first + i];
+        const uint16_t po = bytes[i] ? (uint16_t)page_off[i] : 0, pc = (uint16_t)((bytes[i] + 4095) / 4096);
+        memcpy(e, &pn, 4);
+        memcpy(e + 4, &po, 2);
+        memcpy(e + 6, &ele, 4);
+        memcpy(e + 10, &pc, 2);
+    }
+    // the lists in placement order (ascending start), and the list area's size: the last list's end, padded to a page
+    std::vector<long long> start, eoff;
+    std::vector<int> cnt;
+    for (int id : order) {
+        start.push_back((long long)page_num[id] * 4096 + page_off[id]);
+        eoff.push_back((*b.edge_off)[first + id]);
+        cnt.push_back((*b.count)[first + id]);
+    }
+    const long long area = order.empty() ? 0 : (long long)round_up((size_t)(start.back() + bytes[order.back()]), 4096);
+    FILE* f = std::fopen(path.c_str(), "wb");
+    if (!f) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot write %s", path.c_str());
+    std::unique_ptr<FILE, int (*)(FILE*)> closer(f, std::fclose);
+    if (std::fwrite(hdr.data(), 1, hdr.size(), f) != hdr.size()) return fail(SPTAG_B200_FAIL, "writing %s failed", path.c_str());
+    if (area == 0) return 0;
+    const long long kWindow = 64ll << 20;
+    const size_t win = (size_t)std::min(kWindow, area);
+    DeviceBuffer d_start, d_eoff, d_cnt, d_win;
+    if (int rc = d_start.ensure(start.size() * 8)) return rc;
+    if (int rc = d_eoff.ensure(eoff.size() * 8)) return rc;
+    if (int rc = d_cnt.ensure(cnt.size() * 4)) return rc;
+    if (int rc = d_win.ensure(win)) return rc;
+    CUDA_OK(cudaMemcpyAsync(d_start.ptr, start.data(), start.size() * 8, cudaMemcpyHostToDevice, stream));
+    CUDA_OK(cudaMemcpyAsync(d_eoff.ptr, eoff.data(), eoff.size() * 8, cudaMemcpyHostToDevice, stream));
+    CUDA_OK(cudaMemcpyAsync(d_cnt.ptr, cnt.data(), cnt.size() * 4, cudaMemcpyHostToDevice, stream));
+    struct Pinned {
+        void* p[2] = {nullptr, nullptr};
+        cudaEvent_t ev[2] = {nullptr, nullptr};
+        ~Pinned() {
+            for (int i = 0; i < 2; ++i) {
+                if (p[i]) cudaFreeHost(p[i]);
+                if (ev[i]) cudaEventDestroy(ev[i]);
+            }
+        }
+    } pin;
+    for (int i = 0; i < 2; ++i) {
+        if (cudaMallocHost(&pin.p[i], win) != cudaSuccess)
+            return fail(SPTAG_B200_MEMORY_OVERFLOW, "pinned window buffer (%zu bytes) failed", win);
+        CUDA_OK(cudaEventCreateWithFlags(&pin.ev[i], cudaEventDisableTiming));
+    }
+    SpannImageParams p;
+    memset(&p, 0, sizeof(p));
+    p.start = (const long long*)d_start.ptr;
+    p.edge_off = (const long long*)d_eoff.ptr;
+    p.count = (const int*)d_cnt.ptr;
+    p.tonode = b.d_tonode;
+    p.rows = b.d_rows;
+    p.row_bytes = b.row_bytes;
+    p.rearranged = b.rearranged;
+    p.out = (unsigned char*)d_win.ptr;
+    size_t lo = 0;  // the first list that ends after the window's start
+    long long pending = -1;  // the window waiting for its fwrite (its buffer: pending & 1)
+    auto flush = [&](long long w) -> int {
+        CUDA_OK(cudaEventSynchronize(pin.ev[w & 1]));
+        const size_t n = (size_t)std::min(kWindow, area - w * kWindow);
+        if (std::fwrite(pin.p[w & 1], 1, n, f) != n) return fail(SPTAG_B200_FAIL, "writing %s failed", path.c_str());
+        return 0;
+    };
+    for (long long w = 0; w * kWindow < area; ++w) {
+        p.win_begin = w * kWindow;
+        p.win_end = std::min(area, p.win_begin + kWindow);
+        while (lo < start.size() && start[lo] + (long long)cnt[lo] * vis <= p.win_begin) ++lo;
+        size_t hi = lo;
+        while (hi < start.size() && start[hi] < p.win_end) ++hi;
+        p.first_list = (int)lo;
+        p.num_lists = (int)(hi - lo);
+        CUDA_OK(cudaMemsetAsync(d_win.ptr, 0, (size_t)(p.win_end - p.win_begin), stream));
+        CUDA_OK(launch_spann_posting_image(p, stream));
+        g_launches++;
+        CUDA_OK(cudaMemcpyAsync(pin.p[w & 1], d_win.ptr, (size_t)(p.win_end - p.win_begin), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaEventRecord(pin.ev[w & 1], stream));
+        if (pending >= 0)
+            if (int rc = flush(pending)) return rc;
+        pending = w;
+    }
+    if (int rc = flush(pending)) return rc;
+    if (std::fflush(f) != 0) return fail(SPTAG_B200_FAIL, "writing %s failed", path.c_str());
+    return 0;
+}
+
+// Owns what one sptag_b200_spann_build call allocates on the device and its stream; frees them with the device current
+struct SpannBuildState {
+    sptag_b200_handle head = nullptr;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    DeviceBuffer d_rows, d_head, d_list, d_ids, d_dists, d_keys[2], d_tonode[2], d_size, d_counters, d_temp;
+    ~SpannBuildState() {
+        if (head) {
+            DeviceGuard guard(head->device);
+            if (stream) cudaStreamSynchronize(stream);
+            for (cudaEvent_t e : ev)
+                if (e) cudaEventDestroy(e);
+            if (stream) cudaStreamDestroy(stream);
+            for (DeviceBuffer* b : {&d_rows, &d_head, &d_list, &d_ids, &d_dists, &d_keys[0], &d_keys[1], &d_tonode[0],
+                                    &d_tonode[1], &d_size, &d_counters, &d_temp})
+                b->release();
+        }
+        sptag_b200_destroy(head);
+    }
+    // device milliseconds between ev[0] and ev[1], recorded around work on the stream
+    int elapsed(float& acc) {
+        CUDA_OK(cudaEventSynchronize(ev[1]));
+        float ms = 0;
+        CUDA_OK(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+        acc += ms;
+        return 0;
+    }
+};
 }  // namespace
 
 extern "C" {
@@ -3109,6 +3293,237 @@ int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_h
         return rc;
     }
     *out = s;
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_spann_build(const char* folder, const void* vectors, int32_t num, int32_t dim, int32_t normalized,
+                           int32_t device, int64_t* out_stats) {
+    if (!folder || !vectors || num <= 0) return fail(SPTAG_B200_EMPTY_DATA, "no vectors to build from");
+    const std::string dir(folder);
+    IniSections ini;
+    if (!read_ini(dir + "/indexloader.ini", ini)) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot open %s/indexloader.ini", folder);
+    auto get = [&](const char* section, const char* name, const char* def) { return ini_get(ini, section, name, def); };
+    // Refusals: what the device does not reproduce (SPANN/ParameterDefinitionList.h:34, :80-92)
+    if (!get("Base", "QuantizerFilePath", "").empty())
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "posting lists of quantized SPANN indexes are not built on the device");
+    for (const char* key : {"EnableDataCompression", "EnableDeltaEncoding", "OutputEmptyReplicaID"})
+        if (ini_true(get("BuildSSDIndex", key, "false")))
+            return fail(SPTAG_B200_LACK_OF_INPUTS, "%s is not supported by the device build", key);
+    const int value_type = enum_value(kValueTypes, get("Base", "ValueType", "Undefined"));
+    const int metric = enum_value(kDistCalcMethods, get("Base", "DistCalcMethod", "Undefined"));
+    if (value_type < 0 || metric < 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "unsupported ValueType or DistCalcMethod");
+    const int ini_dim = atoi(get("Base", "Dim", "-1").c_str());
+    if (dim <= 0 || (ini_dim != -1 && ini_dim != dim))
+        return fail(SPTAG_B200_DIMENSION_MISMATCH, "vectors have %d dimensions, the folder %d", dim, ini_dim);
+    const int replicas = atoi(get("BuildSSDIndex", "ReplicaCount", "8").c_str());
+    const int k = atoi(get("BuildSSDIndex", "InternalResultNum", "64").c_str());
+    const float rng_factor = strtof(get("BuildSSDIndex", "RNGFactor", "1.0").c_str(), nullptr);
+    int page_limit = atoi(get("BuildSSDIndex", "PostingPageLimit", "3").c_str());
+    const long long vector_limit = atoll(get("BuildSSDIndex", "PostingVectorLimit", "118").c_str());
+    const bool exclude_head = ini_true(get("BuildSSDIndex", "ExcludeHead", "true"));
+    const int rearranged = ini_true(get("BuildSSDIndex", "EnablePostingListRearrange", "false")) ? 1 : 0;
+    const std::string max_check = get("BuildSSDIndex", "MaxCheck", "4096");
+    const int file_num = atoi(get("Base", "SSDIndexFileNum", "1").c_str());
+    if (replicas < 1 || replicas > kSpannBuildMaxReplicas || k < 1 || k > 2048 || file_num < 1 || !std::isfinite(rng_factor))
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "ReplicaCount %d (1..%d), InternalResultNum %d (1..2048) or SSDIndexFileNum %d",
+                    replicas, kSpannBuildMaxReplicas, k, file_num);
+
+    SpannBuildState st;
+    const std::string head_dir = dir + "/" + get("Base", "HeadIndexFolder", "HeadIndex");
+    if (int rc = sptag_b200_load(head_dir.c_str(), device, 0, &st.head)) return rc;
+    sptag_b200_handle h = st.head;
+    if (h->q_type != 0 || h->value_type != value_type || h->metric != metric)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "the head index's value type or distance does not match the folder's");
+    if (h->dim != dim) return fail(SPTAG_B200_DIMENSION_MISMATCH, "vectors have %d dimensions, the head index %d", dim, h->dim);
+    // SPANNIndex.cpp:901: the head searches with [BuildSSDIndex] MaxCheck
+    if (int rc = sptag_b200_set_param(h, "MaxCheck", max_check.c_str())) return rc;
+    const int num_heads = h->n;
+    // SPANNIndex.cpp:914-925: with ExcludeHead false every head id becomes MaxSize, so that no vector is skipped
+    const std::string id_path = dir + "/" + get("Base", "HeadVectorIDs", "SPTAGHeadVectorIDs.bin");
+    if (!exclude_head) {
+        FILE* f = std::fopen(id_path.c_str(), "wb");
+        if (!f) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot write %s", id_path.c_str());
+        const std::vector<uint64_t> ids((size_t)num_heads, (uint64_t)INT_MAX);
+        const bool ok = std::fwrite(ids.data(), 8, ids.size(), f) == ids.size();
+        if (std::fclose(f) != 0 || !ok) return fail(SPTAG_B200_FAIL, "writing %s failed", id_path.c_str());
+    }
+    // the head-id set: every uint64 of the file cast to SizeType (ExtraFullGraphSearcher.h:604-616)
+    std::vector<unsigned char> is_head((size_t)num, 0);
+    {
+        std::vector<char> blob;
+        if (!read_file(id_path, blob)) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot read %s", id_path.c_str());
+        for (size_t i = 0; i + 8 <= blob.size(); i += 8) {
+            uint64_t v;
+            memcpy(&v, blob.data() + i, 8);
+            const int32_t id = (int32_t)(uint32_t)v;
+            if (id >= 0 && id < num) is_head[(size_t)id] = 1;
+        }
+    }
+    const size_t edges = (size_t)num * replicas;
+    if (edges > (size_t)INT_MAX) return fail(SPTAG_B200_MEMORY_OVERFLOW, "%zu edges: more than 2^31 - 1", edges);
+    const size_t row_bytes = (size_t)dim * value_size(value_type);
+    const int vis = (int)row_bytes + 4;
+
+    DeviceGuard guard(h->device);
+    CUDA_OK(cudaStreamCreateWithFlags(&st.stream, cudaStreamNonBlocking));
+    for (cudaEvent_t& e : st.ev) CUDA_OK(cudaEventCreate(&e));
+    cudaStream_t stream = st.stream;
+    const int kBatch = 1 << 16;
+    const int batch = std::min(num, kBatch);
+    if (int rc = st.d_rows.ensure((size_t)num * row_bytes)) return rc;
+    for (int i = 0; i < 2; ++i) {
+        if (int rc = st.d_keys[i].ensure(edges * 8)) return rc;
+        if (int rc = st.d_tonode[i].ensure(edges * 4)) return rc;
+    }
+    if (int rc = st.d_head.ensure((size_t)num)) return rc;
+    if (int rc = st.d_list.ensure(((size_t)batch + 1) * 4)) return rc;
+    if (int rc = st.d_ids.ensure((size_t)batch * k * 4)) return rc;
+    if (int rc = st.d_dists.ensure((size_t)batch * k * 4)) return rc;
+    if (int rc = st.d_size.ensure((size_t)num_heads * 4 + 4)) return rc;
+    if (int rc = st.d_counters.ensure(16)) return rc;  // rejections (uint64), the non-finite flag
+    unsigned long long* d_rejected = (unsigned long long*)st.d_counters.ptr;
+    int* d_bad = (int*)((unsigned char*)st.d_counters.ptr + 8);
+    CUDA_OK(cudaMemsetAsync(st.d_counters.ptr, 0, 16, stream));
+    CUDA_OK(cudaMemsetAsync(st.d_size.ptr, 0, (size_t)num_heads * 4, stream));
+    CUDA_OK(cudaMemcpyAsync(st.d_head.ptr, is_head.data(), (size_t)num, cudaMemcpyHostToDevice, stream));
+    ArraySource src;
+    src.ptr = vectors;
+    if (int rc = upload_rows(src, st.d_rows.ptr, (size_t)num, row_bytes, row_bytes, stream)) return rc;
+    unsigned char* rows = (unsigned char*)st.d_rows.ptr;
+    // sort and NaN have no order (std::sort under NaN is undefined): rows must be finite
+    if (value_type == SPTAG_B200_VT_FLOAT) {
+        CUDA_OK(launch_spann_nonfinite_check((const float*)rows, (size_t)num * dim, d_bad, stream));
+        int bad = 0;
+        CUDA_OK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        if (bad) return fail(SPTAG_B200_LACK_OF_INPUTS, "a row holds a NaN or an infinity");
+    }
+    // ExtraFullGraphSearcher.h:650: Cosine rows are normalised unless the caller says they are
+    if (metric == SPTAG_B200_METRIC_COSINE && !normalized) {
+        const int base = value_base(value_type);
+        with_elem(h, [&](auto el) {
+            normalize_rows_kernel<typename decltype(el)::type><<<(unsigned)((num + 127) / 128), 128, 0, stream>>>(
+                rows, row_bytes, 0, num, dim, base);
+        });
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+    }
+    // ApproximateRNG in batches of rows: the head search at K = InternalResultNum for the batch's non-head rows (queries
+    // read in place through the query list), then the RNG selection of the whole batch
+    const MetricElem me = metric_elem(h);
+    float ms_search = 0, ms_rng = 0, ms_sort = 0;
+    long long searched = 0;
+    std::vector<unsigned int> list((size_t)batch + 1);
+    SpannRngParams rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.res_ids = (const int*)st.d_ids.ptr;
+    rp.res_dists = (const float*)st.d_dists.ptr;
+    rp.k = k;
+    rp.head = (const unsigned char*)st.d_head.ptr;
+    rp.rows = (const unsigned char*)h->d_vectors.ptr;
+    rp.row_stride = h->row_stride;
+    rp.dim = dim;
+    rp.simd_width = h->simd_width;
+    rp.replicas = replicas;
+    rp.num_heads = num_heads;
+    rp.rng_factor = rng_factor;
+    rp.keys = (unsigned long long*)st.d_keys[0].ptr;
+    rp.tonode = (int*)st.d_tonode[0].ptr;
+    rp.list_size = (int*)st.d_size.ptr;
+    rp.rejected = d_rejected;
+    rp.bad = d_bad;
+    for (int b0 = 0; b0 < num; b0 += batch) {
+        const int nb = std::min(batch, num - b0);
+        unsigned int c = 0;
+        for (int i = 0; i < nb; ++i)
+            if (!is_head[(size_t)b0 + i]) list[1 + c++] = (unsigned int)i;
+        list[0] = c;
+        searched += c;
+        CUDA_OK(cudaMemcpyAsync(st.d_list.ptr, list.data(), ((size_t)c + 1) * 4, cudaMemcpyHostToDevice, stream));
+        CUDA_OK(cudaEventRecord(st.ev[0], stream));
+        if (c > 0) {
+            CallOpts opts;
+            opts.search_deleted = 0;
+            opts.d_query_list = (const unsigned int*)st.d_list.ptr;
+            std::lock_guard<std::mutex> lock(h->mu);
+            if (int rc = search_device_impl(h, rows + (size_t)b0 * row_bytes, nb, k, (int*)st.d_ids.ptr,
+                                            (float*)st.d_dists.ptr, nullptr, stream, false, opts))
+                return rc;
+        }
+        CUDA_OK(cudaEventRecord(st.ev[1], stream));
+        if (int rc = st.elapsed(ms_search)) return rc;  // also frees `list` for the next batch
+        rp.first = b0;
+        rp.num = nb;
+        CUDA_OK(cudaEventRecord(st.ev[0], stream));
+        CUDA_OK(launch_spann_rng_select(rp, me.cosine, me.elem, stream));
+        g_launches++;
+        CUDA_OK(cudaEventRecord(st.ev[1], stream));
+        if (int rc = st.elapsed(ms_rng)) return rc;
+    }
+    int bad = 0;
+    unsigned long long rejected = 0;
+    CUDA_OK(cudaMemcpy(&bad, d_bad, 4, cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(&rejected, d_rejected, 8, cudaMemcpyDeviceToHost));
+    if (bad) return fail(SPTAG_B200_LACK_OF_INPUTS, "a distance is not finite");
+    // SortSelections: node, then distance, then tonode; unfilled edges (node = num_heads) last
+    int end_bit = 32;
+    while (end_bit < 64 && ((unsigned long long)num_heads >> (end_bit - 32)) != 0) ++end_bit;
+    size_t temp_bytes = 0;
+    CUDA_OK(spann_sort_edges(nullptr, &temp_bytes, nullptr, nullptr, nullptr, nullptr, (int)edges, end_bit, stream));
+    if (int rc = st.d_temp.ensure(std::max<size_t>(temp_bytes, 1))) return rc;
+    CUDA_OK(cudaEventRecord(st.ev[0], stream));
+    CUDA_OK(spann_sort_edges(st.d_temp.ptr, &temp_bytes, (const unsigned long long*)st.d_keys[0].ptr,
+                             (unsigned long long*)st.d_keys[1].ptr, (const int*)st.d_tonode[0].ptr, (int*)st.d_tonode[1].ptr,
+                             (int)edges, end_bit, stream));
+    g_launches++;
+    CUDA_OK(cudaEventRecord(st.ev[1], stream));
+    if (int rc = st.elapsed(ms_sort)) return rc;
+    st.d_keys[0].release();
+    st.d_tonode[0].release();
+    st.d_temp.release();
+    // the posting cut (ExtraFullGraphSearcher.h:722-760): PostingPageLimit is first raised to the pages of
+    // PostingVectorLimit elements; each list keeps its first limit elements
+    std::vector<int> size((size_t)num_heads);
+    CUDA_OK(cudaMemcpy(size.data(), st.d_size.ptr, (size_t)num_heads * 4, cudaMemcpyDeviceToHost));
+    long long limit = INT_MAX;
+    if (page_limit > 0) {
+        page_limit = std::max(page_limit, (int)((vector_limit * vis + 4095) / 4096));
+        limit = (long long)page_limit * 4096 / vis;
+    }
+    std::vector<long long> edge_off((size_t)num_heads);
+    std::vector<int> count((size_t)num_heads);
+    long long before = 0, after = 0;
+    for (int l = 0; l < num_heads; ++l) {
+        edge_off[l] = before;
+        before += size[l];
+        count[l] = (int)std::min<long long>(size[l], limit);
+        after += count[l];
+    }
+    // SSDIndexFileNum files of ceil(lists / files) lists each (ExtraFullGraphSearcher.h:796-802)
+    const auto t0 = std::chrono::steady_clock::now();
+    const int per_file = (num_heads + file_num - 1) / file_num;
+    if ((long long)(file_num - 1) * per_file > num_heads)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "SSDIndexFileNum %d leaves a file without lists", file_num);
+    SpannBuildFile bf;
+    bf.d_tonode = (const int*)st.d_tonode[1].ptr;
+    bf.d_rows = rows;
+    bf.row_bytes = (int)row_bytes;
+    bf.rearranged = rearranged;
+    bf.num_vectors = num;
+    bf.dim = dim;
+    bf.edge_off = &edge_off;
+    bf.count = &count;
+    const std::string out = dir + "/" + get("Base", "SSDIndex", "SPTAGFullList.bin");
+    for (int i = 0; i < file_num; ++i) {
+        const int first = i * per_file, nl = std::min(num_heads, first + per_file) - first;
+        if (int rc = write_posting_file(bf, i == 0 ? out : out + "_" + std::to_string(i), first, nl, stream)) return rc;
+    }
+    const double ms_write = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (out_stats) {
+        const int64_t stats[8] = {searched, (int64_t)rejected, before, after, (int64_t)(ms_search * 1000.0),
+                                  (int64_t)(ms_rng * 1000.0), (int64_t)(ms_sort * 1000.0), (int64_t)(ms_write * 1000.0)};
+        memcpy(out_stats, stats, sizeof(stats));
+    }
     return SPTAG_B200_SUCCESS;
 }
 
