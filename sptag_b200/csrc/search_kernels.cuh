@@ -119,6 +119,7 @@ struct SearchParams {
     int slot_stagger;  // 1: odd ring slots start 64 B later (stride is a multiple of 128); 0: stride = 64 mod 128
     int h_ng, h_spt;
     int off_ng, off_spt, off_cand, off_bar, off_query;
+    int sketch_batch;  // sketch:: kernels: sketch rows per TMA batch through the row ring (fills the padding)
     // PQ / OPQ quantized index (PQQuantizer.h:110-128, ADC off): rows are M code bytes, the query is M code
     // bytes too and distance = sum_i sdc[(i*Ks + x_i)*Ks + y_i]
     // (float rows are never PQ codes, so the row sketches of the sketch:: kernels share the PQ tables' slots: a longer
@@ -1028,7 +1029,8 @@ struct WarpSearch {
     int checked, ndist, nexpand, ntree;
     int tree_checked, no_better;  // KDT: m_iNumberOfTreeCheckedLeaves, m_iNumOfContinuousNoBetterPropagation
     unsigned phase_bits;
-    // SKETCH: the query's sketch (its elements in shared memory) and the candidates whose rows were not fetched
+    // SKETCH: the query's sketch (its elements in shared memory, 16-byte aligned) and the candidates whose rows were not
+    // fetched
     const unsigned* tq;
     RowSketchTail tq_tail;
     int nskipped;
@@ -1692,12 +1694,16 @@ struct WarpSearch {
         return cnt;
     }
 
-    // compute_dists for candidates that only matter while their distance is <= mres.worst.  Pass 1 reads the candidates'
-    // sketches (lane l the 4-byte words l, l + 32, ... of a row: coalesced, 1/4 of the row's bytes) and lane r bounds
-    // candidate r's distance from below.  Pass 2 fetches the rows of the others only, compacted in neighbour order, and
-    // their distances are the reference's bits; a candidate that was proven above worst gets its bound as its distance.
-    // worst never increases, so the caller drops it wherever the true distance would have been dropped, and every
-    // counter advances as if the row had been read.  Until m_Results is full its worst is MaxDist and nothing is skipped.
+    // compute_dists for candidates that only matter while their distance is <= mres.worst.  Pass 1 stages the candidates'
+    // sketch rows, tail included, through the row ring, which the row pass cannot use before the bounds exist: one TMA
+    // batch of p.sketch_batch rows against bars[0] per round trip, while the rows of the later batches are prefetched
+    // into L2.  From shared memory the warp multiplies two rows at a time with the query's sketch (lane l the 16-byte
+    // vectors l, l + 32, ... of a row: conflict-free), and lane r bounds candidate r's distance from below as soon as its
+    // batch is done.  Pass 2 fetches the rows of the others only, compacted in neighbour order, and their distances are
+    // the reference's bits; a candidate that was proven above worst gets its bound as its distance.  worst never
+    // increases, so the caller drops it wherever the true distance would have been dropped, and every counter advances
+    // as if the row had been read.  Until m_Results is full its worst is MaxDist and nothing is skipped.
+    // (Two rows per group and the bound per batch keep every sketch kernel within its register cap without spills.)
     __device__ __forceinline__ void compute_dists_gated(int cnt) {
         if (cnt <= 0) return;
         __syncwarp();
@@ -1705,33 +1711,45 @@ struct WarpSearch {
         const float worst = mres.worst;
         float lb = -INFINITY;
         if (worst < SPTAG_B200_MAXDIST) {  // (warp-uniform)
-            const size_t stride = sketch_stride(p.dim);
-            const int nwords = ((DIM > 0) ? sketch_elems(DIM) : sketch_elems(p.dim)) >> 2;
-            RowSketchTail xt = {0.0f, INFINITY, 0.0f, 0.0f};
-            if (lane < cnt) xt = *reinterpret_cast<const RowSketchTail*>(p.sketch + (size_t)myid * stride + 4 * nwords);
-            int myI = 0;
-            for (int c0 = 0; c0 < cnt; c0 += 4) {
-                const unsigned* rw[4];
-                int acc[4];
+            const int stride = (int)sketch_stride(p.dim);
+            const int nvec = ((DIM > 0) ? sketch_elems(DIM) : sketch_elems(p.dim)) >> 4;  // 16-byte vectors per row
+            const int batch = p.sketch_batch;
+            if (lane >= batch && lane < cnt) tma_prefetch_l2(p.sketch + (size_t)myid * stride, (uint32_t)stride);
+            for (int b0 = 0; b0 < cnt; b0 += batch) {
+                const int nb = min(batch, cnt - b0);
+                const bool in_batch = lane >= b0 && lane < b0 + nb;
+                __syncwarp();
+                fence_proxy_async();  // earlier generic-proxy reads of the ring precede the async writes
+                if (lane == 0) mbar_arrive_expect_tx(&bars[0], (uint32_t)(nb * stride));
+                __syncwarp();
+                if (in_batch) tma_load_1d(ring + (lane - b0) * stride, p.sketch + (size_t)myid * stride, (uint32_t)stride, &bars[0]);
+                mbar_wait(&bars[0], phase_bits & 1u);
+                phase_bits ^= 1u;
+                int myI = 0;
+                for (int r0 = 0; r0 < nb; r0 += 2) {
+                    const unsigned* const rw[2] = {reinterpret_cast<const unsigned*>(ring + r0 * stride),
+                                                   reinterpret_cast<const unsigned*>(ring + min(r0 + 1, nb - 1) * stride)};
+                    int acc[2] = {0, 0};
+                    for (int v = lane; v < nvec; v += 32) {
+                        unsigned t[4];
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int id = __shfl_sync(kFull, myid, min(c0 + u, cnt - 1));
-                    rw[u] = reinterpret_cast<const unsigned*>(p.sketch + (size_t)id * stride);
-                    acc[u] = 0;
+                        for (int e = 0; e < 4; ++e) t[e] = tq[4 * v + e];
+#pragma unroll
+                        for (int u = 0; u < 2; ++u) {
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) acc[u] = __dp4a((int)rw[u][4 * v + e], (int)t[e], acc[u]);
+                        }
+                    }
+#pragma unroll
+                    for (int u = 0; u < 2; ++u) {
+                        const int I = __reduce_add_sync(kFull, acc[u]);
+                        if (r0 + u < nb && lane == b0 + r0 + u) myI = I;
+                    }
                 }
-#pragma unroll
-                for (int w = lane; w < nwords; w += 32) {
-                    const int t = (int)tq[w];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) acc[u] = __dp4a((int)__ldg(rw[u] + w), t, acc[u]);
-                }
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int I = __reduce_add_sync(kFull, acc[u]);
-                    if (lane == c0 + u) myI = I;
-                }
+                if (in_batch)
+                    lb = sketch_lower_bound<COSINE>(myI, tq_tail, *reinterpret_cast<const RowSketchTail*>(ring + (lane - b0) * stride + 16 * nvec),
+                                                    sketch_rel_margin(p.dim));
             }
-            if (lane < cnt) lb = sketch_lower_bound<COSINE>(myI, tq_tail, xt, sketch_rel_margin(p.dim));
         }
         const bool keep = (lane < cnt) && !(lb > worst);
         const unsigned keepmask = __ballot_sync(kFull, keep);

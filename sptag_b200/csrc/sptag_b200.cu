@@ -616,6 +616,9 @@ int lay_out(const sptag_b200_index* h, int nq, SearchLaunch& L) {
     }
     p.stage_rows = stage_rows;
     p.stages = stages;
+    // the sketch pass stages up to 32 sketch rows at a time through the ring (768-d, 2 x 2 rows of 3 136 B: 16 of 784 B)
+    if (sketch)
+        p.sketch_batch = (int)std::min<size_t>(32, (size_t)stage_rows * stages * p.slot_stride / sketch_stride(h->dim));
     const bool big_rows = h->row_stride >= 2048;
     int extra_ng = 0, extra_spt = 0;
     for (int pass = 0;; ++pass) {
@@ -654,8 +657,9 @@ int lay_out(const sptag_b200_index* h, int nq, SearchLaunch& L) {
         if (fit < 1) return fail(SPTAG_B200_MEMORY_OVERFLOW, "search kernel does not fit on an SM (smem %zu)", L.smem);
         int per_sm = h->queries_per_sm;
         if (per_sm <= 0) per_sm = fit;  // the kernel is latency-bound per warp: fill the SM
-        // 3 KB rows (HBM-bound): 11-12 slots, with larger queue heads, were the fastest of 10-18 on an H100 (DESIGN.md §5)
-        if (h->queries_per_sm <= 0 && big_rows) per_sm = std::min(per_sm, 12);
+        // 3 KB rows (HBM-bound): 11-12 slots, with larger queue heads, were the fastest of 10-18 on an H100 (DESIGN.md §5);
+        // with the sketch pass staged through the ring, 11 slots beat 12 by 2.5 % on C2 (DESIGN.md §5)
+        if (h->queries_per_sm <= 0 && big_rows) per_sm = std::min(per_sm, sketch ? 11 : 12);
         // 512 B rows: 14 slots leave 2 KB more shared memory per queue head than 16 and shorten the tail of a 10k-query batch
         if (h->queries_per_sm <= 0 && fast128) per_sm = std::min(per_sm, want_slots);
         L.per_sm = std::max(1, std::min(per_sm, fit));
