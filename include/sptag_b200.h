@@ -153,7 +153,10 @@ void sptag_b200_destroy(sptag_b200_handle h);
  * B200.LastIteratorSuspensions ("step,trees": how often the last iterator call suspended a query at the top of a step /
  * before a tree pop to grow its table), B200.LastIteratorGrowths (tables grown or restarted by that call),
  * B200.LastIteratorVisitedBytes (device bytes of that iterator's visited sets after the call), B200.LastRefineSearchUs
- * and B200.LastRefineRebuildUs (device microseconds of the last sptag_b200_refine_graph call's search and rebuild).
+ * and B200.LastRefineRebuildUs (device microseconds of the last sptag_b200_refine_graph call's search and rebuild),
+ * B200.LastSearchKernel (the demangled name of the last search, refine or iterator kernel instantiation this handle
+ * launched, e.g. "sptag_b200::search_kernel<128, false, 16, false, false, 0, 20>"; empty before the first; the value can
+ * be longer than 64 bytes).
  * Names are matched case-insensitively, as the reference's StrEqualIgnoreCase does.  Unknown names are ParamNotFound;
  * writing a read-only name is LackOfInputs. */
 int sptag_b200_set_param(sptag_b200_handle h, const char* name, const char* value);
@@ -520,6 +523,17 @@ int sptag_b200_last_kernel_ms(sptag_b200_handle h, float* ms_out);
 
 /* Number of kernels this library launched so far in this process (for bench.py's gpu_launches). */
 int64_t sptag_b200_launch_count(void);
+
+/* For tests: the kernel instantiation a launch would take, by the same selectors, as the name B200.LastSearchKernel
+ * reports after it.  Host-only: no CUDA call, no device needed.  value_type / metric / algo as sptag_b200_index_desc;
+ * simd_width, enable_bfs, row_sketch as B200.SimdWidth, EnableBfs, B200.RowSketch (non-zero: the sketches are in use,
+ * which only float BKT rows without breadth-first seeding take); quantized: PQ / OPQ codes (value_type UInt8, dim = M);
+ * mres_cap: max(MaxCheck / 16, K); slots: the query slots per SM the launch aims at (128-d float rows: B200.QueriesPerSM,
+ * or the automatic 14 to 20; otherwise 0); family: 0 search, 1 ResultIterator::Next, 2 the first
+ * SearchIndexIterativeFromNeareast call.  LackOfInputs: no kernel for that m_Results capacity. */
+int sptag_b200_debug_kernel_for(int32_t value_type, int32_t metric, int32_t algo, int32_t dim, int32_t simd_width,
+                                int32_t enable_bfs, int32_t row_sketch, int32_t quantized, int32_t mres_cap, int32_t slots,
+                                int32_t family, char* name_out, int32_t capacity);
 
 /* Index facts (VectorIndex::GetNumSamples / GetFeatureDim / ...). */
 int32_t sptag_b200_num_vectors(sptag_b200_handle h);

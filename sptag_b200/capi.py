@@ -36,7 +36,7 @@ EXPORTS = [
     "sptag_b200_num_deleted", "sptag_b200_spann_load", "sptag_b200_spann_destroy", "sptag_b200_spann_search",
     "sptag_b200_spann_set_param", "sptag_b200_spann_get_param", "sptag_b200_spann_iterator_open",
     "sptag_b200_spann_iterator_next", "sptag_b200_spann_iterator_close", "sptag_b200_multi_scan",
-    "sptag_b200_spann_build",
+    "sptag_b200_spann_build", "sptag_b200_debug_kernel_for",
 ]
 
 
@@ -113,6 +113,7 @@ def lib():
         L.sptag_b200_num_deleted.argtypes = [C.c_void_p]
         L.sptag_b200_last_kernel_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
         L.sptag_b200_launch_count.restype = C.c_int64
+        L.sptag_b200_debug_kernel_for.argtypes = [C.c_int32] * 11 + [C.c_char_p, C.c_int32]
         L.sptag_b200_spann_load.argtypes = [C.c_char_p, C.c_int32, C.POINTER(C.c_void_p)]
         L.sptag_b200_spann_destroy.argtypes = [C.c_void_p]
         L.sptag_b200_spann_destroy.restype = None
@@ -224,8 +225,8 @@ class B200Index:
         return out
 
     def get_param(self, name):
-        buf = C.create_string_buffer(64)
-        _check(lib().sptag_b200_get_param(self._h, name.encode(), buf, 64))
+        buf = C.create_string_buffer(256)
+        _check(lib().sptag_b200_get_param(self._h, name.encode(), buf, 256))
         return buf.value.decode()
 
     # -- search ---------------------------------------------------------------------------------
@@ -454,6 +455,22 @@ def merge_topk(device, d_ids_ptr, d_dists_ptr, num_lists, nq, k, d_out_ids_ptr, 
 
 def launch_count():
     return int(lib().sptag_b200_launch_count())
+
+
+FAMILY_SEARCH, FAMILY_ITERATE, FAMILY_NEAREST_FIRST = 0, 1, 2
+
+
+def debug_kernel_for(*, value_type, metric, algo, dim, simd_width=16, enable_bfs=0, row_sketch=0, quantized=False,
+                     mres_cap, slots=0, family=FAMILY_SEARCH):
+    """The kernel instantiation the selectors pick for these launch inputs (sptag_b200_debug_kernel_for), as the name
+    B200.LastSearchKernel reports; None when no kernel serves that m_Results capacity.  Needs no GPU."""
+    buf = C.create_string_buffer(256)
+    rc = lib().sptag_b200_debug_kernel_for(value_type, metric, algo, dim, simd_width, enable_bfs, row_sketch,
+                                           1 if quantized else 0, mres_cap, slots, family, buf, 256)
+    if rc == 0x13:  # LackOfInputs
+        return None
+    _check(rc)
+    return buf.value.decode()
 
 
 class B200SpannIndex:

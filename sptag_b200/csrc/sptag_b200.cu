@@ -24,6 +24,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <cxxabi.h>
+#include <dlfcn.h>
 #include <fstream>
 #include <map>
 #include <memory>
@@ -294,6 +296,8 @@ struct sptag_b200_index {
     int max_dup = -1;           // largest duplicate group of the tree (the tree never changes); -1 = not computed yet
     // the last iterator call: suspensions at a step top / before a SearchTrees pop, tables grown, visited-set bytes held
     long last_iter_susp_step = 0, last_iter_susp_trees = 0, last_iter_growths = 0, last_iter_visited_bytes = 0;
+    // host stub of the last search, sketch::, bfs:: or iterator kernel this handle launched (B200.LastSearchKernel)
+    const void* last_search_kernel = nullptr;
     // PQ / OPQ quantizer (null when q_type == 0)
     int q_type = 0, q_rtype = SPTAG_B200_VT_FLOAT, q_m = 0, q_ks = 0, q_dsub = 0;
     int q_adc = 0;  // IQuantizer::SetEnableADC (not serialized by the reference either)
@@ -403,6 +407,21 @@ Fn pick_iter_step_kernel(const sptag_b200_index* h, const SearchParams& p) {
     const bool cosine = h->metric != SPTAG_B200_METRIC_L2;
     return p.bfs ? pick_iter_kernel<Fn, true>(h->value_type, cosine, p.mres_cap)
                  : pick_iter_kernel<Fn, false>(h->value_type, cosine, p.mres_cap);
+}
+
+// The demangled name of a kernel's host launch stub without return type and parameter list, e.g.
+// "sptag_b200::search_kernel<128, false, 16, false, false, 0, 20>"; empty if the stub is not an exported symbol
+std::string kernel_name(const void* stub) {
+    Dl_info info;
+    if (!stub || !dladdr(stub, &info) || !info.dli_sname || info.dli_saddr != stub) return std::string();
+    int status = 0;
+    char* d = abi::__cxa_demangle(info.dli_sname, nullptr, nullptr, &status);
+    std::string s = (status == 0 && d) ? d : info.dli_sname;
+    free(d);
+    if (s.compare(0, 5, "void ") == 0) s.erase(0, 5);
+    const size_t args = s.find('(');  // template arguments are integers and booleans only
+    if (args != std::string::npos) s.erase(args);
+    return s;
 }
 
 // What one call may override (the reference passes these per call: p_searchDeleted of SearchIndex / GetIterator,
@@ -895,6 +914,7 @@ int search_device_impl(sptag_b200_index* h, const void* d_queries, int nq, int k
     L.kern<<<L.grid, 32, L.smem, stream>>>(p);
     g_launches++;
     CUDA_OK(cudaGetLastError());
+    h->last_search_kernel = (const void*)L.kern;
     if (p.vhash) {
         // the queries that filled their table run again on the bitmap: same stream, no host synchronisation; the count
         // is read on the device, so an empty list costs one near-empty launch
@@ -1504,6 +1524,7 @@ const Param<Index> kIndexParams[] = {
          }
          return put(o, n, "%ld", (long)c);
      }},
+    {"B200.LastSearchKernel", [](Index* h, char* o, size_t n) { return put(o, n, "%s", kernel_name(h->last_search_kernel).c_str()); }},
     {"B200.LastVisitedOverflows", [](Index* h, char* o, size_t n) { return put(o, n, "%d", h->last_visited_overflows.load()); }},
     {"B200.ScratchBytes", [](Index* h, char* o, size_t n) { return put(o, n, "%zu", h->scratch[0].bytes() + h->scratch[1].bytes()); }},
     {"B200.LastIteratorSuspensions",  // "step,trees" of the last iterator call
@@ -1531,6 +1552,39 @@ extern "C" {
 const char* sptag_b200_last_error(void) { return g_last_error.c_str(); }
 
 int64_t sptag_b200_launch_count(void) { return (int64_t)g_launches.load(); }
+
+int sptag_b200_debug_kernel_for(int32_t value_type, int32_t metric, int32_t algo, int32_t dim, int32_t simd_width,
+                                int32_t enable_bfs, int32_t row_sketch, int32_t quantized, int32_t mres_cap, int32_t slots,
+                                int32_t family, char* name_out, int32_t capacity) {
+    if (!name_out || capacity < 1) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    // the fields the selectors read, on a handle that owns nothing
+    sptag_b200_index h;
+    h.algo = algo;
+    h.metric = metric;
+    h.value_type = value_type;
+    h.q_type = quantized ? 1 : 0;
+    h.dim = dim;
+    h.simd_width = simd_width;
+    h.bfs = enable_bfs;
+    const void* stub = nullptr;
+    if (family == 0) {
+        stub = (const void*)pick_kernel(&h, mres_cap, slots, row_sketch != 0 && sketch_applies(&h));
+    } else if (family == 1 || family == 2) {
+        SearchParams p;
+        memset(&p, 0, sizeof(p));
+        p.bfs = bfs_seeding(&h) ? h.bfs : 0;
+        p.mres_cap = mres_cap;
+        stub = family == 1 ? (const void*)pick_iter_step_kernel<IterateKernelFn>(&h, p)
+                           : (const void*)pick_iter_step_kernel<NearestFirstKernelFn>(&h, p);
+    } else {
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "family %d is not 0 (search), 1 (iterator) or 2 (nearest first)", family);
+    }
+    if (!stub) return fail(SPTAG_B200_LACK_OF_INPUTS, "no kernel for m_Results capacity %d", mres_cap);
+    const std::string name = kernel_name(stub);
+    if (name.empty()) return fail(SPTAG_B200_FAIL, "the kernel's launch stub has no exported symbol");
+    snprintf(name_out, (size_t)capacity, "%s", name.c_str());
+    return SPTAG_B200_SUCCESS;
+}
 
 int sptag_b200_create(const sptag_b200_index_desc* desc, sptag_b200_handle* out) {
     if (!desc || !out) return fail(SPTAG_B200_LACK_OF_INPUTS, "null descriptor");
@@ -2162,6 +2216,7 @@ int next_step(sptag_b200_iterator* it, int batch, int32_t* out_ids, float* out_d
                                  CUDA_OK(cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                                  kern<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, (int*)it->d_counts.ptr,
                                                                   (unsigned char*)it->d_relaxed.ptr, iv);
+                                 h->last_search_kernel = (const void*)kern;
                                  return 0;
                              },
                              d_list);
@@ -2214,6 +2269,7 @@ int nearest_step(sptag_b200_iterator* it, int k, int32_t* out_ids, float* out_di
             if (first) {
                 CUDA_OK(cudaFuncSetAttribute((const void*)kfirst, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                 kfirst<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, iv);
+                h->last_search_kernel = (const void*)kfirst;
             } else {
                 // the caller Reset()s a QueryResult that keeps its k slots (SPANNIndex.cpp:284): no cap from the previous
                 // count (once per call: a resume launch must not undo what its completed queries set).  Every query's
@@ -2224,6 +2280,7 @@ int nearest_step(sptag_b200_iterator* it, int k, int32_t* out_ids, float* out_di
                 reset_slots = false;
                 CUDA_OK(cudaFuncSetAttribute((const void*)knext, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                 knext<<<grid, 32, smem, stream>>>(p, (int*)it->d_state.ptr, (int*)it->d_counts.ptr, (unsigned char*)it->d_relaxed.ptr, iv);
+                h->last_search_kernel = (const void*)knext;
             }
             return 0;
         },
