@@ -1,5 +1,6 @@
 // The posting step of SPANN iterators (SpannIterParams, spann_scan.h), in a translation unit of its own so that the
-// posting scan kernel's code does not change with it.
+// posting scan kernel's code does not change with it.  Its row distance and result set are the posting scan's
+// (spann_device.cuh).
 #include "spann_device.cuh"
 #include "spann_scan.h"
 
@@ -15,13 +16,13 @@ namespace {
 // chunk of up to 32 elements at (pi, offset) is looked up in the deduper without inserting; an element is new if it is not
 // in the set and is the first of its id in the chunk (-1 is always new: its key is the empty key).  The chunk is cut after
 // the (batch - count)-th new element, so that only the elements the reference's calls consume are inserted and offset
-// ends where the reference's does; the kept elements get their distances and AddPoint in element order.  A new element
+// ends where the reference's does; the kept elements get their distances and add_points in element order.  A new element
 // that is the last one of the last list is AddPoint'ed and inserted, but its call returns false: it is not counted and the
 // head is asked for its next batch.
 template <bool COSINE, int ELEM>
 __global__ void __launch_bounds__(32) spann_iter_step_kernel(const SpannIterParams p) {
     extern __shared__ __align__(16) unsigned char smem[];
-    const int lane = threadIdx.x, j = lane & 15, half = lane >> 4;
+    const int lane = threadIdx.x;
     float* rd = reinterpret_cast<float*>(smem);         // the call's QueryResult [batch]
     int* rv = reinterpret_cast<int*>(rd + p.cap);
     float* cd = reinterpret_cast<float*>(rv + p.cap);   // chunk candidates [32]
@@ -62,7 +63,7 @@ __global__ void __launch_bounds__(32) spann_iter_step_kernel(const SpannIterPara
         const int bits = ds.vbits;
         const unsigned mask = (1u << bits) - 1u;
         int fill = ds.vfill;
-        const unsigned char* qrow = p.queries + (size_t)q * p.row_stride;
+        RowDistance<COSINE, ELEM> dist{p.queries + (size_t)q * p.lists.row_stride, p.dim, p.simd_width, lane & 15, lane >> 4};
         int outcome = 0;  // 0: the call ends here, 1: the postings ran out (refill), 2: the table must grow (suspend)
         __syncwarp();
         while (!stop && count < batch) {
@@ -72,7 +73,7 @@ __global__ void __launch_bounds__(32) spann_iter_step_kernel(const SpannIterPara
                     for (int i = 0; i < p.hb; ++i) {
                         const int pid = p.head_ids[(size_t)q * p.hb + i];
                         if (pid == -1) break;
-                        if (searched_count(p, pid) > 0) posts[m++] = pid;  // CheckValidPosting
+                        if (searched_count(p.lists, pid) > 0) posts[m++] = pid;  // CheckValidPosting
                     }
                     shared_int[0] = m;
                 }
@@ -93,16 +94,16 @@ __global__ void __launch_bounds__(32) spann_iter_step_kernel(const SpannIterPara
                 break;
             }
             const int l = posts[pi];
-            const int tc = searched_count(p, l);
+            const int tc = searched_count(p.lists, l);
             if (offset >= tc) {  // the page limit was lowered since this list was started
                 ++pi;
                 offset = 0;
                 continue;
             }
-            const long long base = p.off[l];
+            const long long base = p.lists.off[l];
             const int i = offset + lane;
             const bool in = i < tc;
-            const int vid = in ? p.ids[base + i] : 0;
+            const int vid = in ? p.lists.ids[base + i] : 0;
             bool seen = false;
             if (in && vid != -1) {  // the deduper's lookup, without the insert (L2: the inserts are atomics)
                 const unsigned key = (unsigned)vid + 1u;
@@ -136,31 +137,9 @@ __global__ void __launch_bounds__(32) spann_iter_step_kernel(const SpannIterPara
                 cl[slot] = i;
             }
             __syncwarp();
-            for (int r0 = 0; r0 < cnt; r0 += 2) {
-                const int r = min(r0 + half, cnt - 1);
-                const unsigned char* row = p.rows + (size_t)(base + cl[r]) * p.row_stride;
-                const float d = spann_distance<COSINE, ELEM>(row, qrow, p.dim, j, p.simd_width);
-                if (j == 0 && r0 + half < cnt) cd[r] = d;
-            }
+            dist.chunk(p.lists, base, cl, cnt, cd);
             __syncwarp();
-            // AddPoint in element order (QueryResultSet.h:77-87)
-            int from = 0;
-            for (;;) {
-                const float root_d = rd[0];
-                const int root_v = rv[0];
-                const bool beats = lane >= from && lane < cnt && res_less(cd[lane], cv[lane], root_d, root_v);
-                const unsigned bm = __ballot_sync(kFull, beats);
-                if (bm == 0) break;
-                const int first = __ffs(bm) - 1;
-                if (lane == 0) {
-                    rd[0] = cd[first];
-                    rv[0] = cv[first];
-                    heapify(rd, rv, batch);
-                }
-                __syncwarp();
-                from = first + 1;
-            }
-            __syncwarp();
+            add_points(rd, rv, batch, cd, cv, cnt);
             offset += end;
             const bool last_of_last = pi == np - 1 && offset == tc && ((km >> (end - 1)) & 1u);
             if (offset == tc) {
@@ -170,18 +149,7 @@ __global__ void __launch_bounds__(32) spann_iter_step_kernel(const SpannIterPara
             count += cnt - (last_of_last ? 1 : 0);
         }
         if (outcome == 0) {
-            if (lane == 0) {  // SortResult (QueryResultSet.h:89-96)
-                for (int i = batch - 1; i >= 0; --i) {
-                    const float td = rd[0];
-                    const int tv = rv[0];
-                    rd[0] = rd[i];
-                    rv[0] = rv[i];
-                    rd[i] = td;
-                    rv[i] = tv;
-                    heapify(rd, rv, i);
-                }
-            }
-            __syncwarp();
+            sort_result(rd, rv, batch);
             for (int i = lane; i < p.batch; i += 32) {  // SetResultNum(resultCount)
                 p.out_ids[(size_t)q * p.batch + i] = i < count ? rv[i] : -1;
                 p.out_dists[(size_t)q * p.batch + i] = i < count ? rd[i] : SPTAG_B200_MAXDIST;
@@ -228,8 +196,7 @@ int spann_iter_step_blocks_per_sm(bool cosine, int elem, int cap) {
 
 cudaError_t launch_spann_iter_step(const SpannIterParams& p, bool cosine, int elem, int grid, cudaStream_t stream) {
     return with_cosine_elem(cosine, elem, [&](auto cos, auto el) {
-        spann_iter_step_kernel<cos, el><<<grid, 32, spann_iter_step_smem(p.cap), stream>>>(p);
-        return cudaGetLastError();
+        return launch_warp_blocks(spann_iter_step_kernel<cos, el>, p, grid, spann_iter_step_smem(p.cap), stream);
     });
 }
 

@@ -37,9 +37,9 @@ struct PqDistance {
         __syncwarp();
     }
 
-    __device__ __forceinline__ void chunk(const SpannScanParams& p, int l, const int* cl, int cnt, float* cd) {
+    __device__ __forceinline__ void chunk(const PostingLists pl, long long base, const int* cl, int cnt, float* cd) {
         if (lane >= cnt) return;
-        const unsigned char* row = p.rows + (size_t)(p.off[l] + cl[lane]) * p.row_stride;  // 16-byte aligned
+        const unsigned char* row = pl.rows + (size_t)(base + cl[lane]) * pl.row_stride;  // 16-byte aligned
         float acc = 0.0f;
         const int m4 = pp.m & ~3;
         int i = 0;
@@ -71,14 +71,7 @@ int spann_pq_scan_blocks_per_sm(int w, int m) {
 }
 
 cudaError_t launch_spann_pq_scan(const SpannPqScanParams& p, int grid, cudaStream_t stream) {
-    const size_t smem = spann_pq_scan_smem(p.s.w, p.m);
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute((const void*)spann_pq_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)smem);
-        if (e != cudaSuccess) return e;
-    }
-    spann_pq_scan_kernel<<<grid, 32, smem, stream>>>(p);
-    return cudaGetLastError();
+    return launch_warp_blocks(spann_pq_scan_kernel, p, grid, spann_pq_scan_smem(p.s.w, p.m), stream);
 }
 
 }  // namespace sptag_b200

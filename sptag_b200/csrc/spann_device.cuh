@@ -1,7 +1,8 @@
 // spann_device.cuh -- pieces shared by the posting-side kernels: the SPANN posting scans (kern_spann.cu on raw rows,
 // kern_spann_pq.cu on PQ code rows), the posting step of SPANN iterators (kern_spann_iter.cu) and the multi-index scan's
-// cross distances (kern_multi_scan.cu).  QueryResultSet's comparator and Heapify, the distance, LoadingHeadInfo's
-// truncation, the posting scan's body, and the launchers' dispatch.
+// cross distances (kern_multi_scan.cu).  QueryResultSet's comparator, Heapify, AddPoint of a chunk and SortResult, the
+// distance and the row distance of a chunk, LoadingHeadInfo's truncation, the posting scan's body, and the launchers'
+// dispatch, occupancy query and launch.
 #pragma once
 #include "search_kernels.cuh"
 #include "spann_scan.h"
@@ -35,6 +36,17 @@ inline int warp_blocks_per_sm(const void* k, size_t smem) {
         return 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, k, 32, smem) != cudaSuccess) return 0;
     return fit;
+}
+
+// Launches kernel k on `grid` blocks of one warp with smem bytes of dynamic shared memory; returns the launch error
+template <typename P>
+cudaError_t launch_warp_blocks(void (*k)(P), const P& p, int grid, size_t smem, cudaStream_t stream) {
+    if (smem > 48 * 1024) {
+        const cudaError_t e = cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+    }
+    k<<<grid, 32, smem, stream>>>(p);
+    return cudaGetLastError();
 }
 
 // BasicResult operator< (QueryResultSet.h:17-20)
@@ -71,6 +83,50 @@ __device__ void heapify(float* d, int* v, int count) {
     }
 }
 
+// QueryResultSet::AddPoint (QueryResultSet.h:77-87) of a chunk's cnt (<= 32) candidates (cd, cv), in element order, into
+// the size-entry heap (rd, rv).  AddPoint's Heapify stops at `next < maxidx`, so which entries survive depends on the
+// insertion order: the heap is replayed in element order by one lane.  The lanes only skip work: a candidate that does
+// not beat the current root cannot beat any later root (a replacement never raises the root), so the chunk's candidates
+// are tested against the root, the first that beats it is applied, and the rest are re-tested against the new root.  The
+// warp calls it together after a __syncwarp.
+__device__ __forceinline__ void add_points(float* rd, int* rv, int size, const float* cd, const int* cv, int cnt) {
+    const int lane = threadIdx.x;
+    int from = 0;
+    for (;;) {
+        const float root_d = rd[0];
+        const int root_v = rv[0];
+        const bool beats = lane >= from && lane < cnt && res_less(cd[lane], cv[lane], root_d, root_v);
+        const unsigned bm = __ballot_sync(kFull, beats);
+        if (bm == 0) break;
+        const int first = __ffs(bm) - 1;
+        if (lane == 0) {
+            rd[0] = cd[first];
+            rv[0] = cv[first];
+            heapify(rd, rv, size);
+        }
+        __syncwarp();
+        from = first + 1;
+    }
+    __syncwarp();
+}
+
+// QueryResultSet::SortResult (QueryResultSet.h:89-96) of the size-entry heap (rd, rv), by lane 0; the warp calls it
+// together
+__device__ __forceinline__ void sort_result(float* rd, int* rv, int size) {
+    if (threadIdx.x == 0) {
+        for (int i = size - 1; i >= 0; --i) {
+            const float td = rd[0];
+            const int tv = rv[0];
+            rd[0] = rd[i];
+            rv[0] = rv[i];
+            rd[i] = td;
+            rv[i] = tv;
+            heapify(rd, rv, i);
+        }
+    }
+    __syncwarp();
+}
+
 // ComputeDistance(query, row) by one half-warp with the trees of the search kernels (both are symmetric bit for bit)
 template <bool COSINE, int ELEM>
 __device__ __forceinline__ float spann_distance(const unsigned char* row, const unsigned char* q, int dim, int j,
@@ -85,27 +141,46 @@ __device__ __forceinline__ float spann_distance(const unsigned char* row, const 
     return half_warp_distance_elem_w<COSINE, ELEM>(row, q, dim, j, simd_width);
 }
 
-// LoadingHeadInfo's truncation (ExtraFullGraphSearcher.h:1093-1097)
-template <typename Params>
-__device__ __forceinline__ int searched_count(const Params& p, int l) {
-    const long long lim = (long long)min(p.pages[l], p.page_limit) << 12;
-    return (int)min((long long)p.cnt[l], lim / p.vector_info_size);
+// Elements of list l that a search reads (posting_searched)
+__device__ __forceinline__ int searched_count(const PostingLists pl, int l) {
+    return posting_searched(pl.cnt[l], pl.pages[l], pl.page_limit, pl.vector_info_size);
 }
+
+// The distances of a chunk to the query row qrow on raw rows: a half-warp per row, two rows at a time, with the head
+// index's DistanceUtils tree.  chunk(pl, base, cl, cnt, cd): cd[r] = the distance to element cl[r] of the list whose first
+// element is base (its off[l]), for r < cnt.
+template <bool COSINE, int ELEM>
+struct RowDistance {
+    const unsigned char* qrow;
+    int dim, simd_width;
+    int j, half;  // the lane's place in its half-warp, and which half-warp
+
+    __device__ __forceinline__ void begin_query(const SpannScanParams& p, int q) {
+        qrow = p.queries + (size_t)q * p.lists.row_stride;
+    }
+
+    __device__ __forceinline__ void chunk(const PostingLists pl, long long base, const int* cl, int cnt, float* cd) {
+        for (int r0 = 0; r0 < cnt; r0 += 2) {
+            const int r = min(r0 + half, cnt - 1);
+            const unsigned char* row = pl.rows + (size_t)(base + cl[r]) * pl.row_stride;
+            const float d = spann_distance<COSINE, ELEM>(row, qrow, dim, j, simd_width);
+            if (j == 0 && r0 + half < cnt) cd[r] = d;
+        }
+    }
+};
 
 // The SPANN posting scan (SPANN::Index<T>::SearchIndex after its head search, SPANNIndex.cpp:193-250, and
 // ExtraFullGraphSearcher<T>::SearchIndex, ExtraFullGraphSearcher.h:226-375), one warp per query:
 //   translate the head results and choose the postings (lane 0, in result order), Reverse(), then for every chosen list
-//   and element in order: the deduper, the distance and QueryResultSet::AddPoint, then SortResult (QueryResultSet.h:77-112).
-// AddPoint's Heapify stops at `next < maxidx`, so which entries survive depends on the insertion order: the heap is
-// replayed in element order by one lane.  The lanes only skip work: a candidate that does not beat the current root
-// cannot beat any later root (a replacement never raises the root), so each chunk tests its candidates against the
-// root, applies the first that beats it, and re-tests the rest against the new root.
-// Dist is the distance of one flavour (kern_spann.cu: raw rows, kern_spann_pq.cu: PQ code rows):
-//   dist.begin_query(p, q)           before the first list of query q (the warp is converged)
-//   dist.chunk(p, l, cl, cnt, cd)    cd[r] = distance of the query to element cl[r] of list l, for r < cnt (<= 32); the
-//                                    warp calls it together, cd is read after a __syncwarp
-// smem holds spann_scan_smem(p.w) bytes.  p is taken by value: with a reference the raw-row kernels' instructions
-// differed from those of the scan written out in the kernel, with a copy only the registers of two parameter loads do.
+//   and element in order: the deduper, the distance and add_points, then sort_result.
+// Dist is the distance of one flavour (kern_spann.cu: RowDistance on raw rows, kern_spann_pq.cu: PQ code rows):
+//   dist.begin_query(p, q)                    before the first list of query q (the warp is converged)
+//   dist.chunk(p.lists, first, cl, cnt, cd)   cd[r] = distance of the query to element cl[r] of the list whose first
+//                                             element is first, for r < cnt (<= 32); the warp calls it together, cd is
+//                                             read after a __syncwarp
+// smem holds spann_scan_smem(p.w) bytes.  p is taken by value, and so are the posting-list views of the helpers: with a
+// reference the raw-row kernels' instructions differed from those of the scan written out in the kernel, with a copy only
+// the registers of two parameter loads do.
 template <typename Dist>
 __device__ __forceinline__ void spann_scan_body(const SpannScanParams p, unsigned char* smem, Dist& dist) {
     const int lane = threadIdx.x;
@@ -141,7 +216,7 @@ __device__ __forceinline__ void spann_scan_body(const SpannScanParams p, unsigne
                     rv[i] = t;
                 }
                 if (np >= p.internal || ((double)limit > 0.1 && rd[i] > limit)) continue;
-                const int tc = searched_count(p, pid);
+                const int tc = searched_count(p.lists, pid);
                 if (tc == 0) continue;  // CheckValidPosting (:931-934)
                 posts[np++] = pid;
                 total += tc;
@@ -169,12 +244,13 @@ __device__ __forceinline__ void spann_scan_body(const SpannScanParams p, unsigne
         int elements = 0, ndist = 0;
         for (int pi = 0; pi < np; ++pi) {
             const int l = posts[pi];
-            const int tc = searched_count(p, l);
+            const int tc = searched_count(p.lists, l);
+            const long long first = p.lists.off[l];
             elements += tc;
             for (int base = 0; base < tc; base += 32) {
                 const int i = base + lane;
                 const bool in = i < tc;
-                const int vid = in ? p.ids[p.off[l] + i] : 0;
+                const int vid = in ? p.lists.ids[first + i] : 0;
                 // m_deduper.CheckAndSet(vid) in element order (WorkSpace.h:113-117): an id seen earlier is skipped.  Among
                 // equal ids of this chunk only the lowest lane may insert; -1 maps to the empty key and is never "seen".
                 const unsigned same = __match_any_sync(kFull, in ? vid : INT_MIN);
@@ -200,41 +276,13 @@ __device__ __forceinline__ void spann_scan_body(const SpannScanParams p, unsigne
                     cl[slot] = i;
                 }
                 __syncwarp();
-                dist.chunk(p, l, cl, cnt, cd);
+                dist.chunk(p.lists, first, cl, cnt, cd);
                 ndist += cnt;
                 __syncwarp();
-                // AddPoint in element order (QueryResultSet.h:77-87)
-                int from = 0;
-                for (;;) {
-                    const float root_d = rd[0];
-                    const int root_v = rv[0];
-                    const bool beats = lane >= from && lane < cnt && res_less(cd[lane], cv[lane], root_d, root_v);
-                    const unsigned bm = __ballot_sync(kFull, beats);
-                    if (bm == 0) break;
-                    const int first = __ffs(bm) - 1;
-                    if (lane == 0) {
-                        rd[0] = cd[first];
-                        rv[0] = cv[first];
-                        heapify(rd, rv, p.w);
-                    }
-                    __syncwarp();
-                    from = first + 1;
-                }
-                __syncwarp();
+                add_points(rd, rv, p.w, cd, cv, cnt);
             }
         }
-        if (lane == 0) {  // SortResult (QueryResultSet.h:89-96)
-            for (int i = p.w - 1; i >= 0; --i) {
-                const float td = rd[0];
-                const int tv = rv[0];
-                rd[0] = rd[i];
-                rv[0] = rv[i];
-                rd[i] = td;
-                rv[i] = tv;
-                heapify(rd, rv, i);
-            }
-        }
-        __syncwarp();
+        sort_result(rd, rv, p.w);
         for (int i = lane; i < p.k; i += 32) {
             p.out_ids[(size_t)q * p.k + i] = rv[i];
             p.out_dists[(size_t)q * p.k + i] = rd[i];

@@ -1,5 +1,6 @@
-// spann_scan.h -- the SPANN posting scan (SPANNIndex.cpp:193-250 after the head search, ExtraFullGraphSearcher.h:226-375)
-// as sptag_b200.cu launches it; the kernel lives in kern_spann.cu.
+// spann_scan.h -- the SPANN posting kernels as sptag_b200.cu launches them: the posting scan (SPANNIndex.cpp:193-250
+// after the head search, ExtraFullGraphSearcher.h:226-375; kern_spann.cu on raw rows, kern_spann_pq.cu on PQ code rows)
+// and the posting step of SPANN iterators (kern_spann_iter.cu), with the posting-list view both read.
 #pragma once
 #include <cstddef>
 #include <cuda_runtime.h>
@@ -8,29 +9,41 @@ namespace sptag_b200 {
 
 struct IterState;  // search_kernels.cuh
 
-struct SpannScanParams {
-    // head search results of every query, W per query, ascending, head-local ids (the head's m_results after SortResult)
-    const int* head_ids;
-    const float* head_dists;
-    int nq, w, k;
-    // the query rows, row_stride bytes apart (16-byte aligned, zero padded)
-    const unsigned char* queries;
-    size_t row_stride;
-    int dim, simd_width;
-    // m_vectorTranslateMap, each uint64 cast to SizeType (int32) as the reference does; INT_MAX = MaxSize = "no vector"
-    const int* translate;
-    // posting lists: list l has cnt[l] elements (its full count) and pages[l] pages, its ids at ids[off[l]...] and its
-    // rows at rows + (off[l] + i) * row_stride
+// The posting lists in HBM: list l has cnt[l] elements (its full count) and pages[l] pages, its ids at ids[off[l]...] and
+// its rows at rows + (off[l] + i) * row_stride
+struct PostingLists {
     const long long* off;
     const int* cnt;
     const int* pages;
     const int* ids;
     const unsigned char* rows;
+    size_t row_stride;     // also the stride of the query rows
     int vector_info_size;  // dim * sizeof(T) + sizeof(int)
+    int page_limit;        // SearchPostingPageLimit in force (already max'ed with PostingVectorLimit's pages)
+};
+
+// Elements of a list of cnt elements on `pages` pages that a search reads at page limit `limit` (LoadingHeadInfo's
+// truncation, ExtraFullGraphSearcher.h:1093-1097)
+__host__ __device__ inline int posting_searched(int cnt, int pages, int limit, int vector_info_size) {
+    const long long lim = (long long)(pages < limit ? pages : limit) << 12;
+    const long long fit = lim / vector_info_size;
+    return (int)(cnt < fit ? cnt : fit);
+}
+
+struct SpannScanParams {
+    // head search results of every query, W per query, ascending, head-local ids (the head's m_results after SortResult)
+    const int* head_ids;
+    const float* head_dists;
+    int nq, w, k;
+    // the query rows, lists.row_stride bytes apart (16-byte aligned, zero padded)
+    const unsigned char* queries;
+    int dim, simd_width;
+    // m_vectorTranslateMap, each uint64 cast to SizeType (int32) as the reference does; INT_MAX = MaxSize = "no vector"
+    const int* translate;
+    PostingLists lists;
     // search parameters
     int internal;     // SearchInternalResultNum
     float max_dist_ratio;
-    int page_limit;   // SearchPostingPageLimit in force (already max'ed with PostingVectorLimit's pages)
     // per-block dedup table of table_entries int keys (vid + 1, 0 = empty)
     int* tables;
     int table_entries;
@@ -89,16 +102,10 @@ struct SpannIterParams {
     const unsigned int* list;  // the queries of this launch (kIterListHeader layout), or nullptr: all nq
     int batch;                 // Next(batch) as the caller asked
     int fresh;                 // the first launch of a Next: cap the batch by slots and Reset() the QueryResult
-    const unsigned char* queries;
-    size_t row_stride;
+    const unsigned char* queries;  // lists.row_stride bytes apart
     int dim, simd_width;
-    const long long* off;
-    const int* cnt;
-    const int* pages;
-    const int* ids;
-    const unsigned char* rows;
-    int vector_info_size;
-    int internal, page_limit;  // SearchInternalResultNum, the page limit in force
+    PostingLists lists;
+    int internal;  // SearchInternalResultNum
     SpannIterState* st;
     int* posts;                // [nq x hb] m_postingIDs
     float* heap_d;             // [nq x cap] the call's QueryResult between launches

@@ -2897,9 +2897,10 @@ int spann_snapshot(sptag_b200_spann* s, SpannSnapshot& out) {
     return 0;
 }
 
-// Elements of list l that a search reads (LoadingHeadInfo, ExtraFullGraphSearcher.h:1093-1097)
-int spann_searched(const sptag_b200_spann* s, int l, int limit) {
-    return (int)std::min<long long>(s->cnt[l], ((long long)std::min(s->pages[l], limit) << 12) / s->vis);
+// The posting lists of the index as the posting kernels read them at page limit page_limit
+PostingLists posting_lists(const sptag_b200_spann* s, int page_limit) {
+    return {(const long long*)s->d_off.ptr, (const int*)s->d_cnt.ptr, (const int*)s->d_pages.ptr,
+            (const int*)s->d_ids.ptr, (const unsigned char*)s->d_rows.ptr, s->head->row_stride, s->vis, page_limit};
 }
 
 // The longest list a search reads at the page limit in force, and whether that limit truncates any list (recomputed when
@@ -2909,7 +2910,7 @@ void spann_update_shape(sptag_b200_spann* s) {
     s->longest = 0;
     s->truncated = false;
     for (int l = 0; l < s->num_lists; ++l) {
-        const int tc = spann_searched(s, l, limit);
+        const int tc = posting_searched(s->cnt[l], s->pages[l], limit, s->vis);
         s->longest = std::max(s->longest, tc);
         s->truncated = s->truncated || tc < s->cnt[l];
     }
@@ -3602,7 +3603,6 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     memset(&p, 0, sizeof(p));
     p.internal = sp.internal;
     p.max_dist_ratio = sp.max_dist_ratio;
-    p.page_limit = sp.page_limit;
     // SPANNIndex.cpp:197-201: the head search runs at K when K >= SearchInternalResultNum, else at SearchInternalResultNum
     const int w = k >= p.internal ? k : p.internal;
     if (w > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchInternalResultNum %d exceeds 2048", p.internal);
@@ -3678,16 +3678,10 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     p.w = w;
     p.k = k;
     p.queries = (const unsigned char*)st->d_qpad.ptr;
-    p.row_stride = h->row_stride;
     p.dim = h->dim;
     p.simd_width = h->simd_width;
     p.translate = (const int*)s->d_translate.ptr;
-    p.off = (const long long*)s->d_off.ptr;
-    p.cnt = (const int*)s->d_cnt.ptr;
-    p.pages = (const int*)s->d_pages.ptr;
-    p.ids = (const int*)s->d_ids.ptr;
-    p.rows = (const unsigned char*)s->d_rows.ptr;
-    p.vector_info_size = s->vis;
+    p.lists = posting_lists(s, sp.page_limit);
     p.tables = (int*)st->d_tables.ptr;
     p.table_entries = (int)entries;
     p.out_ids = (int*)st->d_ids.ptr;
@@ -3823,7 +3817,6 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     SpannIterParams p;
     memset(&p, 0, sizeof(p));
     p.internal = sp.internal;
-    p.page_limit = sp.page_limit;
     // The reference has SearchInternalResultNum page buffers and indexes them by m_pi (IExtraSearcher.h:114-122,
     // ExtraFullGraphSearcher.h:405, :500): a load of more lists is undefined there
     if (it->hb > p.internal)
@@ -3852,15 +3845,9 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     p.batch = batch;
     p.fresh = 1;
     p.queries = (const unsigned char*)it->d_queries.ptr;
-    p.row_stride = h->row_stride;
     p.dim = h->dim;
     p.simd_width = h->simd_width;
-    p.off = (const long long*)s->d_off.ptr;
-    p.cnt = (const int*)s->d_cnt.ptr;
-    p.pages = (const int*)s->d_pages.ptr;
-    p.ids = (const int*)s->d_ids.ptr;
-    p.rows = (const unsigned char*)s->d_rows.ptr;
-    p.vector_info_size = s->vis;
+    p.lists = posting_lists(s, sp.page_limit);
     p.st = (SpannIterState*)it->d_state.ptr;
     p.posts = (int*)it->d_posts.ptr;
     p.heap_d = (float*)it->d_heap_d.ptr;
