@@ -395,6 +395,35 @@ typedef struct sptag_b200_spann* sptag_b200_spann_handle;
 int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_handle* out);
 void sptag_b200_spann_destroy(sptag_b200_spann_handle s);
 
+/* Where sptag_b200_spann_load_ex keeps the packed posting lists (rows and ids).
+ *   AUTO:   HBM when cudaMemGetInfo's free bytes, after the head and the translate map are loaded, exceed the lists' bytes
+ *           plus a reserve of 1 GB for the searches' buffers; pinned host memory otherwise.
+ *   DEVICE: HBM, as sptag_b200_spann_load (MemoryOverFlow when they do not fit).
+ *   HOST:   one pinned, mapped host allocation (cudaHostAlloc), in the layout they have in HBM.  The translate map and each
+ *           list's offset, count and page count stay in HBM.  Every search and iterator step copies the lists its queries
+ *           read (their searched prefix, at the page limit in force) into an HBM stage of B200.PostingStageBytes per
+ *           staging set and scans them there; results equal the device placement's bit for bit.  When a batch's union of
+ *           lists does not fit the stage, the batch runs in rounds: a round takes the next n items (queries of a search,
+ *           queries of a posting-step launch of an iterator), n starting at the whole batch and halved (rounded up) until
+ *           their union fits; the next round starts from the same n.  The stage is never smaller than one query's worst
+ *           case, SearchInternalResultNum x the longest searched list x (row stride + 4) bytes.  MemoryOverFlow when the
+ *           pinned allocation fails. */
+enum {
+    SPTAG_B200_POSTINGS_AUTO = 0,
+    SPTAG_B200_POSTINGS_DEVICE = 1,
+    SPTAG_B200_POSTINGS_HOST = 2
+};
+typedef struct {
+    int32_t struct_size;        /* sizeof(sptag_b200_spann_load_options) */
+    int32_t posting_placement;  /* SPTAG_B200_POSTINGS_* */
+} sptag_b200_spann_load_options;
+
+/* sptag_b200_spann_load with a choice of where the posting lists live (options NULL: AUTO).  LackOfInputs for an unknown
+ * placement, Fail for a struct_size other than sizeof(sptag_b200_spann_load_options).  The handle's B200.PostingPlacement
+ * reads "device" or "host". */
+int sptag_b200_spann_load_ex(const char* folder, int32_t device, const sptag_b200_spann_load_options* options,
+                             sptag_b200_spann_handle* out);
+
 /* Replaces: the SSD stage of SPANN::Index<T>::BuildIndex with SelectHead and BuildHead off (SPANNIndex.cpp:889-951):
  * ExtraFullGraphSearcher::BuildIndex (ExtraFullGraphSearcher.h:587-922) with VectorIndex::ApproximateRNG
  * (VectorIndex.cpp:884-986, its CPU form), SortSelections (EdgeCompare, SearchResult.h:29-63), the posting cut (:722-760),
@@ -447,9 +476,15 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
  * default 32, in [1, 1024]; sampled when an iterator opens).  B200.IteratorVisitedSet and B200.IteratorVisitedHashEntries
  * are the head handle's (sptag_b200_set_param): they choose the visited sets of the head iterators SPANN iterators open.
  * B200.SpannDedupEntries: the first dedup table size of an iterator's queries, 0 (default: room for one head batch of
- * the longest list, at most 2^14) or a power of two >= 64; tables double as they fill.  Read-only: PostingBytes (device
- * bytes of the posting lists and the translate map), B200.LastIteratorRounds (head refill rounds of the last
- * sptag_b200_spann_iterator_next on this handle) and B200.LastIteratorDedupBytes (that iterator's dedup table bytes).
+ * the longest list, at most 2^14) or a power of two >= 64; tables double as they fill.  B200.PostingStageBytes (host
+ * placement, sptag_b200_spann_load_ex): the HBM stage of each of the two staging sets, default 268435456 (256 MB), in
+ * [0, 2^31 - 1]; 0 leaves one query's worst case.  The stage grows when a call needs more and never shrinks.
+ * Read-only: PostingBytes (device bytes of the posting lists and the translate map; with host placement the lists'
+ * offsets, counts and page counts only), B200.PostingPlacement ("device" or "host"), B200.PostingHostBytes (pinned
+ * host bytes of the lists' rows and ids, 0 with device placement), B200.LastGatherBytes and B200.LastGatherRounds (host
+ * placement: the bytes copied from host memory and the gather rounds of the last search or iterator step on this
+ * handle), B200.LastIteratorRounds (head refill rounds of the last sptag_b200_spann_iterator_next on this handle) and
+ * B200.LastIteratorDedupBytes (that iterator's dedup table bytes).
  * Names are matched case-insensitively, and codes are those of sptag_b200_set_param. */
 int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, const char* value);
 int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char* value_out, int32_t capacity);

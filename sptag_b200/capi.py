@@ -36,7 +36,7 @@ EXPORTS = [
     "sptag_b200_num_deleted", "sptag_b200_spann_load", "sptag_b200_spann_destroy", "sptag_b200_spann_search",
     "sptag_b200_spann_set_param", "sptag_b200_spann_get_param", "sptag_b200_spann_iterator_open",
     "sptag_b200_spann_iterator_next", "sptag_b200_spann_iterator_close", "sptag_b200_multi_scan",
-    "sptag_b200_spann_build", "sptag_b200_debug_kernel_for",
+    "sptag_b200_spann_build", "sptag_b200_debug_kernel_for", "sptag_b200_spann_load_ex",
 ]
 
 
@@ -52,6 +52,14 @@ class IndexDesc(C.Structure):
 class SearchOptions(C.Structure):
     _fields_ = [("struct_size", C.c_int32), ("search_deleted", C.c_int32), ("max_check", C.c_int32),
                 ("allowed", C.c_void_p)]
+
+
+class SpannLoadOptions(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("posting_placement", C.c_int32)]
+
+
+# sptag_b200_spann_load_ex's posting_placement (SPTAG_B200_POSTINGS_*)
+POSTING_PLACEMENTS = {"auto": 0, "device": 1, "host": 2}
 
 
 class SptagB200Error(RuntimeError):
@@ -115,6 +123,7 @@ def lib():
         L.sptag_b200_launch_count.restype = C.c_int64
         L.sptag_b200_debug_kernel_for.argtypes = [C.c_int32] * 11 + [C.c_char_p, C.c_int32]
         L.sptag_b200_spann_load.argtypes = [C.c_char_p, C.c_int32, C.POINTER(C.c_void_p)]
+        L.sptag_b200_spann_load_ex.argtypes = [C.c_char_p, C.c_int32, C.POINTER(SpannLoadOptions), C.POINTER(C.c_void_p)]
         L.sptag_b200_spann_destroy.argtypes = [C.c_void_p]
         L.sptag_b200_spann_destroy.restype = None
         L.sptag_b200_spann_build.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
@@ -474,7 +483,8 @@ def debug_kernel_for(*, value_type, metric, algo, dim, simd_width=16, enable_bfs
 
 
 class B200SpannIndex:
-    """Handle to a SPANN index whose head and posting lists live in HBM (SPANN::Index<T>: LoadIndex, SearchIndex)."""
+    """Handle to a SPANN index whose head lives in HBM and whose posting lists live in HBM or, loaded with
+    posting_placement="host", in pinned host memory (SPANN::Index<T>: LoadIndex, SearchIndex)."""
 
     STATS_PER_QUERY = 3  # postings scanned, list elements read, distances computed
 
@@ -482,10 +492,18 @@ class B200SpannIndex:
         self._h = C.c_void_p(handle)
 
     @classmethod
-    def load(cls, folder, device=-1):
-        """VectorIndex::LoadIndex(folder) for a SPANN folder."""
+    def load(cls, folder, device=-1, posting_placement=None):
+        """VectorIndex::LoadIndex(folder) for a SPANN folder.  posting_placement: None (the posting lists in HBM, as
+        sptag_b200_spann_load), or "auto", "device" or "host" (sptag_b200_spann_load_ex: "host" keeps them in pinned host
+        memory and gathers each batch's lists into HBM; "auto" picks HBM when they fit)."""
         h = C.c_void_p()
-        _check(lib().sptag_b200_spann_load(os.fsencode(folder), device, C.byref(h)))
+        if posting_placement is None:
+            _check(lib().sptag_b200_spann_load(os.fsencode(folder), device, C.byref(h)))
+        else:
+            if posting_placement not in POSTING_PLACEMENTS:
+                raise ValueError("posting_placement %r: one of %s" % (posting_placement, sorted(POSTING_PLACEMENTS)))
+            o = SpannLoadOptions(C.sizeof(SpannLoadOptions), POSTING_PLACEMENTS[posting_placement])
+            _check(lib().sptag_b200_spann_load_ex(os.fsencode(folder), device, C.byref(o), C.byref(h)))
         return cls(h.value)
 
     BUILD_STATS = ("searched", "rng_rejected", "edges_before_cut", "edges_after_cut", "search_us", "rng_us", "sort_us",

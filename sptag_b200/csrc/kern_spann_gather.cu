@@ -1,0 +1,163 @@
+// The gather path of posting lists in pinned host memory (PostingGather, spann_scan.h): which lists a round's queries
+// read, their union and stage offsets, and the copy of their searched prefixes from mapped host memory into the HBM
+// stage that the unchanged scan and posting-step kernels then read.
+#include "spann_device.cuh"
+#include "spann_scan.h"
+
+#include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
+#include <thrust/iterator/counting_iterator.h>
+
+#include <algorithm>
+
+namespace sptag_b200 {
+namespace {
+
+// choose_postings for every query of p, one warp per query: its head results copied to shared memory as the scan
+// copies them (the rule translates them in place), lane 0 chooses
+__global__ void __launch_bounds__(32) spann_choose_kernel(const SpannScanParams p, int* chosen, int* nchosen, int stride) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    float* rd = reinterpret_cast<float*>(smem);
+    int* rv = reinterpret_cast<int*>(rd + p.w);
+    for (int q = blockIdx.x; q < p.nq; q += gridDim.x) {
+        for (int i = threadIdx.x; i < p.w; i += 32) {
+            rv[i] = p.head_ids[(size_t)q * p.w + i];
+            rd[i] = p.head_dists[(size_t)q * p.w + i];
+        }
+        __syncwarp();
+        if (threadIdx.x == 0) {
+            int np = 0;
+            long long total = 0;
+            choose_postings(p, rd, rv, chosen + (size_t)q * stride, np, total);
+            nchosen[q] = np;
+        }
+        __syncwarp();
+    }
+}
+
+// What the posting step reads for the queries li in [b, e) of its launch: load_postings when the query loads the head's
+// latest batch (it then reads nothing else), else the rest of its lists
+__global__ void spann_iter_chosen_kernel(const SpannIterParams p, int b, int e, int* chosen, int* nchosen,
+                                         unsigned int* sub) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0) sub[0] = (unsigned)(e - b);
+    const int li = b + i;
+    if (li >= e) return;
+    const int q = p.list ? (int)p.list[kIterListHeader + li] : li;
+    sub[kIterListHeader + i] = (unsigned)q;
+    int* out = chosen + (size_t)i * p.hb;
+    const SpannIterState st = p.st[q];
+    if (st.load) {
+        nchosen[i] = load_postings(p, q, out);
+        return;
+    }
+    const int* posts = p.posts + (size_t)q * p.hb;
+    for (int j = st.pi; j < st.np; ++j) out[j - st.pi] = posts[j];
+    nchosen[i] = max(st.np - st.pi, 0);
+}
+
+__global__ void spann_mark_kernel(const int* chosen, const int* nchosen, int stride, int n, unsigned char* flags) {
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < (long long)n * stride;
+         t += (long long)gridDim.x * blockDim.x) {
+        const int q = (int)(t / stride), j = (int)(t % stride);
+        if (j < nchosen[q]) flags[chosen[t]] = 1;
+    }
+}
+
+__global__ void spann_union_len_kernel(const PostingGather g) {
+    for (int l = blockIdx.x * blockDim.x + threadIdx.x; l <= g.num_lists; l += gridDim.x * blockDim.x)
+        g.len[l] = l < g.num_lists && g.flags[l] ? searched_count(g.host, l) : 0;
+}
+
+// One CTA per union list at a time: its rows as 16-byte words (row_stride is a multiple of 16), kUnroll loads in flight
+// per thread before their stores, then its ids
+constexpr int kGatherThreads = 256;
+constexpr int kUnroll = 8;
+__global__ void __launch_bounds__(kGatherThreads) spann_gather_kernel(const PostingGather g) {
+    const int n = *g.nlists;
+    const long long words_per_row = (long long)(g.host.row_stride / 16);
+    for (int u = blockIdx.x; u < n; u += gridDim.x) {
+        const int l = g.lists[u];
+        const long long from = g.host.off[l], to = g.stage_off[l], c = g.len[l];
+        const uint4* src = reinterpret_cast<const uint4*>(g.host.rows) + from * words_per_row;
+        uint4* dst = reinterpret_cast<uint4*>(g.stage_rows) + to * words_per_row;
+        const long long words = c * words_per_row;
+        for (long long w0 = threadIdx.x; w0 < words; w0 += (long long)kUnroll * kGatherThreads) {
+            uint4 v[kUnroll];
+#pragma unroll
+            for (int j = 0; j < kUnroll; ++j) {
+                const long long w = w0 + (long long)j * kGatherThreads;
+                if (w < words) v[j] = src[w];
+            }
+#pragma unroll
+            for (int j = 0; j < kUnroll; ++j) {
+                const long long w = w0 + (long long)j * kGatherThreads;
+                if (w < words) dst[w] = v[j];
+            }
+        }
+        for (long long i = threadIdx.x; i < c; i += kGatherThreads) g.stage_ids[to + i] = g.host.ids[from + i];
+    }
+}
+
+// The stage offsets (exclusive sum of g.len) and the compacted union (the flagged list numbers); with temp null, the
+// scratch bytes the two need
+cudaError_t union_cub(const PostingGather& g, void* temp, size_t& bytes, cudaStream_t stream) {
+    const thrust::counting_iterator<int> list_numbers(0);
+    if (!temp) {
+        size_t scan = 0, select = 0;
+        cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, scan, g.len, g.stage_off, g.num_lists + 1, stream);
+        if (e == cudaSuccess)
+            e = cub::DeviceSelect::Flagged(nullptr, select, list_numbers, g.flags, g.lists, g.nlists, g.num_lists, stream);
+        bytes = std::max(scan, select);
+        return e;
+    }
+    cudaError_t e = cub::DeviceScan::ExclusiveSum(temp, bytes, g.len, g.stage_off, g.num_lists + 1, stream);
+    if (e == cudaSuccess)
+        e = cub::DeviceSelect::Flagged(temp, bytes, list_numbers, g.flags, g.lists, g.nlists, g.num_lists, stream);
+    return e;
+}
+
+}  // namespace
+
+size_t spann_union_temp_bytes(int num_lists) {
+    PostingGather g = {};
+    g.num_lists = num_lists;
+    size_t bytes = 0;
+    return union_cub(g, nullptr, bytes, nullptr) == cudaSuccess ? bytes : 0;
+}
+
+cudaError_t launch_spann_choose(const SpannScanParams& p, int* chosen, int* nchosen, int stride, cudaStream_t stream) {
+    // W <= 2048: at most 16 KB of head results
+    spann_choose_kernel<<<std::min(p.nq, 65535), 32, (size_t)p.w * 8, stream>>>(p, chosen, nchosen, stride);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_spann_iter_chosen(const SpannIterParams& p, int b, int e, int* chosen, int* nchosen, unsigned int* sub,
+                                     cudaStream_t stream) {
+    const int n = std::max(e - b, 1);
+    spann_iter_chosen_kernel<<<(n + 127) / 128, 128, 0, stream>>>(p, b, e, chosen, nchosen, sub);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_spann_union(const PostingGather& g, const int* chosen, const int* nchosen, int stride, int n,
+                               cudaStream_t stream) {
+    cudaError_t e = cudaMemsetAsync(g.flags, 0, (size_t)g.num_lists, stream);
+    if (e != cudaSuccess) return e;
+    const long long marks = (long long)n * stride;
+    if (marks > 0) {
+        spann_mark_kernel<<<(int)std::min<long long>((marks + 255) / 256, 4096), 256, 0, stream>>>(chosen, nchosen, stride, n,
+                                                                                                  g.flags);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    spann_union_len_kernel<<<std::min((g.num_lists + 256) / 256, 4096), 256, 0, stream>>>(g);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    size_t bytes = g.temp_bytes;
+    return union_cub(g, g.temp, bytes, stream);
+}
+
+cudaError_t launch_spann_gather(const PostingGather& g, int grid, cudaStream_t stream) {
+    spann_gather_kernel<<<grid, kGatherThreads, 0, stream>>>(g);
+    return cudaGetLastError();
+}
+
+}  // namespace sptag_b200

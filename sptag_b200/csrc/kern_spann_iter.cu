@@ -68,15 +68,7 @@ __global__ void __launch_bounds__(32) spann_iter_step_kernel(const SpannIterPara
         __syncwarp();
         while (!stop && count < batch) {
             if (load) {  // SearchDiskIndexIterative with m_loadPosting (SPANNIndex.cpp:420-442)
-                if (lane == 0) {
-                    int m = 0;
-                    for (int i = 0; i < p.hb; ++i) {
-                        const int pid = p.head_ids[(size_t)q * p.hb + i];
-                        if (pid == -1) break;
-                        if (searched_count(p.lists, pid) > 0) posts[m++] = pid;  // CheckValidPosting
-                    }
-                    shared_int[0] = m;
-                }
+                if (lane == 0) shared_int[0] = load_postings(p, q, posts);
                 __syncwarp();
                 np = shared_int[0];
                 if (loaded >= p.internal) relaxed = 1;

@@ -146,6 +146,46 @@ __device__ __forceinline__ int searched_count(const PostingLists pl, int l) {
     return posting_searched(pl.cnt[l], pl.pages[l], pl.page_limit, pl.vector_info_size);
 }
 
+// The postings a search reads (SPANNIndex.cpp:213-234), by one lane: limitDist = result[0].Dist * MaxDistRatio (float),
+// then per head result until VID -1: translate it in place in (rd, rv) (INT_MAX: no vector, (MaxDist, -1)), and choose
+// its list while fewer than SearchInternalResultNum are chosen, its distance is within limitDist and the list holds
+// elements at the page limit (CheckValidPosting, :931-934).  Appends the chosen lists to posts in result order, counting
+// them in np and their elements in total (both start at 0).  The posting scan reads exactly these lists.  (p by
+// reference and np / total as the caller's variables: so the scan's instructions stay those of the rule written out.)
+__device__ __forceinline__ void choose_postings(const SpannScanParams& p, float* rd, int* rv, int* posts, int& np,
+                                                long long& total) {
+    const float limit = __fmul_rn(rd[0], p.max_dist_ratio);
+    for (int i = 0; i < p.w; ++i) {
+        const int pid = rv[i];
+        if (pid == -1) break;
+        const int t = p.translate[pid];
+        if (t == INT_MAX) {
+            rv[i] = -1;
+            rd[i] = SPTAG_B200_MAXDIST;
+        } else {
+            rv[i] = t;
+        }
+        if (np >= p.internal || ((double)limit > 0.1 && rd[i] > limit)) continue;
+        const int tc = searched_count(p.lists, pid);
+        if (tc == 0) continue;
+        posts[np++] = pid;
+        total += tc;
+    }
+}
+
+// SearchDiskIndexIterative's load of the head iterator's latest batch for query q (SPANNIndex.cpp:420-442), by one lane:
+// its lists up to the first -1 that hold elements at the page limit (CheckValidPosting), in result order, written to
+// posts; returns their number
+__device__ __forceinline__ int load_postings(const SpannIterParams p, int q, int* posts) {
+    int m = 0;
+    for (int i = 0; i < p.hb; ++i) {
+        const int pid = p.head_ids[(size_t)q * p.hb + i];
+        if (pid == -1) break;
+        if (searched_count(p.lists, pid) > 0) posts[m++] = pid;
+    }
+    return m;
+}
+
 // The distances of a chunk to the query row qrow on raw rows: a half-warp per row, two rows at a time, with the head
 // index's DistanceUtils tree.  chunk(pl, base, cl, cnt, cd): cd[r] = the distance to element cl[r] of the list whose first
 // element is base (its off[l]), for r < cnt.
@@ -201,26 +241,9 @@ __device__ __forceinline__ void spann_scan_body(const SpannScanParams p, unsigne
         }
         __syncwarp();
         if (lane == 0) {
-            // SPANNIndex.cpp:213-234: limitDist = result[0].Dist * MaxDistRatio (float), then per result until VID -1
-            const float limit = __fmul_rn(rd[0], p.max_dist_ratio);
             int np = 0;
             long long total = 0;
-            for (int i = 0; i < p.w; ++i) {
-                const int pid = rv[i];
-                if (pid == -1) break;
-                const int t = p.translate[pid];
-                if (t == INT_MAX) {
-                    rv[i] = -1;
-                    rd[i] = SPTAG_B200_MAXDIST;
-                } else {
-                    rv[i] = t;
-                }
-                if (np >= p.internal || ((double)limit > 0.1 && rd[i] > limit)) continue;
-                const int tc = searched_count(p.lists, pid);
-                if (tc == 0) continue;  // CheckValidPosting (:931-934)
-                posts[np++] = pid;
-                total += tc;
-            }
+            choose_postings(p, rd, rv, posts, np, total);
             shared_int[0] = np;
             // the deduper needs room for every element this query reads; the table keeps at most half its entries used
             int entries = 64;

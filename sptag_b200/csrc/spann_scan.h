@@ -123,4 +123,38 @@ struct SpannIterParams {
 cudaError_t launch_spann_iter_step(const SpannIterParams& p, bool cosine, int elem, int grid, cudaStream_t stream);
 int spann_iter_step_blocks_per_sm(bool cosine, int elem, int cap);
 
+// Posting lists in pinned host memory (kern_spann_gather.cu).  The packed lists stay where they were loaded (`host`: ids
+// and rows in mapped host memory, off, cnt and pages in HBM); before the scan or a posting step runs, the union of the
+// lists its queries read is copied into an HBM stage, and the kernels read a PostingLists view of the stage:
+// off = stage_off, ids = stage_ids, rows = stage_rows, cnt and pages unchanged.  A union list keeps its searched prefix
+// (posting_searched at host.page_limit) in the stage.
+struct PostingGather {
+    PostingLists host;
+    int num_lists;
+    unsigned char* flags;   // [num_lists] the union's lists
+    long long* len;         // [num_lists + 1] searched elements of a union list, 0 for the others
+    long long* stage_off;   // [num_lists + 1] exclusive sum of len: a union list's first element in the stage; the last
+                            // entry is the union's element count
+    int* lists;             // [num_lists] the union, compacted in list order
+    int* nlists;            // its size
+    void* temp;             // CUB scratch of spann_union_temp_bytes(num_lists) bytes
+    size_t temp_bytes;
+    int* stage_ids;
+    unsigned char* stage_rows;
+};
+size_t spann_union_temp_bytes(int num_lists);
+// chosen[q * stride ...] / nchosen[q]: the lists query q of a search reads (choose_postings), for every query of p
+cudaError_t launch_spann_choose(const SpannScanParams& p, int* chosen, int* nchosen, int stride, cudaStream_t stream);
+// chosen[(li - b) * p.hb ...] / nchosen[li - b]: the lists the queries li in [b, e) of an iterator launch read (p.list, or
+// every query when it is null): the head's latest batch if the query loads it (load_postings), else posts[pi .. np).
+// sub (kIterListHeader layout) receives those queries, for a launch over them.
+cudaError_t launch_spann_iter_chosen(const SpannIterParams& p, int b, int e, int* chosen, int* nchosen, unsigned int* sub,
+                                     cudaStream_t stream);
+// The union of the lists of n items (chosen / nchosen as above, stride apart): g.flags, g.len, g.stage_off, g.lists and
+// g.nlists.  g.stage_off[g.num_lists] is the union's element count.
+cudaError_t launch_spann_union(const PostingGather& g, const int* chosen, const int* nchosen, int stride, int n,
+                               cudaStream_t stream);
+// Copies the searched prefix of every union list's rows and ids from host memory into the stage
+cudaError_t launch_spann_gather(const PostingGather& g, int grid, cudaStream_t stream);
+
 }  // namespace sptag_b200

@@ -2857,11 +2857,22 @@ struct sptag_b200_spann {
     int dedup_entries = 0;
     long last_iter_rounds = 0, last_iter_dedup_bytes = 0;
     DeviceBuffer d_translate, d_off, d_cnt, d_pages, d_ids, d_rows;
+    // Host placement (sptag_b200_spann_load_ex): the rows, then the ids, in one pinned mapped allocation, and the HBM stage
+    // of each staging set (B200.PostingStageBytes); what the last search or iterator step on this handle gathered
+    bool host_postings = false;
+    void* h_postings = nullptr;
+    size_t h_posting_bytes = 0;
+    const unsigned char* h_rows = nullptr;  // device (mapped) pointers into h_postings
+    const int* h_ids = nullptr;
+    int stage_bytes = 256 << 20;
+    long last_gather_bytes = 0, last_gather_rounds = 0;
     // Host-buffer calls run on one of two staging sets, each with its own stream, head results, dedup tables and outputs,
     // so that two callers overlap; the head search kernels are ordered by the head handle (search_device_impl)
     struct StagingBuffers {
         DeviceBuffer d_q, d_qpad, d_hids, d_hdists, d_ids, d_dists, d_stats, d_tables;
         DeviceBuffer d_codes, d_adc;  // quantized: the queries' codes (SDC) or rotated vectors (ADC); ADC tables per block
+        // host placement: the chosen lists per item, the union (PostingGather), an iterator launch's sub-list, the stage
+        DeviceBuffer d_chosen, d_nchosen, d_flags, d_len, d_stage_off, d_union, d_nunion, d_cub, d_sub, d_stage;
     };
     StagingPool<StagingBuffers> staging;
     std::mutex mu;  // the search parameters
@@ -2875,7 +2886,7 @@ int spann_page_limit(const sptag_b200_spann* s) { return std::max(s->page_limit,
 
 // The parameters a SPANN search or iterator step runs with, read together under s->mu
 struct SpannSnapshot {
-    int internal, page_limit, longest;
+    int internal, page_limit, longest, stage_bytes;
     float max_dist_ratio;
 };
 // Takes the snapshot, and refuses a page limit that truncates lists of the rearranged layout: the reference reads a
@@ -2889,6 +2900,7 @@ int spann_snapshot(sptag_b200_spann* s, SpannSnapshot& out) {
         out.max_dist_ratio = s->max_dist_ratio;
         out.page_limit = spann_page_limit(s);
         out.longest = s->longest;
+        out.stage_bytes = s->stage_bytes;
         truncated = s->truncated;
     }
     if (truncated && s->rearranged)
@@ -2897,10 +2909,79 @@ int spann_snapshot(sptag_b200_spann* s, SpannSnapshot& out) {
     return 0;
 }
 
-// The posting lists of the index as the posting kernels read them at page limit page_limit
+// The posting lists of the index as the posting kernels read them at page limit page_limit (host placement: the ids and
+// rows in mapped host memory, which gather_rounds stages)
 PostingLists posting_lists(const sptag_b200_spann* s, int page_limit) {
-    return {(const long long*)s->d_off.ptr, (const int*)s->d_cnt.ptr, (const int*)s->d_pages.ptr,
-            (const int*)s->d_ids.ptr, (const unsigned char*)s->d_rows.ptr, s->head->row_stride, s->vis, page_limit};
+    const int* ids = s->host_postings ? s->h_ids : (const int*)s->d_ids.ptr;
+    const unsigned char* rows = s->host_postings ? s->h_rows : (const unsigned char*)s->d_rows.ptr;
+    return {(const long long*)s->d_off.ptr, (const int*)s->d_cnt.ptr, (const int*)s->d_pages.ptr, ids, rows,
+            s->head->row_stride, s->vis, page_limit};
+}
+
+// Host placement: runs the n items of a call (the queries of a search, or of an iterator's posting-step launch) in
+// gather rounds on staging set sb.  A round takes the next m items, m starting at n and halved (rounded up) until the
+// union of their lists fits the stage (never below one item), gathers that union into the stage and runs them on it;
+// the next round starts from the same m.  choose(b, e, chosen, nchosen) points chosen / nchosen at the lists items
+// [b, e) read (stride apart), enqueued on stream; run(b, e, view) runs items [b, e) on the staged view.  The stage holds
+// the larger of B200.PostingStageBytes and one query's worst case.  Adds the bytes gathered and the rounds to bytes and
+// rounds.
+template <typename Buffers, typename Choose, typename Run>
+int gather_rounds(sptag_b200_spann* s, Buffers& sb, const SpannSnapshot& sp, int n, int stride, cudaStream_t stream,
+                  Choose&& choose, Run&& run, long& bytes, long& rounds) {
+    const PostingLists host = posting_lists(s, sp.page_limit);
+    const long long elem_bytes = (long long)host.row_stride + 4;
+    const long long cap = std::max<long long>(sp.stage_bytes, (long long)std::max(sp.internal, 0) * sp.longest * elem_bytes);
+    const long long cap_elems = cap / elem_bytes;
+    const size_t nl = (size_t)s->num_lists;
+    const size_t temp = spann_union_temp_bytes(s->num_lists);
+    if (temp == 0) return fail(SPTAG_B200_FAIL, "the posting-list union's scratch size query failed");
+    if (int rc = sb.d_flags.ensure(nl)) return rc;
+    if (int rc = sb.d_len.ensure((nl + 1) * 8)) return rc;
+    if (int rc = sb.d_stage_off.ensure((nl + 1) * 8)) return rc;
+    if (int rc = sb.d_union.ensure(nl * 4 + 4)) return rc;
+    if (int rc = sb.d_nunion.ensure(4)) return rc;
+    if (int rc = sb.d_cub.ensure(temp)) return rc;
+    if (int rc = sb.d_stage.ensure((size_t)std::max(cap_elems, 1ll) * elem_bytes)) return rc;
+    PostingGather g;
+    memset(&g, 0, sizeof(g));
+    g.host = host;
+    g.num_lists = s->num_lists;
+    g.flags = (unsigned char*)sb.d_flags.ptr;
+    g.len = (long long*)sb.d_len.ptr;
+    g.stage_off = (long long*)sb.d_stage_off.ptr;
+    g.lists = (int*)sb.d_union.ptr;
+    g.nlists = (int*)sb.d_nunion.ptr;
+    g.temp = sb.d_cub.ptr;
+    g.temp_bytes = sb.d_cub.bytes;
+    g.stage_rows = (unsigned char*)sb.d_stage.ptr;
+    g.stage_ids = (int*)(g.stage_rows + (size_t)std::max(cap_elems, 1ll) * host.row_stride);
+    PostingLists view = host;
+    view.off = g.stage_off;
+    view.ids = g.stage_ids;
+    view.rows = g.stage_rows;
+    const int grid = s->head->num_sms * 4;
+    for (int b = 0, m = n; b < n; b += m) {
+        m = std::min(m, n - b);
+        long long elems = 0;
+        for (;;) {
+            const int* chosen = nullptr;
+            const int* nchosen = nullptr;
+            if (int rc = choose(b, b + m, chosen, nchosen)) return rc;
+            CUDA_OK(launch_spann_union(g, chosen, nchosen, stride, m, stream));
+            CUDA_OK(cudaMemcpyAsync(&elems, g.stage_off + nl, 8, cudaMemcpyDeviceToHost, stream));
+            CUDA_OK(cudaStreamSynchronize(stream));
+            if (elems <= cap_elems || m == 1) break;
+            m = (m + 1) / 2;
+        }
+        if (elems > cap_elems)  // one query reads at most SearchInternalResultNum lists of at most `longest` elements
+            return fail(SPTAG_B200_FAIL, "one query's %lld posting elements exceed the stage's %lld", elems, cap_elems);
+        CUDA_OK(launch_spann_gather(g, grid, stream));
+        g_launches++;
+        if (int rc = run(b, b + m, view)) return rc;
+        bytes += (long)(elems * elem_bytes);
+        ++rounds;
+    }
+    return 0;
 }
 
 // The longest list a search reads at the page limit in force, and whether that limit truncates any list (recomputed when
@@ -2935,6 +3016,12 @@ const Param<Spann> kSpannParams[] = {
     {"PostingBytes", [](Spann* s, char* o, size_t n) {
          return put(o, n, "%zu", s->d_translate.bytes + s->d_off.bytes + s->d_cnt.bytes + s->d_pages.bytes + s->d_ids.bytes + s->d_rows.bytes);
      }},
+    // host placement (sptag_b200_spann_load_ex): the HBM stage per staging set, and what the placement holds and gathered
+    {"B200.PostingStageBytes", &Spann::stage_bytes, 0, 0, INT_MAX},
+    {"B200.PostingPlacement", [](Spann* s, char* o, size_t n) { return put(o, n, "%s", s->host_postings ? "host" : "device"); }},
+    {"B200.PostingHostBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%zu", s->h_posting_bytes); }},
+    {"B200.LastGatherBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_gather_bytes); }},
+    {"B200.LastGatherRounds", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_gather_rounds); }},
     {"B200.LastIteratorRounds", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_iter_rounds); }},
     {"B200.LastIteratorDedupBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_iter_dedup_bytes); }},
 };
@@ -2980,8 +3067,9 @@ int read_posting_header(FILE* f, PostingFile& pf, const char* name) {
 
 
 // Everything sptag_b200_spann_load reads after the head: the head's [BuildHead] parameters, the search parameters, the
-// translate map and the posting files.  The caller destroys s on failure.
-int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& ini) {
+// translate map and the posting files, with the lists' rows and ids placed as `placement` says (SPTAG_B200_POSTINGS_*).
+// The caller destroys s on failure.
+int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& ini, int placement) {
     auto get = [&](const char* section, const char* name, const char* def) { return ini_get(ini, section, name, def); };
     sptag_b200_handle head = s->head;
     // SPANN::Index::LoadConfig hands every [BuildHead] entry to the head (SPANNIndex.cpp:59-71, :1033-1038)
@@ -3040,12 +3128,43 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
     if (int rc = s->d_off.ensure(off.size() * 8)) return rc;
     if (int rc = s->d_cnt.ensure(off.size() * 4)) return rc;
     if (int rc = s->d_pages.ensure(off.size() * 4)) return rc;
-    if (int rc = s->d_ids.ensure(((size_t)total + 1) * 4)) return rc;
-    if (int rc = s->d_rows.ensure(((size_t)total + 1) * rs)) return rc;
+    const size_t rows_bytes = ((size_t)total + 1) * rs, ids_bytes = ((size_t)total + 1) * 4;
+    if (placement == SPTAG_B200_POSTINGS_AUTO) {
+        // HBM when the lists fit beside a reserve for the searches' buffers (head results, dedup tables, outputs)
+        const size_t kReserve = 1ull << 30;
+        size_t free_bytes = 0, total_bytes = 0;
+        CUDA_OK(cudaMemGetInfo(&free_bytes, &total_bytes));
+        placement = free_bytes >= rows_bytes + ids_bytes + kReserve ? SPTAG_B200_POSTINGS_DEVICE : SPTAG_B200_POSTINGS_HOST;
+    }
+    unsigned char* rows_base = nullptr;
+    int32_t* ids_base = nullptr;
+    if (placement == SPTAG_B200_POSTINGS_HOST) {
+        // the rows, then the ids (rows_bytes is a multiple of 16), in the layout they have in HBM
+        if (cudaHostAlloc(&s->h_postings, rows_bytes + ids_bytes, cudaHostAllocMapped) != cudaSuccess) {
+            s->h_postings = nullptr;
+            cudaGetLastError();
+            return fail(SPTAG_B200_MEMORY_OVERFLOW, "cudaHostAlloc(%zu) of the posting lists failed", rows_bytes + ids_bytes);
+        }
+        s->host_postings = true;
+        s->h_posting_bytes = rows_bytes + ids_bytes;
+        memset(s->h_postings, 0, rows_bytes);
+        void* dev = nullptr;
+        CUDA_OK(cudaHostGetDevicePointer(&dev, s->h_postings, 0));
+        rows_base = (unsigned char*)dev;
+        ids_base = (int32_t*)(rows_base + rows_bytes);
+        s->h_rows = rows_base;
+        s->h_ids = ids_base;
+    } else {
+        if (int rc = s->d_ids.ensure(ids_bytes)) return rc;
+        if (int rc = s->d_rows.ensure(rows_bytes)) return rc;
+        CUDA_OK(cudaMemset(s->d_rows.ptr, 0, s->d_rows.bytes));
+        rows_base = (unsigned char*)s->d_rows.ptr;
+        ids_base = (int32_t*)s->d_ids.ptr;
+    }
+    const cudaMemcpyKind to = s->host_postings ? cudaMemcpyDefault : cudaMemcpyDeviceToDevice;  // UVA: to mapped host memory
     CUDA_OK(cudaMemcpy(s->d_off.ptr, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(s->d_cnt.ptr, s->cnt.data(), off.size() * 4, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(s->d_pages.ptr, s->pages.data(), off.size() * 4, cudaMemcpyHostToDevice));
-    CUDA_OK(cudaMemset(s->d_rows.ptr, 0, s->d_rows.bytes));
     // The lists of a file are read in file order, in runs of consecutive lists of at most kRun bytes (a longer list is a
     // run of its own), each run streamed through upload_rows' pinned chunks into one device staging buffer and split
     // there: ParsePostingList lays an element out as int32 id + row, ParsePostingListRearrange as every row of the list,
@@ -3085,14 +3204,14 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
                 const int i = order[r];
                 const size_t c = (size_t)pf.cnt[i], l = first_list + (size_t)i;
                 const unsigned char* src_list = (const unsigned char*)stage.ptr + (pf.start[i] - begin);
-                unsigned char* drow = (unsigned char*)s->d_rows.ptr + (size_t)off[l] * rs;
-                int32_t* did = (int32_t*)s->d_ids.ptr + off[l];
+                unsigned char* drow = rows_base + (size_t)off[l] * rs;
+                int32_t* did = ids_base + off[l];
                 if (s->rearranged) {
-                    CUDA_OK(cudaMemcpy2DAsync(drow, rs, src_list, row_bytes, row_bytes, c, cudaMemcpyDeviceToDevice, up));
-                    CUDA_OK(cudaMemcpyAsync(did, src_list + c * row_bytes, c * 4, cudaMemcpyDeviceToDevice, up));
+                    CUDA_OK(cudaMemcpy2DAsync(drow, rs, src_list, row_bytes, row_bytes, c, to, up));
+                    CUDA_OK(cudaMemcpyAsync(did, src_list + c * row_bytes, c * 4, to, up));
                 } else {
-                    CUDA_OK(cudaMemcpy2DAsync(did, 4, src_list, (size_t)s->vis, 4, c, cudaMemcpyDeviceToDevice, up));
-                    CUDA_OK(cudaMemcpy2DAsync(drow, rs, src_list + 4, (size_t)s->vis, row_bytes, c, cudaMemcpyDeviceToDevice, up));
+                    CUDA_OK(cudaMemcpy2DAsync(did, 4, src_list, (size_t)s->vis, 4, c, to, up));
+                    CUDA_OK(cudaMemcpy2DAsync(drow, rs, src_list + 4, (size_t)s->vis, row_bytes, c, to, up));
                 }
             }
             CUDA_OK(cudaStreamSynchronize(up));  // the next run reuses the staging buffer
@@ -3291,13 +3410,32 @@ void sptag_b200_spann_destroy(sptag_b200_spann_handle s) {
         DeviceGuard guard(s->head ? s->head->device : 0);
         cudaDeviceSynchronize();
         sptag_b200_handle head = s->head;
+        if (s->h_postings) cudaFreeHost(s->h_postings);
         delete s;  // frees the device buffers, with the index's device current
         sptag_b200_destroy(head);
     }
 }
 
 int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_handle* out) {
+    sptag_b200_spann_load_options o;
+    o.struct_size = (int32_t)sizeof(o);
+    o.posting_placement = SPTAG_B200_POSTINGS_DEVICE;
+    return sptag_b200_spann_load_ex(folder, device, &o, out);
+}
+
+int sptag_b200_spann_load_ex(const char* folder, int32_t device, const sptag_b200_spann_load_options* options,
+                             sptag_b200_spann_handle* out) {
     if (!folder || !out) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
+    int placement = SPTAG_B200_POSTINGS_AUTO;
+    if (options) {
+        if (options->struct_size != (int32_t)sizeof(sptag_b200_spann_load_options))
+            return fail(SPTAG_B200_FAIL, "options size mismatch: %d vs %zu", options->struct_size,
+                        sizeof(sptag_b200_spann_load_options));
+        placement = options->posting_placement;
+        if (placement != SPTAG_B200_POSTINGS_AUTO && placement != SPTAG_B200_POSTINGS_DEVICE &&
+            placement != SPTAG_B200_POSTINGS_HOST)
+            return fail(SPTAG_B200_LACK_OF_INPUTS, "unknown posting placement %d", placement);
+    }
     *out = nullptr;
     const std::string dir(folder);
     IniSections ini;
@@ -3350,7 +3488,7 @@ int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_h
         sptag_b200_spann_destroy(s);
         return fail(SPTAG_B200_LACK_OF_INPUTS, "head index value type %d does not match ValueType %s", head->value_type, vt.c_str());
     }
-    if (int rc = spann_fill(s, dir, ini)) {
+    if (int rc = spann_fill(s, dir, ini, placement)) {
         sptag_b200_spann_destroy(s);
         return rc;
     }
@@ -3688,11 +3826,56 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     p.out_dists = (float*)st->d_dists.ptr;
     p.out_stats = out_stats ? (int*)st->d_stats.ptr : nullptr;
     pq.s = p;
-    cudaError_t e = s->quantized ? launch_spann_pq_scan(pq, grid, stream) : launch_spann_scan(p, me.cosine, me.elem, grid, stream);
-    g_launches++;
-    if (e != cudaSuccess) {
-        cudaStreamSynchronize(stream);
-        return fail(SPTAG_B200_FAIL, "posting scan launch failed: %s", cudaGetErrorString(e));
+    if (s->host_postings) {
+        // the queries' chosen lists, once; then the rounds, each a scan over its queries on the staged lists
+        const int stride = std::max(p.internal, 1);
+        long bytes = 0, rounds = 0;
+        int rc = 0;
+        if (!(rc = st->d_chosen.ensure(nq * stride * 4)) && !(rc = st->d_nchosen.ensure(nq * 4))) {
+            const cudaError_t e = launch_spann_choose(p, (int*)st->d_chosen.ptr, (int*)st->d_nchosen.ptr, stride, stream);
+            g_launches++;
+            if (e != cudaSuccess) rc = fail(SPTAG_B200_FAIL, "posting choice launch failed: %s", cudaGetErrorString(e));
+        }
+        auto choose = [&](int b, int, const int*& chosen, const int*& nchosen) {
+            chosen = (const int*)st->d_chosen.ptr + (size_t)b * stride;
+            nchosen = (const int*)st->d_nchosen.ptr + b;
+            return 0;
+        };
+        auto run = [&](int b, int e, const PostingLists& view) {
+            SpannPqScanParams r = pq;
+            r.s.head_ids += (size_t)b * w;
+            r.s.head_dists += (size_t)b * w;
+            r.s.nq = e - b;
+            r.s.queries += (size_t)b * h->row_stride;
+            r.s.lists = view;
+            r.s.out_ids += (size_t)b * k;
+            r.s.out_dists += (size_t)b * k;
+            if (r.s.out_stats) r.s.out_stats += (size_t)b * 3;
+            if (r.qcodes) r.qcodes += (size_t)b * r.m;
+            if (r.qrot) r.qrot += (size_t)b * r.m * r.dsub;
+            const int g = std::min(grid, e - b);
+            const cudaError_t err = s->quantized ? launch_spann_pq_scan(r, g, stream)
+                                                 : launch_spann_scan(r.s, me.cosine, me.elem, g, stream);
+            g_launches++;
+            if (err != cudaSuccess) return fail(SPTAG_B200_FAIL, "posting scan launch failed: %s", cudaGetErrorString(err));
+            return 0;
+        };
+        if (!rc) rc = gather_rounds(s, *st, sp, num_queries, stride, stream, choose, run, bytes, rounds);
+        if (rc) {
+            cudaStreamSynchronize(stream);
+            return rc;
+        }
+        std::lock_guard<std::mutex> lock(s->mu);
+        s->last_gather_bytes = bytes;
+        s->last_gather_rounds = rounds;
+    } else {
+        cudaError_t e = s->quantized ? launch_spann_pq_scan(pq, grid, stream)
+                                     : launch_spann_scan(p, me.cosine, me.elem, grid, stream);
+        g_launches++;
+        if (e != cudaSuccess) {
+            cudaStreamSynchronize(stream);
+            return fail(SPTAG_B200_FAIL, "posting scan launch failed: %s", cudaGetErrorString(e));
+        }
     }
     CUDA_OK(cudaMemcpyAsync(out_ids, st->d_ids.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaMemcpyAsync(out_dists, st->d_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
@@ -3866,11 +4049,40 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
         CUDA_OK(cudaMemsetAsync(p.susp, 0, kIterListHeader * 4, stream));
         return 0;
     };
-    auto launch = [&](long long n) -> int {
-        const cudaError_t e = launch_spann_iter_step(p, me.cosine, me.elem, (int)std::min(n, max_grid), stream);
+    auto step = [&](const SpannIterParams& sp_, long long n) -> int {
+        const cudaError_t e = launch_spann_iter_step(sp_, me.cosine, me.elem, (int)std::min(n, max_grid), stream);
         g_launches++;
         if (e != cudaSuccess) return fail(SPTAG_B200_FAIL, "posting step launch failed: %s", cudaGetErrorString(e));
         return 0;
+    };
+    // Host placement: a staging set for the call, whose stage each launch's rounds fill (gather_rounds over the launch's
+    // queries, each round a launch over its sub-list)
+    std::unique_lock<std::mutex> slock;
+    auto* gs = s->host_postings ? s->staging.acquire(slock) : nullptr;
+    long gather_bytes = 0, gather_rounds_n = 0;
+    if (gs) {
+        if (int rc = gs->d_chosen.ensure(nq * it->hb * 4)) return rc;
+        if (int rc = gs->d_nchosen.ensure(nq * 4)) return rc;
+        if (int rc = gs->d_sub.ensure((kIterListHeader + nq) * 4)) return rc;
+    }
+    auto launch = [&](long long n) -> int {
+        if (!gs) return step(p, n);
+        unsigned int* sub = (unsigned int*)gs->d_sub.ptr;
+        auto choose = [&](int b, int e, const int*& chosen, const int*& nchosen) {
+            chosen = (const int*)gs->d_chosen.ptr;
+            nchosen = (const int*)gs->d_nchosen.ptr;
+            const cudaError_t err = launch_spann_iter_chosen(p, b, e, (int*)gs->d_chosen.ptr, (int*)gs->d_nchosen.ptr, sub, stream);
+            g_launches++;
+            if (err != cudaSuccess) return fail(SPTAG_B200_FAIL, "posting choice launch failed: %s", cudaGetErrorString(err));
+            return 0;
+        };
+        auto run = [&](int b, int e, const PostingLists& view) {
+            SpannIterParams r = p;
+            r.list = sub;
+            r.lists = view;
+            return step(r, e - b);
+        };
+        return gather_rounds(s, *gs, sp, (int)n, it->hb, stream, choose, run, gather_bytes, gather_rounds_n);
     };
     // Rounds: the posting step over the queries of the round; queries whose tables must grow run again (same round);
     // then the head's FromNeareast(false) for the queries whose postings ran out, and the posting step over those.
@@ -3907,6 +4119,10 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     std::lock_guard<std::mutex> lock(s->mu);
     s->last_iter_rounds = rounds;
     s->last_iter_dedup_bytes = (long)it->dedup.bytes();
+    if (gs) {
+        s->last_gather_bytes = gather_bytes;
+        s->last_gather_rounds = gather_rounds_n;
+    }
     return SPTAG_B200_SUCCESS;
 }
 
