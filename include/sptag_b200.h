@@ -484,7 +484,9 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
  * host bytes of the lists' rows and ids, 0 with device placement), B200.LastGatherBytes and B200.LastGatherRounds (host
  * placement: the bytes copied from host memory and the gather rounds of the last search or iterator step on this
  * handle), B200.LastIteratorRounds (head refill rounds of the last sptag_b200_spann_iterator_next on this handle) and
- * B200.LastIteratorDedupBytes (that iterator's dedup table bytes).
+ * B200.LastIteratorDedupBytes (that iterator's dedup table bytes), and B200.LastPostingKernel (the demangled name of the
+ * last posting-scan or posting-step kernel instantiation a search or iterator step on this handle launched, e.g.
+ * "sptag_b200::(anonymous namespace)::spann_scan_kernel<true, 2>"; empty before the first).
  * Names are matched case-insensitively, and codes are those of sptag_b200_set_param. */
 int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, const char* value);
 int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char* value_out, int32_t capacity);

@@ -539,8 +539,8 @@ class B200SpannIndex:
         _check(lib().sptag_b200_spann_set_param(self._h, name.encode(), str(value).encode()))
 
     def get_param(self, name):
-        buf = C.create_string_buffer(64)
-        _check(lib().sptag_b200_spann_get_param(self._h, name.encode(), buf, 64))
+        buf = C.create_string_buffer(256)  # room for B200.LastPostingKernel's kernel names
+        _check(lib().sptag_b200_spann_get_param(self._h, name.encode(), buf, 256))
         return buf.value.decode()
 
     def search(self, queries, k, want_stats=False):

@@ -21,8 +21,10 @@ int spann_scan_blocks_per_sm(bool cosine, int elem, int w) {
     });
 }
 
-cudaError_t launch_spann_scan(const SpannScanParams& p, bool cosine, int elem, int grid, cudaStream_t stream) {
+cudaError_t launch_spann_scan(const SpannScanParams& p, bool cosine, int elem, int grid, cudaStream_t stream,
+                              const void** kernel) {
     return with_cosine_elem(cosine, elem, [&](auto cos, auto el) {
+        *kernel = (const void*)spann_scan_kernel<cos, el>;
         return launch_warp_blocks(spann_scan_kernel<cos, el>, p, grid, spann_scan_smem(p.w), stream);
     });
 }

@@ -186,8 +186,10 @@ int spann_iter_step_blocks_per_sm(bool cosine, int elem, int cap) {
     });
 }
 
-cudaError_t launch_spann_iter_step(const SpannIterParams& p, bool cosine, int elem, int grid, cudaStream_t stream) {
+cudaError_t launch_spann_iter_step(const SpannIterParams& p, bool cosine, int elem, int grid, cudaStream_t stream,
+                                   const void** kernel) {
     return with_cosine_elem(cosine, elem, [&](auto cos, auto el) {
+        *kernel = (const void*)spann_iter_step_kernel<cos, el>;
         return launch_warp_blocks(spann_iter_step_kernel<cos, el>, p, grid, spann_iter_step_smem(p.cap), stream);
     });
 }

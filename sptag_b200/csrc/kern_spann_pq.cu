@@ -70,7 +70,8 @@ int spann_pq_scan_blocks_per_sm(int w, int m) {
     return warp_blocks_per_sm((const void*)spann_pq_scan_kernel, spann_pq_scan_smem(w, m));
 }
 
-cudaError_t launch_spann_pq_scan(const SpannPqScanParams& p, int grid, cudaStream_t stream) {
+cudaError_t launch_spann_pq_scan(const SpannPqScanParams& p, int grid, cudaStream_t stream, const void** kernel) {
+    *kernel = (const void*)spann_pq_scan_kernel;
     return launch_warp_blocks(spann_pq_scan_kernel, p, grid, spann_pq_scan_smem(p.s.w, p.m), stream);
 }
 

@@ -54,8 +54,10 @@ struct SpannScanParams {
 };
 
 // Launches the scan for the index's metric and element type (0 float, 1 int8, 2 uint8, 3 int16) on `stream`.
-// grid: blocks of one warp, each serving queries blockIdx.x, blockIdx.x + grid, ...  Returns the launch error.
-cudaError_t launch_spann_scan(const SpannScanParams& p, bool cosine, int elem, int grid, cudaStream_t stream);
+// grid: blocks of one warp, each serving queries blockIdx.x, blockIdx.x + grid, ...  Returns the launch error; *kernel
+// receives the host stub of the instantiation it launched (B200.LastPostingKernel names it), as do the launchers below.
+cudaError_t launch_spann_scan(const SpannScanParams& p, bool cosine, int elem, int grid, cudaStream_t stream,
+                              const void** kernel);
 // Single-warp blocks of the scan kernel that fit on one SM with W results per query.
 int spann_scan_blocks_per_sm(bool cosine, int elem, int w);
 // Its dynamic shared memory: W result dists, vids and posting ids, three 32-entry chunk arrays and two counters
@@ -74,7 +76,7 @@ struct SpannPqScanParams {
     const float* codebooks;       // ADC: [m x ks x dsub]
     float* adc_tables;            // ADC: per block, the current query's m x ks table
 };
-cudaError_t launch_spann_pq_scan(const SpannPqScanParams& p, int grid, cudaStream_t stream);
+cudaError_t launch_spann_pq_scan(const SpannPqScanParams& p, int grid, cudaStream_t stream, const void** kernel);
 int spann_pq_scan_blocks_per_sm(int w, int m);
 size_t spann_pq_scan_smem(int w, int m);
 
@@ -120,7 +122,8 @@ struct SpannIterParams {
     int* out_counts;
     unsigned char* out_relaxed;
 };
-cudaError_t launch_spann_iter_step(const SpannIterParams& p, bool cosine, int elem, int grid, cudaStream_t stream);
+cudaError_t launch_spann_iter_step(const SpannIterParams& p, bool cosine, int elem, int grid, cudaStream_t stream,
+                                   const void** kernel);
 int spann_iter_step_blocks_per_sm(bool cosine, int elem, int cap);
 
 // Posting lists in pinned host memory (kern_spann_gather.cu).  The packed lists stay where they were loaded (`host`: ids

@@ -410,17 +410,34 @@ Fn pick_iter_step_kernel(const sptag_b200_index* h, const SearchParams& p) {
 }
 
 // The demangled name of a kernel's host launch stub without return type and parameter list, e.g.
-// "sptag_b200::search_kernel<128, false, 16, false, false, 0, 20>"; empty if the stub is not an exported symbol
+// "sptag_b200::search_kernel<128, false, 16, false, false, 0, 20>".  A kernel of internal linkage (the SPANN posting
+// kernels) has no exported stub symbol: its device name comes from the runtime instead, e.g.
+// "sptag_b200::(anonymous namespace)::spann_scan_kernel<false, 2>".  Empty if neither knows the stub.
 std::string kernel_name(const void* stub) {
+    if (!stub) return std::string();
     Dl_info info;
-    if (!stub || !dladdr(stub, &info) || !info.dli_sname || info.dli_saddr != stub) return std::string();
+    const char* mangled = nullptr;
+    if (dladdr(stub, &info) && info.dli_sname && info.dli_saddr == stub)
+        mangled = info.dli_sname;
+    else if (cudaFuncGetName(&mangled, stub) != cudaSuccess || !mangled) {
+        cudaGetLastError();
+        return std::string();
+    }
     int status = 0;
-    char* d = abi::__cxa_demangle(info.dli_sname, nullptr, nullptr, &status);
-    std::string s = (status == 0 && d) ? d : info.dli_sname;
+    char* d = abi::__cxa_demangle(mangled, nullptr, nullptr, &status);
+    std::string s = (status == 0 && d) ? d : mangled;
     free(d);
     if (s.compare(0, 5, "void ") == 0) s.erase(0, 5);
-    const size_t args = s.find('(');  // template arguments are integers and booleans only
-    if (args != std::string::npos) s.erase(args);
+    // the parameter list: the (...) that ends the name ("(anonymous namespace)" may come before it; template arguments
+    // are integers and booleans only)
+    if (!s.empty() && s.back() == ')') {
+        size_t i = s.size(), depth = 0;
+        while (i-- > 0) {
+            if (s[i] == ')') ++depth;
+            else if (s[i] == '(' && --depth == 0) break;
+        }
+        if (i < s.size()) s.erase(i);
+    }
     return s;
 }
 
@@ -2856,6 +2873,8 @@ struct sptag_b200_spann {
     int head_batch = 32;
     int dedup_entries = 0;
     long last_iter_rounds = 0, last_iter_dedup_bytes = 0;
+    // host stub of the last posting-scan or posting-step kernel this handle launched (B200.LastPostingKernel)
+    const void* last_posting_kernel = nullptr;
     DeviceBuffer d_translate, d_off, d_cnt, d_pages, d_ids, d_rows;
     // Host placement (sptag_b200_spann_load_ex): the rows, then the ids, in one pinned mapped allocation, and the HBM stage
     // of each staging set (B200.PostingStageBytes); what the last search or iterator step on this handle gathered
@@ -3024,6 +3043,7 @@ const Param<Spann> kSpannParams[] = {
     {"B200.LastGatherRounds", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_gather_rounds); }},
     {"B200.LastIteratorRounds", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_iter_rounds); }},
     {"B200.LastIteratorDedupBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_iter_dedup_bytes); }},
+    {"B200.LastPostingKernel", [](Spann* s, char* o, size_t n) { return put(o, n, "%s", kernel_name(s->last_posting_kernel).c_str()); }},
 };
 
 // One posting file (OutputSSDIndexFile, ExtraFullGraphSearcher.h:1292-1420; read as LoadingHeadInfo does, :1030-1120):
@@ -3826,6 +3846,7 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     p.out_dists = (float*)st->d_dists.ptr;
     p.out_stats = out_stats ? (int*)st->d_stats.ptr : nullptr;
     pq.s = p;
+    const void* kern = nullptr;
     if (s->host_postings) {
         // the queries' chosen lists, once; then the rounds, each a scan over its queries on the staged lists
         const int stride = std::max(p.internal, 1);
@@ -3854,8 +3875,8 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
             if (r.qcodes) r.qcodes += (size_t)b * r.m;
             if (r.qrot) r.qrot += (size_t)b * r.m * r.dsub;
             const int g = std::min(grid, e - b);
-            const cudaError_t err = s->quantized ? launch_spann_pq_scan(r, g, stream)
-                                                 : launch_spann_scan(r.s, me.cosine, me.elem, g, stream);
+            const cudaError_t err = s->quantized ? launch_spann_pq_scan(r, g, stream, &kern)
+                                                 : launch_spann_scan(r.s, me.cosine, me.elem, g, stream, &kern);
             g_launches++;
             if (err != cudaSuccess) return fail(SPTAG_B200_FAIL, "posting scan launch failed: %s", cudaGetErrorString(err));
             return 0;
@@ -3869,13 +3890,17 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
         s->last_gather_bytes = bytes;
         s->last_gather_rounds = rounds;
     } else {
-        cudaError_t e = s->quantized ? launch_spann_pq_scan(pq, grid, stream)
-                                     : launch_spann_scan(p, me.cosine, me.elem, grid, stream);
+        cudaError_t e = s->quantized ? launch_spann_pq_scan(pq, grid, stream, &kern)
+                                     : launch_spann_scan(p, me.cosine, me.elem, grid, stream, &kern);
         g_launches++;
         if (e != cudaSuccess) {
             cudaStreamSynchronize(stream);
             return fail(SPTAG_B200_FAIL, "posting scan launch failed: %s", cudaGetErrorString(e));
         }
+    }
+    if (kern) {
+        std::lock_guard<std::mutex> lock(s->mu);
+        s->last_posting_kernel = kern;
     }
     CUDA_OK(cudaMemcpyAsync(out_ids, st->d_ids.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaMemcpyAsync(out_dists, st->d_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
@@ -4049,8 +4074,9 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
         CUDA_OK(cudaMemsetAsync(p.susp, 0, kIterListHeader * 4, stream));
         return 0;
     };
+    const void* kern = nullptr;
     auto step = [&](const SpannIterParams& sp_, long long n) -> int {
-        const cudaError_t e = launch_spann_iter_step(sp_, me.cosine, me.elem, (int)std::min(n, max_grid), stream);
+        const cudaError_t e = launch_spann_iter_step(sp_, me.cosine, me.elem, (int)std::min(n, max_grid), stream, &kern);
         g_launches++;
         if (e != cudaSuccess) return fail(SPTAG_B200_FAIL, "posting step launch failed: %s", cudaGetErrorString(e));
         return 0;
@@ -4119,6 +4145,7 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     std::lock_guard<std::mutex> lock(s->mu);
     s->last_iter_rounds = rounds;
     s->last_iter_dedup_bytes = (long)it->dedup.bytes();
+    if (kern) s->last_posting_kernel = kern;
     if (gs) {
         s->last_gather_bytes = gather_bytes;
         s->last_gather_rounds = gather_rounds_n;
