@@ -407,7 +407,9 @@ void sptag_b200_spann_destroy(sptag_b200_spann_handle s);
  *           queries of a posting-step launch of an iterator), n starting at the whole batch and halved (rounded up) until
  *           their union fits; the next round starts from the same n.  The stage is never smaller than one query's worst
  *           case, SearchInternalResultNum x the longest searched list x (row stride + 4) bytes.  MemoryOverFlow when the
- *           pinned allocation fails. */
+ *           pinned allocation fails.  sptag_b200_spann_cache_warm / sptag_b200_spann_cache_lists keep some lists, whole,
+ *           in HBM as well: those are read in place and never copied, and a batch's union and its rounds count the
+ *           other lists only. */
 enum {
     SPTAG_B200_POSTINGS_AUTO = 0,
     SPTAG_B200_POSTINGS_DEVICE = 1,
@@ -490,6 +492,33 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
  * Names are matched case-insensitively, and codes are those of sptag_b200_set_param. */
 int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, const char* value);
 int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char* value_out, int32_t capacity);
+
+/* An HBM cache of posting lists on a handle loaded with the HOST placement.  Ranks the posting lists by how many of
+ * num_queries sample queries choose them, and caches the top of that order in HBM.  Each query runs the head search and
+ * the posting choice of a search with K <= SearchInternalResultNum (W = SearchInternalResultNum), with the search
+ * parameters in force; the lists are counted on the device, ranked by count, descending, then list id, ascending, and
+ * walked in that order: a list is taken when its full size, element count x (row stride + 4) bytes, fits what is left
+ * of budget_bytes, and skipped otherwise.  Lists no query chose are never taken.  budget_bytes -1: cudaMemGetInfo's
+ * free bytes, after the previous cache is released, less the 1 GB reserve of the AUTO placement.  The taken lists are
+ * installed as sptag_b200_spann_cache_lists installs them, and written to out_lists (HOST, NULL when capacity is 0) in
+ * rank order, at most capacity of them; *out_num_lists receives how many were taken.
+ * queries: HOST, as sptag_b200_spann_search's.  Codes as sptag_b200_spann_cache_lists', and LackOfInputs for a null
+ * buffer, a budget below -1 and a page limit that truncates lists of the rearranged layout. */
+int sptag_b200_spann_cache_warm(sptag_b200_spann_handle s, const void* queries, int32_t num_queries,
+                                int64_t budget_bytes, int32_t* out_lists, int32_t capacity, int32_t* out_num_lists);
+/* Caches exactly the given lists in HBM (num_lists = 0 releases the cache), e.g. a set an earlier
+ * sptag_b200_spann_cache_warm returned.  lists: HOST, distinct ids in [0, number of lists).  The call waits until no
+ * search or iterator step runs on the handle (it takes both staging sets), releases the old cache and copies every
+ * element of each list, whatever SearchPostingPageLimit is, from the pinned host allocation into one HBM allocation that
+ * also holds the stage of each staging set.  Searches and iterator steps that start after it returns read the cached
+ * lists in place; iterators opened earlier keep working, with unchanged results.  Results equal the device placement's
+ * bit for bit with any cache.  B200.LastGatherBytes and B200.LastGatherRounds count only what is still copied from host
+ * memory.  A stage that a later call needs to grow (B200.PostingStageBytes, SearchInternalResultNum or the page limit
+ * raised) re-installs the same lists.  Read-only parameters: B200.PostingCacheLists (lists cached) and
+ * B200.PostingCacheBytes (the HBM their rows and ids take).  Device memory: those bytes plus both stages.
+ * Codes: LackOfInputs for a DEVICE-placed handle, an id outside the range, an id given twice and a null buffer;
+ * MemoryOverFlow when the allocation fails, after which the handle works uncached. */
+int sptag_b200_spann_cache_lists(sptag_b200_spann_handle s, const int32_t* lists, int32_t num_lists);
 
 /* Replaces: SPANN::Index<T>::GetIterator(p_target) (SPANNIndex.cpp:299-314) and SPANNResultIterator::Next(batch)
  * (SPANNResultIterator.h:37-63, SPANNIndex.cpp:261-296, :416-446, ExtraFullGraphSearcher.h:131-147, :492-525) for every

@@ -36,7 +36,8 @@ EXPORTS = [
     "sptag_b200_num_deleted", "sptag_b200_spann_load", "sptag_b200_spann_destroy", "sptag_b200_spann_search",
     "sptag_b200_spann_set_param", "sptag_b200_spann_get_param", "sptag_b200_spann_iterator_open",
     "sptag_b200_spann_iterator_next", "sptag_b200_spann_iterator_close", "sptag_b200_multi_scan",
-    "sptag_b200_spann_build", "sptag_b200_debug_kernel_for", "sptag_b200_spann_load_ex",
+    "sptag_b200_spann_build", "sptag_b200_debug_kernel_for", "sptag_b200_spann_load_ex", "sptag_b200_spann_cache_warm",
+    "sptag_b200_spann_cache_lists",
 ]
 
 
@@ -131,6 +132,9 @@ def lib():
         L.sptag_b200_spann_search.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.sptag_b200_spann_set_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p]
         L.sptag_b200_spann_get_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_int32]
+        L.sptag_b200_spann_cache_warm.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
+                                                  C.POINTER(C.c_int32)]
+        L.sptag_b200_spann_cache_lists.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
         L.sptag_b200_spann_iterator_open.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]
         L.sptag_b200_spann_iterator_next.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                      C.c_void_p]
@@ -558,6 +562,29 @@ class B200SpannIndex:
     def iterators(self, queries):
         """SPANN::Index::GetIterator for a batch of HOST queries, one iterator per query."""
         return B200SpannIterators(self, queries)
+
+    def cache_warm(self, queries, budget_bytes=-1):
+        """On a posting_placement="host" handle: caches in HBM the lists the sample HOST queries choose most often, as
+        many as fit budget_bytes (-1: free HBM less 1 GB), and returns them as int32 list ids in rank order
+        (sptag_b200_spann_cache_warm).  cache_lists(ids) installs the same set again later."""
+        queries = np.ascontiguousarray(queries)
+        nq = queries.shape[0]
+        # a query chooses at most SearchInternalResultNum lists, so that many per query bound the taken set
+        cap = max(nq * max(int(self.get_param("SearchInternalResultNum")), 1), 1)
+        out = np.empty(cap, np.int32)
+        n = C.c_int32()
+        _check(lib().sptag_b200_spann_cache_warm(self._h, queries.ctypes.data, nq, int(budget_bytes), out.ctypes.data,
+                                                 cap, C.byref(n)))
+        if n.value > cap:  # SearchInternalResultNum was raised during the call
+            raise RuntimeError("cache_warm installed a cache of %d lists, but only the first %d ids were returned; read "
+                               "them again with a second cache_warm at the same budget" % (n.value, cap))
+        return out[:n.value].copy()
+
+    def cache_lists(self, lists):
+        """On a posting_placement="host" handle: caches exactly these list ids in HBM (empty: releases the cache;
+        sptag_b200_spann_cache_lists)."""
+        lists = np.ascontiguousarray(lists, np.int32)
+        _check(lib().sptag_b200_spann_cache_lists(self._h, lists.ctypes.data, len(lists)))
 
 
 class B200SpannIterators:

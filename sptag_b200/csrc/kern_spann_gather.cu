@@ -1,6 +1,7 @@
 // The gather path of posting lists in pinned host memory (PostingGather, spann_scan.h): which lists a round's queries
 // read, their union and stage offsets, and the copy of their searched prefixes from mapped host memory into the HBM
-// stage that the unchanged scan and posting-step kernels then read.
+// stage that the unchanged scan and posting-step kernels then read; with an HBM cache of lists, the union of the uncached
+// ones only and the view's offsets into the cache and the stage, and the counts that rank lists for the cache.
 #include "spann_device.cuh"
 #include "spann_scan.h"
 
@@ -56,11 +57,31 @@ __global__ void spann_iter_chosen_kernel(const SpannIterParams p, int b, int e, 
     nchosen[i] = max(st.np - st.pi, 0);
 }
 
-__global__ void spann_mark_kernel(const int* chosen, const int* nchosen, int stride, int n, unsigned char* flags) {
+// With a cache (CACHED), only the lists it does not hold join the union
+template <bool CACHED>
+__global__ void spann_mark_kernel(const int* chosen, const int* nchosen, int stride, int n, const long long* resident,
+                                  unsigned char* flags) {
     for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < (long long)n * stride;
          t += (long long)gridDim.x * blockDim.x) {
         const int q = (int)(t / stride), j = (int)(t % stride);
-        if (j < nchosen[q]) flags[chosen[t]] = 1;
+        if (j < nchosen[q] && (!CACHED || resident[chosen[t]] < 0)) flags[chosen[t]] = 1;
+    }
+}
+
+// counts[l] += the items that chose list l
+__global__ void spann_count_kernel(const int* chosen, const int* nchosen, int stride, int n, int* counts) {
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < (long long)n * stride;
+         t += (long long)gridDim.x * blockDim.x) {
+        const int q = (int)(t / stride), j = (int)(t % stride);
+        if (j < nchosen[q]) atomicAdd(&counts[chosen[t]], 1);
+    }
+}
+
+// The view's offsets with a cache: a cached list's first element in the pool, a union list's in this set's stage
+__global__ void spann_view_off_kernel(const PostingGather g) {
+    for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < g.num_lists; l += gridDim.x * blockDim.x) {
+        const long long r = g.resident[l];
+        g.view_off[l] = r >= 0 ? r : g.stage_base + g.stage_off[l];
     }
 }
 
@@ -145,14 +166,27 @@ cudaError_t launch_spann_union(const PostingGather& g, const int* chosen, const 
     if (e != cudaSuccess) return e;
     const long long marks = (long long)n * stride;
     if (marks > 0) {
-        spann_mark_kernel<<<(int)std::min<long long>((marks + 255) / 256, 4096), 256, 0, stream>>>(chosen, nchosen, stride, n,
-                                                                                                  g.flags);
+        const int grid = (int)std::min<long long>((marks + 255) / 256, 4096);
+        if (g.resident)
+            spann_mark_kernel<true><<<grid, 256, 0, stream>>>(chosen, nchosen, stride, n, g.resident, g.flags);
+        else
+            spann_mark_kernel<false><<<grid, 256, 0, stream>>>(chosen, nchosen, stride, n, nullptr, g.flags);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     spann_union_len_kernel<<<std::min((g.num_lists + 256) / 256, 4096), 256, 0, stream>>>(g);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     size_t bytes = g.temp_bytes;
-    return union_cub(g, g.temp, bytes, stream);
+    if ((e = union_cub(g, g.temp, bytes, stream)) != cudaSuccess || !g.resident) return e;
+    spann_view_off_kernel<<<std::min((g.num_lists + 255) / 256, 4096), 256, 0, stream>>>(g);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_spann_count(const int* chosen, const int* nchosen, int stride, int n, int* counts, cudaStream_t stream) {
+    const long long marks = (long long)n * stride;
+    if (marks > 0)
+        spann_count_kernel<<<(int)std::min<long long>((marks + 255) / 256, 4096), 256, 0, stream>>>(chosen, nchosen, stride,
+                                                                                                   n, counts);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_spann_gather(const PostingGather& g, int grid, cudaStream_t stream) {

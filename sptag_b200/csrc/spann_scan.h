@@ -131,6 +131,10 @@ int spann_iter_step_blocks_per_sm(bool cosine, int elem, int cap);
 // lists its queries read is copied into an HBM stage, and the kernels read a PostingLists view of the stage:
 // off = stage_off, ids = stage_ids, rows = stage_rows, cnt and pages unchanged.  A union list keeps its searched prefix
 // (posting_searched at host.page_limit) in the stage.
+// With an HBM cache of lists (sptag_b200_spann_cache_lists), the cached lists, whole, and the stage of each staging set
+// share one allocation and one element space: `resident` holds a cached list's first element there (-1: not cached),
+// the union takes the other lists only, the stage starts at element stage_base (stage_rows / stage_ids point there), and
+// the kernels read a view of the whole allocation with off = view_off.
 struct PostingGather {
     PostingLists host;
     int num_lists;
@@ -144,6 +148,9 @@ struct PostingGather {
     size_t temp_bytes;
     int* stage_ids;
     unsigned char* stage_rows;
+    const long long* resident;  // [num_lists], or nullptr without a cache
+    long long stage_base;
+    long long* view_off;        // [num_lists] with a cache: resident[l], or stage_base + stage_off[l]
 };
 size_t spann_union_temp_bytes(int num_lists);
 // chosen[q * stride ...] / nchosen[q]: the lists query q of a search reads (choose_postings), for every query of p
@@ -154,10 +161,13 @@ cudaError_t launch_spann_choose(const SpannScanParams& p, int* chosen, int* ncho
 cudaError_t launch_spann_iter_chosen(const SpannIterParams& p, int b, int e, int* chosen, int* nchosen, unsigned int* sub,
                                      cudaStream_t stream);
 // The union of the lists of n items (chosen / nchosen as above, stride apart): g.flags, g.len, g.stage_off, g.lists and
-// g.nlists.  g.stage_off[g.num_lists] is the union's element count.
+// g.nlists (and with a cache g.view_off).  g.stage_off[g.num_lists] is the union's element count.
 cudaError_t launch_spann_union(const PostingGather& g, const int* chosen, const int* nchosen, int stride, int n,
                                cudaStream_t stream);
-// Copies the searched prefix of every union list's rows and ids from host memory into the stage
+// Copies g.len[l] elements of every list l of g.lists (the union: its searched prefix) from host memory to element
+// g.stage_off[l] of the stage
 cudaError_t launch_spann_gather(const PostingGather& g, int grid, cudaStream_t stream);
+// counts[l] += the items (chosen / nchosen as above) that read list l
+cudaError_t launch_spann_count(const int* chosen, const int* nchosen, int stride, int n, int* counts, cudaStream_t stream);
 
 }  // namespace sptag_b200

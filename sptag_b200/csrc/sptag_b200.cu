@@ -2885,6 +2885,14 @@ struct sptag_b200_spann {
     const int* h_ids = nullptr;
     int stage_bytes = 256 << 20;
     long last_gather_bytes = 0, last_gather_rounds = 0;
+    // Host placement's HBM cache of lists (sptag_b200_spann_cache_lists): one allocation of cache_pool elements (the cached
+    // lists, whole, in the order given) then cache_stage elements per staging set, their rows at the head's row stride,
+    // then their ids; d_resident: per list, its first element in the pool or -1.  Replaced with both staging sets held;
+    // cache_stage never shrinks, so that a stage a caller fitted before taking its set is still there.  The sizes are
+    // also written under mu, for the parameters.
+    DeviceBuffer d_cache, d_resident;
+    std::vector<int> cache_lists;
+    long long cache_pool = 0, cache_stage = 0, cache_bytes = 0;
     // Host-buffer calls run on one of two staging sets, each with its own stream, head results, dedup tables and outputs,
     // so that two callers overlap; the head search kernels are ordered by the head handle (search_device_impl)
     struct StagingBuffers {
@@ -2892,6 +2900,7 @@ struct sptag_b200_spann {
         DeviceBuffer d_codes, d_adc;  // quantized: the queries' codes (SDC) or rotated vectors (ADC); ADC tables per block
         // host placement: the chosen lists per item, the union (PostingGather), an iterator launch's sub-list, the stage
         DeviceBuffer d_chosen, d_nchosen, d_flags, d_len, d_stage_off, d_union, d_nunion, d_cub, d_sub, d_stage;
+        DeviceBuffer d_view_off;  // with a cache: the view's list offsets
     };
     StagingPool<StagingBuffers> staging;
     std::mutex mu;  // the search parameters
@@ -2902,6 +2911,10 @@ namespace {
 // The page limit a search uses: LoadIndex raises SearchPostingPageLimit to the pages of PostingVectorLimit vectors
 // (ExtraFullGraphSearcher.h:167)
 int spann_page_limit(const sptag_b200_spann* s) { return std::max(s->page_limit, s->vector_limit_pages); }
+
+// HBM that AUTO placement and cache_warm's default budget leave for the searches' buffers (head results, dedup tables,
+// outputs, stages)
+constexpr long long kPostingReserve = 1ll << 30;
 
 // The parameters a SPANN search or iterator step runs with, read together under s->mu
 struct SpannSnapshot {
@@ -2937,6 +2950,13 @@ PostingLists posting_lists(const sptag_b200_spann* s, int page_limit) {
             s->head->row_stride, s->vis, page_limit};
 }
 
+// The elements of a stage: B200.PostingStageBytes, or one query's worst case if larger
+long long stage_elems(const sptag_b200_spann* s, const SpannSnapshot& sp) {
+    const long long elem_bytes = (long long)s->head->row_stride + 4;
+    const long long cap = std::max<long long>(sp.stage_bytes, (long long)std::max(sp.internal, 0) * sp.longest * elem_bytes);
+    return cap / elem_bytes;
+}
+
 // Host placement: runs the n items of a call (the queries of a search, or of an iterator's posting-step launch) in
 // gather rounds on staging set sb.  A round takes the next m items, m starting at n and halved (rounded up) until the
 // union of their lists fits the stage (never below one item), gathers that union into the stage and runs them on it;
@@ -2949,9 +2969,14 @@ int gather_rounds(sptag_b200_spann* s, Buffers& sb, const SpannSnapshot& sp, int
                   Choose&& choose, Run&& run, long& bytes, long& rounds) {
     const PostingLists host = posting_lists(s, sp.page_limit);
     const long long elem_bytes = (long long)host.row_stride + 4;
-    const long long cap = std::max<long long>(sp.stage_bytes, (long long)std::max(sp.internal, 0) * sp.longest * elem_bytes);
-    const long long cap_elems = cap / elem_bytes;
+    const long long cap_elems = stage_elems(s, sp);
     const size_t nl = (size_t)s->num_lists;
+    // the cache cannot change while this caller holds a staging set (spann_cache_install holds both), and
+    // spann_acquire_fitted took the set with a cache stage of at least cap_elems
+    const bool cached = s->d_cache.ptr != nullptr;
+    if (cached && cap_elems > s->cache_stage)
+        return fail(SPTAG_B200_FAIL, "the cache's stage of %lld elements is smaller than the %lld needed", s->cache_stage,
+                    cap_elems);
     const size_t temp = spann_union_temp_bytes(s->num_lists);
     if (temp == 0) return fail(SPTAG_B200_FAIL, "the posting-list union's scratch size query failed");
     if (int rc = sb.d_flags.ensure(nl)) return rc;
@@ -2960,7 +2985,11 @@ int gather_rounds(sptag_b200_spann* s, Buffers& sb, const SpannSnapshot& sp, int
     if (int rc = sb.d_union.ensure(nl * 4 + 4)) return rc;
     if (int rc = sb.d_nunion.ensure(4)) return rc;
     if (int rc = sb.d_cub.ensure(temp)) return rc;
-    if (int rc = sb.d_stage.ensure((size_t)std::max(cap_elems, 1ll) * elem_bytes)) return rc;
+    if (cached) {
+        if (int rc = sb.d_view_off.ensure(nl * 8)) return rc;
+    } else if (int rc = sb.d_stage.ensure((size_t)std::max(cap_elems, 1ll) * elem_bytes)) {
+        return rc;
+    }
     PostingGather g;
     memset(&g, 0, sizeof(g));
     g.host = host;
@@ -2978,6 +3007,19 @@ int gather_rounds(sptag_b200_spann* s, Buffers& sb, const SpannSnapshot& sp, int
     view.off = g.stage_off;
     view.ids = g.stage_ids;
     view.rows = g.stage_rows;
+    if (cached) {  // the pool, then the stage of each staging set, in one element space
+        const long long all = s->cache_pool + 2 * s->cache_stage;
+        unsigned char* rows = (unsigned char*)s->d_cache.ptr;
+        int* ids = (int*)(rows + (size_t)all * host.row_stride);
+        g.resident = (const long long*)s->d_resident.ptr;
+        g.stage_base = s->cache_pool + (long long)(&sb - s->staging.sets) * s->cache_stage;
+        g.view_off = (long long*)sb.d_view_off.ptr;
+        g.stage_rows = rows + (size_t)g.stage_base * host.row_stride;
+        g.stage_ids = ids + g.stage_base;
+        view.off = g.view_off;
+        view.ids = ids;
+        view.rows = rows;
+    }
     const int grid = s->head->num_sms * 4;
     for (int b = 0, m = n; b < n; b += m) {
         m = std::min(m, n - b);
@@ -3016,6 +3058,112 @@ void spann_update_shape(sptag_b200_spann* s) {
     }
 }
 
+// Host placement: both staging sets, so that no search or iterator step runs while the cache changes (in set order, as
+// nothing else holds more than one)
+struct BothSets {
+    std::unique_lock<std::mutex> a, b;
+    explicit BothSets(sptag_b200_spann* s) : a(s->staging.sets[0].mu), b(s->staging.sets[1].mu) {}
+};
+
+// Releases the cache, and the stages of the uncached path (HBM the cache's own stages replace).  Caller holds BothSets.
+void spann_cache_release(sptag_b200_spann* s) {
+    s->d_cache.release();
+    for (auto& set : s->staging.sets) set.d_stage.release();
+    std::lock_guard<std::mutex> lock(s->mu);
+    s->cache_lists.clear();
+    s->cache_pool = s->cache_bytes = 0;
+}
+
+// The copy of spann_cache_install, on the handle's device
+int spann_cache_copy(sptag_b200_spann* s, const std::vector<int>& lists, long long stage) {
+    const size_t nl = (size_t)s->num_lists, rs = s->head->row_stride;
+    stage = std::max({stage, s->cache_stage, 1ll});
+    std::vector<long long> resident(nl, -1), len(nl, 0);
+    long long pool = 0;
+    for (int l : lists) {
+        resident[l] = pool;
+        len[l] = s->cnt[l];
+        pool += s->cnt[l];
+    }
+    const long long all = pool + 2 * stage;
+    if (int rc = s->d_cache.ensure((size_t)all * (rs + 4))) return rc;
+    // the copy's inputs: the lists, their count, each one's length
+    DeviceBuffer d_in;
+    if (int rc = s->d_resident.ensure(nl * 8)) return rc;
+    if (int rc = d_in.ensure(nl * 8 + lists.size() * 4 + 4)) return rc;
+    long long* d_len = (long long*)d_in.ptr;
+    int* d_lists = (int*)(d_len + nl);
+    int* d_n = d_lists + lists.size();
+    const int n = (int)lists.size();
+    CUDA_OK(cudaMemcpy(s->d_resident.ptr, resident.data(), nl * 8, cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(d_len, len.data(), nl * 8, cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(d_lists, lists.data(), lists.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(d_n, &n, 4, cudaMemcpyHostToDevice));
+    PostingGather g;
+    memset(&g, 0, sizeof(g));
+    g.host = posting_lists(s, 0);
+    g.num_lists = s->num_lists;
+    g.len = d_len;
+    g.stage_off = (long long*)s->d_resident.ptr;
+    g.lists = d_lists;
+    g.nlists = d_n;
+    g.stage_rows = (unsigned char*)s->d_cache.ptr;
+    g.stage_ids = (int*)(g.stage_rows + (size_t)all * rs);
+    cudaStream_t stream = s->staging.sets[0].stream;
+    CUDA_OK(launch_spann_gather(g, s->head->num_sms * 4, stream));
+    g_launches++;
+    CUDA_OK(cudaStreamSynchronize(stream));
+    std::lock_guard<std::mutex> lock(s->mu);
+    s->cache_lists = lists;
+    s->cache_pool = pool;
+    s->cache_stage = stage;
+    s->cache_bytes = pool * (long long)(rs + 4);
+    return 0;
+}
+
+// Installs the cache of `lists` (valid, distinct) with stages of at least `stage` elements: releases the old one, then
+// copies every element of each list from mapped host memory into the pool with the gather kernel.  MemoryOverFlow when
+// the allocation fails; the handle is then uncached.  Caller holds BothSets.
+int spann_cache_install(sptag_b200_spann* s, const std::vector<int>& lists, long long stage) {
+    DeviceGuard guard(s->head->device);
+    spann_cache_release(s);
+    if (lists.empty()) return 0;
+    const int rc = spann_cache_copy(s, lists, stage);
+    if (rc) s->d_cache.release();
+    return rc;
+}
+
+// Before a host-placed call takes its staging set: a cache whose stages are smaller than the call's (the stage
+// parameters grew since the install) is re-installed with the call's
+int spann_cache_fit(sptag_b200_spann* s, const SpannSnapshot& sp) {
+    const long long need = stage_elems(s, sp);
+    {
+        std::lock_guard<std::mutex> lock(s->mu);
+        if (s->cache_lists.empty() || s->cache_stage >= need) return 0;
+    }
+    BothSets both(s);
+    std::vector<int> lists;
+    {
+        std::lock_guard<std::mutex> lock(s->mu);
+        if (s->cache_lists.empty() || s->cache_stage >= need) return 0;
+        lists = s->cache_lists;
+    }
+    return spann_cache_install(s, lists, need);
+}
+
+// A host-placed call's staging set, with a cache (if any) whose stages hold the call's stage: the cache is fitted, the
+// set taken, and both again if an install from smaller stage parameters came in between (a cache's stage only grows,
+// so the second fit holds)
+template <typename Set>
+int spann_acquire_fitted(sptag_b200_spann* s, const SpannSnapshot& sp, std::unique_lock<std::mutex>& slock, Set*& set) {
+    for (;;) {
+        if (int rc = spann_cache_fit(s, sp)) return rc;
+        set = s->staging.acquire(slock);
+        if (!s->d_cache.ptr || s->cache_stage >= stage_elems(s, sp)) return 0;  // held set: the cache cannot change
+        slock.unlock();
+    }
+}
+
 // Search parameters (SPANN/ParameterDefinitionList.h:110-125), under s->mu; the kHead ones are set and read on the head
 // (SPANNIndex.cpp:901) without it
 using Spann = sptag_b200_spann;
@@ -3041,6 +3189,9 @@ const Param<Spann> kSpannParams[] = {
     {"B200.PostingHostBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%zu", s->h_posting_bytes); }},
     {"B200.LastGatherBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_gather_bytes); }},
     {"B200.LastGatherRounds", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_gather_rounds); }},
+    // the HBM cache of lists (sptag_b200_spann_cache_lists): its lists and the pool's bytes
+    {"B200.PostingCacheLists", [](Spann* s, char* o, size_t n) { return put(o, n, "%zu", s->cache_lists.size()); }},
+    {"B200.PostingCacheBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%lld", s->cache_bytes); }},
     {"B200.LastIteratorRounds", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_iter_rounds); }},
     {"B200.LastIteratorDedupBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_iter_dedup_bytes); }},
     {"B200.LastPostingKernel", [](Spann* s, char* o, size_t n) { return put(o, n, "%s", kernel_name(s->last_posting_kernel).c_str()); }},
@@ -3151,10 +3302,9 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
     const size_t rows_bytes = ((size_t)total + 1) * rs, ids_bytes = ((size_t)total + 1) * 4;
     if (placement == SPTAG_B200_POSTINGS_AUTO) {
         // HBM when the lists fit beside a reserve for the searches' buffers (head results, dedup tables, outputs)
-        const size_t kReserve = 1ull << 30;
         size_t free_bytes = 0, total_bytes = 0;
         CUDA_OK(cudaMemGetInfo(&free_bytes, &total_bytes));
-        placement = free_bytes >= rows_bytes + ids_bytes + kReserve ? SPTAG_B200_POSTINGS_DEVICE : SPTAG_B200_POSTINGS_HOST;
+        placement = free_bytes >= rows_bytes + ids_bytes + kPostingReserve ? SPTAG_B200_POSTINGS_DEVICE : SPTAG_B200_POSTINGS_HOST;
     }
     unsigned char* rows_base = nullptr;
     int32_t* ids_base = nullptr;
@@ -3770,7 +3920,11 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     while (entries < 2 * reads) entries <<= 1;
     if (entries > (1ll << 30)) return fail(SPTAG_B200_MEMORY_OVERFLOW, "dedup table of %lld entries", entries);
     std::unique_lock<std::mutex> slock;
-    auto* st = s->staging.acquire(slock);
+    decltype(s->staging.acquire(slock)) st = nullptr;
+    if (!s->host_postings)
+        st = s->staging.acquire(slock);
+    else if (int rc = spann_acquire_fitted(s, sp, slock, st))
+        return rc;
     DeviceGuard guard(h->device);
     cudaStream_t stream = st->stream;
     const size_t nq = (size_t)num_queries;
@@ -3923,6 +4077,105 @@ int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char
     if (p && (p->flags & kHead)) return sptag_b200_get_param(s->head, name, value_out, capacity);
     std::lock_guard<std::mutex> lock(s->mu);
     return get_param(s, p, name, value_out, (size_t)capacity);
+}
+
+int sptag_b200_spann_cache_warm(sptag_b200_spann_handle s, const void* queries, int32_t num_queries, int64_t budget_bytes,
+                                int32_t* out_lists, int32_t capacity, int32_t* out_num_lists) {
+    if (!s) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (!s->host_postings) return fail(SPTAG_B200_LACK_OF_INPUTS, "the HBM cache of posting lists needs the host placement");
+    if (num_queries < 0 || (num_queries > 0 && !queries) || !out_num_lists || capacity < 0 || (capacity > 0 && !out_lists))
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    if (budget_bytes < -1) return fail(SPTAG_B200_LACK_OF_INPUTS, "budget %lld below -1", (long long)budget_bytes);
+    *out_num_lists = 0;
+    SpannSnapshot sp;
+    if (int rc = spann_snapshot(s, sp)) return rc;
+    sptag_b200_handle h = s->head;
+    const size_t nl = (size_t)s->num_lists, nq = (size_t)num_queries;
+    // a search's head search and posting choice at K <= SearchInternalResultNum, on staging set 0's buffers
+    const int w = std::max(sp.internal, 1);
+    if (w > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchInternalResultNum %d exceeds 2048", sp.internal);
+    std::vector<int> counts(nl, 0);
+    BothSets both(s);
+    DeviceGuard guard(h->device);
+    auto& st = s->staging.sets[0];
+    cudaStream_t stream = st.stream;
+    if (nq > 0) {
+        DeviceBuffer d_counts;
+        if (int rc = st.d_q.ensure(nq * query_bytes(h))) return rc;
+        if (int rc = st.d_hids.ensure(nq * w * 4)) return rc;
+        if (int rc = st.d_hdists.ensure(nq * w * 4)) return rc;
+        if (int rc = st.d_chosen.ensure(nq * w * 4)) return rc;
+        if (int rc = st.d_nchosen.ensure(nq * 4)) return rc;
+        if (int rc = d_counts.ensure(nl * 4)) return rc;
+        CUDA_OK(cudaMemcpyAsync(st.d_q.ptr, queries, nq * query_bytes(h), cudaMemcpyHostToDevice, stream));
+        {
+            std::lock_guard<std::mutex> lock(h->mu);
+            if (int rc = search_device_impl(h, st.d_q.ptr, num_queries, w, (int*)st.d_hids.ptr, (float*)st.d_hdists.ptr,
+                                            nullptr, stream)) {
+                cudaStreamSynchronize(stream);
+                return rc;
+            }
+        }
+        SpannScanParams p;
+        memset(&p, 0, sizeof(p));
+        p.head_ids = (const int*)st.d_hids.ptr;
+        p.head_dists = (const float*)st.d_hdists.ptr;
+        p.nq = num_queries;
+        p.w = w;
+        p.k = w;
+        p.translate = (const int*)s->d_translate.ptr;
+        p.lists = posting_lists(s, sp.page_limit);
+        p.internal = sp.internal;
+        p.max_dist_ratio = sp.max_dist_ratio;
+        CUDA_OK(cudaMemsetAsync(d_counts.ptr, 0, nl * 4, stream));
+        CUDA_OK(launch_spann_choose(p, (int*)st.d_chosen.ptr, (int*)st.d_nchosen.ptr, w, stream));
+        CUDA_OK(launch_spann_count((const int*)st.d_chosen.ptr, (const int*)st.d_nchosen.ptr, w, num_queries,
+                                   (int*)d_counts.ptr, stream));
+        g_launches += 2;
+        CUDA_OK(cudaMemcpyAsync(counts.data(), d_counts.ptr, nl * 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+    }
+    spann_cache_release(s);
+    long long budget = budget_bytes;
+    if (budget == -1) {
+        size_t free_bytes = 0, total_bytes = 0;
+        CUDA_OK(cudaMemGetInfo(&free_bytes, &total_bytes));
+        budget = std::max(0ll, (long long)free_bytes - kPostingReserve);
+    }
+    // by count, descending, then list id; each list that fits what is left of the budget, whole
+    std::vector<int> order;
+    for (size_t l = 0; l < nl; ++l)
+        if (counts[l] > 0) order.push_back((int)l);
+    std::sort(order.begin(), order.end(), [&](int a, int b) { return counts[a] != counts[b] ? counts[a] > counts[b] : a < b; });
+    const long long elem_bytes = (long long)h->row_stride + 4;
+    std::vector<int> taken;
+    for (int l : order) {
+        const long long bytes = (long long)s->cnt[l] * elem_bytes;
+        if (bytes > budget) continue;
+        taken.push_back(l);
+        budget -= bytes;
+    }
+    if (int rc = spann_cache_install(s, taken, stage_elems(s, sp))) return rc;
+    *out_num_lists = (int32_t)taken.size();
+    std::copy_n(taken.begin(), std::min<size_t>(taken.size(), (size_t)capacity), out_lists);
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_spann_cache_lists(sptag_b200_spann_handle s, const int32_t* lists, int32_t num_lists) {
+    if (!s) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (!s->host_postings) return fail(SPTAG_B200_LACK_OF_INPUTS, "the HBM cache of posting lists needs the host placement");
+    if (num_lists < 0 || (num_lists > 0 && !lists)) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    std::vector<char> seen((size_t)s->num_lists, 0);
+    for (int32_t i = 0; i < num_lists; ++i) {
+        const int l = lists[i];
+        if (l < 0 || l >= s->num_lists) return fail(SPTAG_B200_LACK_OF_INPUTS, "list %d outside [0, %d)", l, s->num_lists);
+        if (seen[l]) return fail(SPTAG_B200_LACK_OF_INPUTS, "list %d given twice", l);
+        seen[l] = 1;
+    }
+    SpannSnapshot sp;
+    spann_snapshot(s, sp);  // fills sp whether or not the page limit would refuse a search
+    BothSets both(s);
+    return spann_cache_install(s, std::vector<int>(lists, lists + num_lists), stage_elems(s, sp));
 }
 
 }  // extern "C"
@@ -4084,7 +4337,9 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     // Host placement: a staging set for the call, whose stage each launch's rounds fill (gather_rounds over the launch's
     // queries, each round a launch over its sub-list)
     std::unique_lock<std::mutex> slock;
-    auto* gs = s->host_postings ? s->staging.acquire(slock) : nullptr;
+    decltype(s->staging.acquire(slock)) gs = nullptr;
+    if (s->host_postings)
+        if (int rc = spann_acquire_fitted(s, sp, slock, gs)) return rc;
     long gather_bytes = 0, gather_rounds_n = 0;
     if (gs) {
         if (int rc = gs->d_chosen.ensure(nq * it->hb * 4)) return rc;
