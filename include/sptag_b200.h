@@ -454,6 +454,50 @@ int sptag_b200_spann_load_ex(const char* folder, int32_t device, const sptag_b20
 int sptag_b200_spann_build(const char* folder, const void* vectors, int32_t num, int32_t dim, int32_t normalized,
                            int32_t device, int64_t* out_stats);
 
+/* sptag_b200_spann_build for vector sets whose rows or edges do not fit the device.  device_budget_bytes: the device bytes
+ * the call may allocate beyond the head index (and beyond what the head search allocates, as in every search); -1:
+ * cudaMemGetInfo's free bytes after the head is loaded, less 1 GB (AUTO's reserve, sptag_b200_spann_load_ex). */
+typedef struct {
+    int32_t struct_size;          /* sizeof(sptag_b200_spann_build_options) */
+    int64_t device_budget_bytes;  /* >= -1 */
+} sptag_b200_spann_build_options;
+
+/* sptag_b200_spann_build with a device budget (options NULL: budget -1).  The same arguments, ini keys and refusals; the
+ * files are the same byte for byte, whichever path runs.  Fail for a struct_size other than
+ * sizeof(sptag_b200_spann_build_options), LackOfInputs for a budget below -1.
+ * Path: the resident path (sptag_b200_spann_build's) runs when num x ReplicaCount <= 2^31 - 1 and its working set fits
+ * the budget: num x dim x sizeof(T) (the rows) + 24 x num x ReplicaCount (the edges) + the radix sort's scratch for them
+ * + min(num, 65536) x InternalResultNum x 8 (one search batch of results) + 64 MB (the window).  Otherwise the streamed
+ * path runs:
+ *   The caller's rows stay where they are: the buffer is registered (cudaHostRegisterMapped; one registered before is
+ *   used as it is) for the call and never written.  Pass 1 copies batches of B rows into two HBM batch buffers (batch
+ *   i + 1's copy overlaps batch i's search), checks and normalises them as the resident path does, searches the head,
+ *   runs the RNG selection and appends the filled edges, in vector-id order, to a pinned host edge store of 12 B per
+ *   edge (keys and vector ids, room for every non-head vector x min(ReplicaCount, InternalResultNum, head count)).  B is
+ *   65536 (at most num), halved while pass 1's device bytes exceed the budget:
+ *     P1(B) = B x (2 x row + 5 + 8 x InternalResultNum + 25 x ReplicaCount) + the selection's scratch for B x
+ *             ReplicaCount edges + 4 x heads + 40,  row = dim x sizeof(T).
+ *   Pass 2 cuts each file's lists, in placement order, into groups (never across files, at least one list each) and
+ *   per group streams the whole edge store through HBM in chunks of C edges, keeps the group's edges, sorts them,
+ *   gathers the rows of the kept elements from the caller's buffer and writes the group's part of the file.  Its
+ *   device bytes are F(C) + the largest group's G:
+ *     F(C) = 25 x C + the selection's scratch for C edges + 32 + 4 x heads + 28 x (lists of the largest file) + the
+ *            window, min(64 MB, the largest file's list area);
+ *     G    = a(8E) x 2 + a(4E) x 2 + a(the radix sort's scratch for E edges) + a(kept elements x row), for a group of
+ *            E edges before the cut, a(x) = x rounded up to 256.
+ *   C is min(edges, 2^22), halved while F(C) + G(the longest list) exceeds the budget, never below min(edges, 4096);
+ *   a group then takes lists while its G fits budget - F(C).  Every group costs one pass over the store:
+ *   groups x 12 B x edges host to device.
+ * MemoryOverFlow, before any posting file is created: a budget below the streamed path's minimum, the larger of P1(1)
+ * and F(min(edges, 4096)) + G(the longest list) (the two passes never hold their buffers at once; the message names
+ * the minimum), or a pinned edge store that cannot be allocated.
+ * out_stats: HOST int64[12] or NULL: sptag_b200_spann_build's 8 (on the streamed path the sort is every group's, and the
+ * write's host microseconds are pass 2's other work: edge passes, gathers, images and fwrite), then the path (0
+ * resident, 1 streamed), the row batches, the edge groups (1 on the resident path) and the bytes copied host to device
+ * (rows, edge passes and gathered rows). */
+int sptag_b200_spann_build_ex(const char* folder, const void* vectors, int32_t num, int32_t dim, int32_t normalized,
+                              int32_t device, const sptag_b200_spann_build_options* options, int64_t* out_stats);
+
 /* Replaces: SPANN::Index<T>::SearchIndex(QueryResult&) (SPANNIndex.cpp:193-250) with ExtraFullGraphSearcher::SearchIndex
  * (ExtraFullGraphSearcher.h:226-375) for a batch.  The head search runs at W = max(K, SearchInternalResultNum); the
  * postings are chosen from its results, the result array is reversed, every chosen list is scanned in order with the

@@ -37,7 +37,7 @@ EXPORTS = [
     "sptag_b200_spann_set_param", "sptag_b200_spann_get_param", "sptag_b200_spann_iterator_open",
     "sptag_b200_spann_iterator_next", "sptag_b200_spann_iterator_close", "sptag_b200_multi_scan",
     "sptag_b200_spann_build", "sptag_b200_debug_kernel_for", "sptag_b200_spann_load_ex", "sptag_b200_spann_cache_warm",
-    "sptag_b200_spann_cache_lists",
+    "sptag_b200_spann_cache_lists", "sptag_b200_spann_build_ex",
 ]
 
 
@@ -57,6 +57,10 @@ class SearchOptions(C.Structure):
 
 class SpannLoadOptions(C.Structure):
     _fields_ = [("struct_size", C.c_int32), ("posting_placement", C.c_int32)]
+
+
+class SpannBuildOptions(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("device_budget_bytes", C.c_int64)]
 
 
 # sptag_b200_spann_load_ex's posting_placement (SPTAG_B200_POSTINGS_*)
@@ -129,6 +133,8 @@ def lib():
         L.sptag_b200_spann_destroy.restype = None
         L.sptag_b200_spann_build.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                              C.c_void_p]
+        L.sptag_b200_spann_build_ex.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                C.POINTER(SpannBuildOptions), C.c_void_p]
         L.sptag_b200_spann_search.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.sptag_b200_spann_set_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p]
         L.sptag_b200_spann_get_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_int32]
@@ -512,19 +518,31 @@ class B200SpannIndex:
 
     BUILD_STATS = ("searched", "rng_rejected", "edges_before_cut", "edges_after_cut", "search_us", "rng_us", "sort_us",
                    "write_us")
+    # sptag_b200_spann_build_ex's: BUILD_STATS, the path (0 resident, 1 streamed), the row batches, the edge groups and
+    # the bytes copied host to device
+    BUILD_STATS_EX = BUILD_STATS + ("streamed", "row_batches", "edge_groups", "h2d_bytes")
 
     @classmethod
-    def build(cls, folder, vectors, normalized=False, device=-1, stats=None):
+    def build(cls, folder, vectors, normalized=False, device=-1, stats=None, budget_bytes=None):
         """The SSD stage of SPANN::Index::BuildIndex (SelectHead and BuildHead off) on the device: writes the posting
         files of `folder`, whose head is already built, from HOST vectors (row i is vector id i), and returns
-        load(folder, device).  If `stats` is a dict it receives BUILD_STATS."""
+        load(folder, device).  budget_bytes: None (sptag_b200_spann_build: rows and edges in HBM), or the device bytes
+        the build may use (sptag_b200_spann_build_ex, -1: free HBM less 1 GB), which streams rows and edges from host
+        memory when they do not fit.  If `stats` is a dict it receives BUILD_STATS, or BUILD_STATS_EX with a budget."""
         vectors = np.ascontiguousarray(vectors)
-        out = np.zeros(len(cls.BUILD_STATS), np.int64)
-        _check(lib().sptag_b200_spann_build(os.fsencode(folder), vectors.ctypes.data, vectors.shape[0],
-                                            vectors.shape[1] if vectors.ndim == 2 else 0, int(bool(normalized)), device,
-                                            out.ctypes.data))
+        args = (os.fsencode(folder), vectors.ctypes.data, vectors.shape[0], vectors.shape[1] if vectors.ndim == 2 else 0,
+                int(bool(normalized)), device)
+        if budget_bytes is None:
+            names = cls.BUILD_STATS
+            out = np.zeros(len(names), np.int64)
+            _check(lib().sptag_b200_spann_build(*args, out.ctypes.data))
+        else:
+            names = cls.BUILD_STATS_EX
+            out = np.zeros(len(names), np.int64)
+            o = SpannBuildOptions(C.sizeof(SpannBuildOptions), int(budget_bytes))
+            _check(lib().sptag_b200_spann_build_ex(*args, C.byref(o), out.ctypes.data))
         if stats is not None:
-            stats.update(zip(cls.BUILD_STATS, out.tolist()))
+            stats.update(zip(names, out.tolist()))
         return cls.load(folder, device)
 
     def close(self):

@@ -6,6 +6,7 @@
 #include "spann_device.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_select.cuh>
 
 namespace sptag_b200 {
 namespace {
@@ -75,8 +76,10 @@ __global__ void spann_nonfinite_kernel(const float* __restrict__ v, size_t n, in
         if (!isfinite(v[i])) *bad = 1;
 }
 
-// One block per list that overlaps the window, one byte per thread and step
-__global__ void __launch_bounds__(256) spann_posting_image_kernel(const SpannImageParams p) {
+// One block per list that overlaps the window, one byte per thread and step.  GATHERED: element e of list l reads its row
+// from row row_off[l] + e of the gathered rows, not from the vector's own row
+template <bool GATHERED>
+__device__ __forceinline__ void posting_image(const SpannImageParams& p) {
     const long long rb = p.row_bytes, vis = rb + 4;
     for (int li = blockIdx.x; li < p.num_lists; li += gridDim.x) {
         const int l = p.first_list + li;
@@ -98,8 +101,46 @@ __global__ void __launch_bounds__(256) spann_posting_image_kernel(const SpannIma
                 if (!id) at -= 4;
             }
             const int vec = ton[e];
-            p.out[b - p.win_begin] = id ? (unsigned char)((unsigned int)vec >> (8 * at))
-                                        : p.rows[(size_t)vec * rb + at];
+            const size_t row = GATHERED ? (size_t)(p.row_off[l] + e) : (size_t)vec;
+            p.out[b - p.win_begin] = id ? (unsigned char)((unsigned int)vec >> (8 * at)) : p.rows[row * rb + at];
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) spann_posting_image_kernel(const SpannImageParams p) { posting_image<false>(p); }
+__global__ void __launch_bounds__(256) spann_posting_image_gathered_kernel(const SpannImageParams p) { posting_image<true>(p); }
+
+// One thread per edge: flags[i] = the edge is kept.  group_of == nullptr: the edge is filled (node < num_heads), and
+// tonode[i] += tonode_add; otherwise: its list belongs to `group`
+__global__ void spann_edge_flag_kernel(const unsigned long long* __restrict__ keys, int* __restrict__ tonode, int n,
+                                       int tonode_add, int num_heads, const int* __restrict__ group_of, int group,
+                                       unsigned char* __restrict__ flags) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int node = (int)(keys[i] >> 32);
+    if (group_of) {
+        flags[i] = group_of[node] == group;
+    } else {
+        flags[i] = node < num_heads;
+        tonode[i] += tonode_add;
+    }
+}
+
+// One block per list, one word of W per thread and step: the list's first count[l] sorted edges' rows, from src (row
+// tonode[e], row_bytes apart) to dst (row row_off[l] + e)
+template <typename W>
+__global__ void __launch_bounds__(256) spann_row_gather_kernel(const SpannGatherParams p) {
+    const int wpr = p.row_bytes / (int)sizeof(W);
+    const W* src = reinterpret_cast<const W*>(p.src);
+    W* dst = reinterpret_cast<W*>(p.dst);
+    for (int li = blockIdx.x; li < p.num_lists; li += gridDim.x) {
+        const int l = p.first_list + li;
+        const int* ton = p.tonode + p.edge_off[l];
+        W* out = dst + (size_t)p.row_off[l] * wpr;
+        const long long words = (long long)p.count[l] * wpr;
+        for (long long t = threadIdx.x; t < words; t += blockDim.x) {
+            const long long e = t / wpr;
+            out[t] = src[(size_t)ton[e] * wpr + (t - e * wpr)];
         }
     }
 }
@@ -130,7 +171,48 @@ cudaError_t spann_sort_edges(void* temp, size_t* temp_bytes, const unsigned long
 
 cudaError_t launch_spann_posting_image(const SpannImageParams& p, cudaStream_t stream) {
     if (p.num_lists <= 0) return cudaSuccess;
-    spann_posting_image_kernel<<<(unsigned)std::min(p.num_lists, 65535), 256, 0, stream>>>(p);
+    if (p.row_off)
+        spann_posting_image_gathered_kernel<<<(unsigned)std::min(p.num_lists, 65535), 256, 0, stream>>>(p);
+    else
+        spann_posting_image_kernel<<<(unsigned)std::min(p.num_lists, 65535), 256, 0, stream>>>(p);
+    return cudaGetLastError();
+}
+
+cudaError_t spann_select_edges(void* temp, size_t* temp_bytes, const unsigned long long* keys, int* tonode, int n,
+                               int tonode_add, int num_heads, const int* group_of, int group, unsigned char* flags,
+                               unsigned long long* keys_out, int* tonode_out, int* num_selected, cudaStream_t stream) {
+    if (!temp) {
+        size_t a = 0, b = 0;
+        cudaError_t e = cub::DeviceSelect::Flagged(nullptr, a, keys, flags, keys_out, num_selected, n, stream);
+        if (e == cudaSuccess) e = cub::DeviceSelect::Flagged(nullptr, b, tonode, flags, tonode_out, num_selected, n, stream);
+        *temp_bytes = std::max(a, b);
+        return e;
+    }
+    if (n <= 0) return cudaMemsetAsync(num_selected, 0, 4, stream);
+    spann_edge_flag_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(keys, tonode, n, tonode_add, num_heads, group_of,
+                                                                           group, flags);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cub::DeviceSelect::Flagged(temp, *temp_bytes, keys, flags, keys_out, num_selected, n, stream);
+    if (e == cudaSuccess)
+        e = cub::DeviceSelect::Flagged(temp, *temp_bytes, (const int*)tonode, flags, tonode_out, num_selected, n, stream);
+    return e;
+}
+
+cudaError_t launch_spann_row_gather(const SpannGatherParams& p, cudaStream_t stream) {
+    if (p.num_lists <= 0) return cudaSuccess;
+    const unsigned grid = (unsigned)std::min(p.num_lists, 65535);
+    // the widest word that divides the row size and both bases' alignment
+    const size_t align = (size_t)p.row_bytes | (size_t)(uintptr_t)p.src | (size_t)(uintptr_t)p.dst;
+    if (align % 16 == 0)
+        spann_row_gather_kernel<uint4><<<grid, 256, 0, stream>>>(p);
+    else if (align % 8 == 0)
+        spann_row_gather_kernel<uint2><<<grid, 256, 0, stream>>>(p);
+    else if (align % 4 == 0)
+        spann_row_gather_kernel<unsigned int><<<grid, 256, 0, stream>>>(p);
+    else if (align % 2 == 0)
+        spann_row_gather_kernel<unsigned short><<<grid, 256, 0, stream>>>(p);
+    else
+        spann_row_gather_kernel<unsigned char><<<grid, 256, 0, stream>>>(p);
     return cudaGetLastError();
 }
 

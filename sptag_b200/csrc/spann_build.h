@@ -54,7 +54,32 @@ struct SpannImageParams {
     int row_bytes, rearranged;
     long long win_begin, win_end;
     unsigned char* out;
+    const long long* row_off;   // nullptr: element e of list l is row tonode[edge_off[l] + e] of `rows`; otherwise row
+                                // row_off[l] + e (the rows a group gathered, sptag_b200_spann_build_ex's streamed path)
 };
 cudaError_t launch_spann_posting_image(const SpannImageParams& p, cudaStream_t stream);
+
+// The order-preserving selection of n edges (keys, tonode) into keys_out / tonode_out, *num_selected (device) their
+// count: group_of == nullptr keeps the filled edges (node < num_heads) and first adds tonode_add to every tonode in
+// place; otherwise it keeps the edges whose list l has group_of[l] == group.  flags: n bytes of scratch.
+// temp == nullptr: *temp_bytes receives the scratch size.
+cudaError_t spann_select_edges(void* temp, size_t* temp_bytes, const unsigned long long* keys, int* tonode, int n,
+                               int tonode_add, int num_heads, const int* group_of, int group, unsigned char* flags,
+                               unsigned long long* keys_out, int* tonode_out, int* num_selected, cudaStream_t stream);
+
+// The rows of lists [first_list, first_list + num_lists) of a group: list l's first count[l] sorted edges
+// tonode[edge_off[l]], ... name rows of src (row_bytes apart, unpadded; mapped host memory), copied to dst rows
+// row_off[l], ... with the widest word that the row size and both bases' alignment allow
+struct SpannGatherParams {
+    const long long* edge_off;
+    const long long* row_off;
+    const int* count;
+    int first_list, num_lists;
+    const int* tonode;
+    const unsigned char* src;
+    int row_bytes;
+    unsigned char* dst;
+};
+cudaError_t launch_spann_row_gather(const SpannGatherParams& p, cudaStream_t stream);
 
 }  // namespace sptag_b200

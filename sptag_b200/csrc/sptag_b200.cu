@@ -3442,122 +3442,189 @@ struct SpannBuildFile {
     int row_bytes, rearranged, num_vectors, dim;
     const std::vector<long long>* edge_off;  // per list: its first sorted edge
     const std::vector<int>* count;           // per list: its elements after the cut
+    const std::vector<long long>* row_off;   // nullptr, or per list: its first row of d_rows (gathered rows)
 };
-int write_posting_file(const SpannBuildFile& b, const std::string& path, int first, int nl, cudaStream_t stream) {
+
+// A file's placement: its lists in placement order (file-local ids), where each starts in the list area, the area's
+// size (the last list's end, padded to a page) and the header
+struct SpannFileLayout {
+    std::vector<int> order;
+    std::vector<long long> start, bytes;
+    std::vector<unsigned char> hdr;
+    long long area = 0;
+};
+void spann_file_layout(const SpannBuildFile& b, int first, int nl, SpannFileLayout& L) {
     const long long vis = b.row_bytes + 4;
-    std::vector<long long> bytes((size_t)nl);
-    for (int i = 0; i < nl; ++i) bytes[i] = (long long)(*b.count)[first + i] * vis;
-    std::vector<int> page_num, page_off, order;
-    select_posting_offset(bytes, page_num, page_off, order);
+    L.bytes.assign((size_t)nl, 0);
+    for (int i = 0; i < nl; ++i) L.bytes[i] = (long long)(*b.count)[first + i] * vis;
+    std::vector<int> page_num, page_off;
+    select_posting_offset(L.bytes, page_num, page_off, L.order);
     // header: list count, vector count, dimension, the list area's first page; per list page, offset, count, pages
     const size_t meta = 16 + 12 * (size_t)nl;
-    std::vector<unsigned char> hdr(round_up(meta, 4096), 0);
-    const int32_t h4[4] = {nl, b.num_vectors, b.dim, (int32_t)(hdr.size() / 4096)};
-    memcpy(hdr.data(), h4, 16);
+    L.hdr.assign(round_up(meta, 4096), 0);
+    const int32_t h4[4] = {nl, b.num_vectors, b.dim, (int32_t)(L.hdr.size() / 4096)};
+    memcpy(L.hdr.data(), h4, 16);
     for (int i = 0; i < nl; ++i) {
-        unsigned char* e = hdr.data() + 16 + 12 * (size_t)i;
-        const int32_t pn = bytes[i] ? page_num[i] : 0, ele = (*b.count)[first + i];
-        const uint16_t po = bytes[i] ? (uint16_t)page_off[i] : 0, pc = (uint16_t)((bytes[i] + 4095) / 4096);
+        unsigned char* e = L.hdr.data() + 16 + 12 * (size_t)i;
+        const int32_t pn = L.bytes[i] ? page_num[i] : 0, ele = (*b.count)[first + i];
+        const uint16_t po = L.bytes[i] ? (uint16_t)page_off[i] : 0, pc = (uint16_t)((L.bytes[i] + 4095) / 4096);
         memcpy(e, &pn, 4);
         memcpy(e + 4, &po, 2);
         memcpy(e + 6, &ele, 4);
         memcpy(e + 10, &pc, 2);
     }
-    // the lists in placement order (ascending start), and the list area's size: the last list's end, padded to a page
-    std::vector<long long> start, eoff;
-    std::vector<int> cnt;
-    for (int id : order) {
-        start.push_back((long long)page_num[id] * 4096 + page_off[id]);
-        eoff.push_back((*b.edge_off)[first + id]);
-        cnt.push_back((*b.count)[first + id]);
-    }
-    const long long area = order.empty() ? 0 : (long long)round_up((size_t)(start.back() + bytes[order.back()]), 4096);
-    FILE* f = std::fopen(path.c_str(), "wb");
-    if (!f) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot write %s", path.c_str());
-    std::unique_ptr<FILE, int (*)(FILE*)> closer(f, std::fclose);
-    if (std::fwrite(hdr.data(), 1, hdr.size(), f) != hdr.size()) return fail(SPTAG_B200_FAIL, "writing %s failed", path.c_str());
-    if (area == 0) return 0;
-    const long long kWindow = 64ll << 20;
-    const size_t win = (size_t)std::min(kWindow, area);
-    DeviceBuffer d_start, d_eoff, d_cnt, d_win;
-    if (int rc = d_start.ensure(start.size() * 8)) return rc;
-    if (int rc = d_eoff.ensure(eoff.size() * 8)) return rc;
-    if (int rc = d_cnt.ensure(cnt.size() * 4)) return rc;
-    if (int rc = d_win.ensure(win)) return rc;
-    CUDA_OK(cudaMemcpyAsync(d_start.ptr, start.data(), start.size() * 8, cudaMemcpyHostToDevice, stream));
-    CUDA_OK(cudaMemcpyAsync(d_eoff.ptr, eoff.data(), eoff.size() * 8, cudaMemcpyHostToDevice, stream));
-    CUDA_OK(cudaMemcpyAsync(d_cnt.ptr, cnt.data(), cnt.size() * 4, cudaMemcpyHostToDevice, stream));
-    struct Pinned {
-        void* p[2] = {nullptr, nullptr};
-        cudaEvent_t ev[2] = {nullptr, nullptr};
-        ~Pinned() {
-            for (int i = 0; i < 2; ++i) {
-                if (p[i]) cudaFreeHost(p[i]);
-                if (ev[i]) cudaEventDestroy(ev[i]);
-            }
-        }
-    } pin;
-    for (int i = 0; i < 2; ++i) {
-        if (cudaMallocHost(&pin.p[i], win) != cudaSuccess)
-            return fail(SPTAG_B200_MEMORY_OVERFLOW, "pinned window buffer (%zu bytes) failed", win);
-        CUDA_OK(cudaEventCreateWithFlags(&pin.ev[i], cudaEventDisableTiming));
-    }
-    SpannImageParams p;
-    memset(&p, 0, sizeof(p));
-    p.start = (const long long*)d_start.ptr;
-    p.edge_off = (const long long*)d_eoff.ptr;
-    p.count = (const int*)d_cnt.ptr;
-    p.tonode = b.d_tonode;
-    p.rows = b.d_rows;
-    p.row_bytes = b.row_bytes;
-    p.rearranged = b.rearranged;
-    p.out = (unsigned char*)d_win.ptr;
-    size_t lo = 0;  // the first list that ends after the window's start
-    long long pending = -1;  // the window waiting for its fwrite (its buffer: pending & 1)
-    auto flush = [&](long long w) -> int {
-        CUDA_OK(cudaEventSynchronize(pin.ev[w & 1]));
-        const size_t n = (size_t)std::min(kWindow, area - w * kWindow);
-        if (std::fwrite(pin.p[w & 1], 1, n, f) != n) return fail(SPTAG_B200_FAIL, "writing %s failed", path.c_str());
-        return 0;
-    };
-    for (long long w = 0; w * kWindow < area; ++w) {
-        p.win_begin = w * kWindow;
-        p.win_end = std::min(area, p.win_begin + kWindow);
-        while (lo < start.size() && start[lo] + (long long)cnt[lo] * vis <= p.win_begin) ++lo;
-        size_t hi = lo;
-        while (hi < start.size() && start[hi] < p.win_end) ++hi;
-        p.first_list = (int)lo;
-        p.num_lists = (int)(hi - lo);
-        CUDA_OK(cudaMemsetAsync(d_win.ptr, 0, (size_t)(p.win_end - p.win_begin), stream));
-        CUDA_OK(launch_spann_posting_image(p, stream));
-        g_launches++;
-        CUDA_OK(cudaMemcpyAsync(pin.p[w & 1], d_win.ptr, (size_t)(p.win_end - p.win_begin), cudaMemcpyDeviceToHost, stream));
-        CUDA_OK(cudaEventRecord(pin.ev[w & 1], stream));
-        if (pending >= 0)
-            if (int rc = flush(pending)) return rc;
-        pending = w;
-    }
-    if (int rc = flush(pending)) return rc;
-    if (std::fflush(f) != 0) return fail(SPTAG_B200_FAIL, "writing %s failed", path.c_str());
-    return 0;
+    L.start.clear();
+    for (int id : L.order) L.start.push_back((long long)page_num[id] * 4096 + page_off[id]);
+    L.area = L.order.empty() ? 0 : (long long)round_up((size_t)(L.start.back() + L.bytes[L.order.back()]), 4096);
 }
 
-// Owns what one sptag_b200_spann_build call allocates on the device and its stream; frees them with the device current
+// Writes one file: open() writes the header and uploads the placed lists' start, edge offset, count (and row offset);
+// write() images and writes the list area's bytes [begin, end) in windows of at most kWindow bytes from the sorted
+// edges and rows given; finish() writes the last window.  The areas of successive write() calls follow each other.
+struct SpannFileWriter {
+    static constexpr long long kWindow = 64ll << 20;
+    const SpannBuildFile* b = nullptr;
+    const SpannFileLayout* L = nullptr;
+    std::string path;
+    cudaStream_t stream = nullptr;
+    std::unique_ptr<FILE, int (*)(FILE*)> f{nullptr, std::fclose};
+    std::vector<int> cnt;  // per placed list
+    DeviceBuffer d_start, d_eoff, d_cnt, d_roff, d_win;
+    void* pin[2] = {nullptr, nullptr};
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    SpannImageParams p;
+    size_t lo = 0;           // the first list that ends after the window's start
+    long long next = 0;      // the next window's number (its buffer: number & 1)
+    long long pending = -1;  // the window waiting for its fwrite
+    long long pending_bytes = 0;
+    ~SpannFileWriter() {
+        for (int i = 0; i < 2; ++i) {
+            if (pin[i]) cudaFreeHost(pin[i]);
+            if (ev[i]) cudaEventDestroy(ev[i]);
+        }
+    }
+    // the window size: an upper bound of the device bytes the writer allocates besides the per-list arrays
+    static long long window_bytes(long long area) { return std::min(kWindow, area); }
+    int open(const SpannBuildFile& bf, const SpannFileLayout& lay, const std::string& file_path, int first, cudaStream_t s) {
+        b = &bf;
+        L = &lay;
+        path = file_path;
+        stream = s;
+        FILE* fp = std::fopen(path.c_str(), "wb");
+        if (!fp) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot write %s", path.c_str());
+        f.reset(fp);
+        if (std::fwrite(L->hdr.data(), 1, L->hdr.size(), fp) != L->hdr.size())
+            return fail(SPTAG_B200_FAIL, "writing %s failed", path.c_str());
+        if (L->area == 0) return 0;
+        std::vector<long long> eoff, roff;
+        for (int id : L->order) {
+            eoff.push_back((*b->edge_off)[first + id]);
+            cnt.push_back((*b->count)[first + id]);
+            if (b->row_off) roff.push_back((*b->row_off)[first + id]);
+        }
+        const size_t win = (size_t)window_bytes(L->area);
+        if (int rc = d_start.ensure(L->start.size() * 8)) return rc;
+        if (int rc = d_eoff.ensure(eoff.size() * 8)) return rc;
+        if (int rc = d_cnt.ensure(cnt.size() * 4)) return rc;
+        if (b->row_off)
+            if (int rc = d_roff.ensure(roff.size() * 8)) return rc;
+        if (int rc = d_win.ensure(win)) return rc;
+        CUDA_OK(cudaMemcpyAsync(d_start.ptr, L->start.data(), L->start.size() * 8, cudaMemcpyHostToDevice, stream));
+        CUDA_OK(cudaMemcpyAsync(d_eoff.ptr, eoff.data(), eoff.size() * 8, cudaMemcpyHostToDevice, stream));
+        CUDA_OK(cudaMemcpyAsync(d_cnt.ptr, cnt.data(), cnt.size() * 4, cudaMemcpyHostToDevice, stream));
+        if (b->row_off) CUDA_OK(cudaMemcpyAsync(d_roff.ptr, roff.data(), roff.size() * 8, cudaMemcpyHostToDevice, stream));
+        for (int i = 0; i < 2; ++i) {
+            if (cudaMallocHost(&pin[i], win) != cudaSuccess)
+                return fail(SPTAG_B200_MEMORY_OVERFLOW, "pinned window buffer (%zu bytes) failed", win);
+            CUDA_OK(cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
+        }
+        memset(&p, 0, sizeof(p));
+        p.start = (const long long*)d_start.ptr;
+        p.edge_off = (const long long*)d_eoff.ptr;
+        p.count = (const int*)d_cnt.ptr;
+        p.row_off = b->row_off ? (const long long*)d_roff.ptr : nullptr;
+        p.row_bytes = b->row_bytes;
+        p.rearranged = b->rearranged;
+        p.out = (unsigned char*)d_win.ptr;
+        // the first stream work on the uploads' host vectors must end before they go out of scope
+        CUDA_OK(cudaStreamSynchronize(stream));
+        return 0;
+    }
+    int write(long long begin, long long end, const int* d_tonode, const unsigned char* d_rows) {
+        const long long vis = b->row_bytes + 4;
+        p.tonode = d_tonode;
+        p.rows = d_rows;
+        for (long long wb = begin; wb < end; wb += kWindow) {
+            p.win_begin = wb;
+            p.win_end = std::min(end, wb + kWindow);
+            while (lo < L->start.size() && L->start[lo] + (long long)cnt[lo] * vis <= p.win_begin) ++lo;
+            size_t hi = lo;
+            while (hi < L->start.size() && L->start[hi] < p.win_end) ++hi;
+            p.first_list = (int)lo;
+            p.num_lists = (int)(hi - lo);
+            const long long w = next++;
+            CUDA_OK(cudaMemsetAsync(d_win.ptr, 0, (size_t)(p.win_end - p.win_begin), stream));
+            CUDA_OK(launch_spann_posting_image(p, stream));
+            g_launches++;
+            CUDA_OK(cudaMemcpyAsync(pin[w & 1], d_win.ptr, (size_t)(p.win_end - p.win_begin), cudaMemcpyDeviceToHost, stream));
+            CUDA_OK(cudaEventRecord(ev[w & 1], stream));
+            if (int rc = write_pending()) return rc;
+            pending = w;
+            pending_bytes = p.win_end - p.win_begin;
+        }
+        return 0;
+    }
+    int write_pending() {
+        if (pending < 0) return 0;
+        const int i = (int)(pending & 1);
+        pending = -1;
+        CUDA_OK(cudaEventSynchronize(ev[i]));
+        const size_t n = (size_t)pending_bytes;
+        if (std::fwrite(pin[i], 1, n, f.get()) != n) return fail(SPTAG_B200_FAIL, "writing %s failed", path.c_str());
+        return 0;
+    }
+    int finish() {
+        if (int rc = write_pending()) return rc;
+        if (std::fflush(f.get()) != 0) return fail(SPTAG_B200_FAIL, "writing %s failed", path.c_str());
+        return 0;
+    }
+};
+
+int write_posting_file(const SpannBuildFile& b, const std::string& path, int first, int nl, cudaStream_t stream) {
+    SpannFileLayout L;
+    spann_file_layout(b, first, nl, L);
+    SpannFileWriter w;
+    if (int rc = w.open(b, L, path, first, stream)) return rc;
+    if (L.area == 0) return 0;
+    if (int rc = w.write(0, L.area, b.d_tonode, b.d_rows)) return rc;
+    return w.finish();
+}
+
+// Owns what one sptag_b200_spann_build call allocates on the device, in pinned host memory and its streams; frees them
+// (and unregisters the caller's rows) with the device current
 struct SpannBuildState {
     sptag_b200_handle head = nullptr;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev[2] = {nullptr, nullptr};
+    cudaStream_t stream = nullptr, copy = nullptr;
+    cudaEvent_t ev[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr};
     DeviceBuffer d_rows, d_head, d_list, d_ids, d_dists, d_keys[2], d_tonode[2], d_size, d_counters, d_temp;
+    DeviceBuffer d_brows[2], d_flags, d_group_of, d_arena;  // the streamed path's
+    void* h_store = nullptr;            // the streamed path's pinned edge store
+    const void* registered = nullptr;   // the caller's rows, registered by this call
     ~SpannBuildState() {
         if (head) {
             DeviceGuard guard(head->device);
-            if (stream) cudaStreamSynchronize(stream);
-            for (cudaEvent_t e : ev)
+            for (cudaStream_t s : {stream, copy})
+                if (s) cudaStreamSynchronize(s);
+            for (cudaEvent_t e : {ev[0], ev[1], copied[0], copied[1]})
                 if (e) cudaEventDestroy(e);
-            if (stream) cudaStreamDestroy(stream);
+            for (cudaStream_t s : {stream, copy})
+                if (s) cudaStreamDestroy(s);
             for (DeviceBuffer* b : {&d_rows, &d_head, &d_list, &d_ids, &d_dists, &d_keys[0], &d_keys[1], &d_tonode[0],
-                                    &d_tonode[1], &d_size, &d_counters, &d_temp})
+                                    &d_tonode[1], &d_size, &d_counters, &d_temp, &d_brows[0], &d_brows[1], &d_flags,
+                                    &d_group_of, &d_arena})
                 b->release();
+            if (h_store) cudaFreeHost(h_store);
+            if (registered) cudaHostUnregister((void*)registered);
         }
         sptag_b200_destroy(head);
     }
@@ -3570,6 +3637,677 @@ struct SpannBuildState {
         return 0;
     }
 };
+
+// What both build paths read from the folder and the call
+struct SpannBuildConfig {
+    std::string dir, out;  // out: the first posting file's path
+    int value_type = 0, metric = 0, num = 0, dim = 0, normalized = 0, num_heads = 0;
+    int replicas = 0, k = 0, rearranged = 0, file_num = 0;
+    float rng_factor = 0;
+    long long limit = INT_MAX;  // elements a list keeps after the cut
+    size_t row_bytes = 0;
+    std::vector<unsigned char> is_head;
+    long long searched = 0;     // vectors that are not heads
+};
+
+// The ini, the refusals, the head (loaded into st.head with [BuildSSDIndex] MaxCheck) and the head-id file (rewritten
+// first with ExcludeHead false)
+int spann_build_prepare(const char* folder, const void* vectors, int32_t num, int32_t dim, int32_t normalized, int32_t device,
+                        SpannBuildState& st, SpannBuildConfig& c) {
+    if (!folder || !vectors || num <= 0) return fail(SPTAG_B200_EMPTY_DATA, "no vectors to build from");
+    c.dir = folder;
+    IniSections ini;
+    if (!read_ini(c.dir + "/indexloader.ini", ini)) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot open %s/indexloader.ini", folder);
+    auto get = [&](const char* section, const char* name, const char* def) { return ini_get(ini, section, name, def); };
+    // Refusals: what the device does not reproduce (SPANN/ParameterDefinitionList.h:34, :80-92)
+    if (!get("Base", "QuantizerFilePath", "").empty())
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "posting lists of quantized SPANN indexes are not built on the device");
+    for (const char* key : {"EnableDataCompression", "EnableDeltaEncoding", "OutputEmptyReplicaID"})
+        if (ini_true(get("BuildSSDIndex", key, "false")))
+            return fail(SPTAG_B200_LACK_OF_INPUTS, "%s is not supported by the device build", key);
+    c.value_type = enum_value(kValueTypes, get("Base", "ValueType", "Undefined"));
+    c.metric = enum_value(kDistCalcMethods, get("Base", "DistCalcMethod", "Undefined"));
+    if (c.value_type < 0 || c.metric < 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "unsupported ValueType or DistCalcMethod");
+    const int ini_dim = atoi(get("Base", "Dim", "-1").c_str());
+    if (dim <= 0 || (ini_dim != -1 && ini_dim != dim))
+        return fail(SPTAG_B200_DIMENSION_MISMATCH, "vectors have %d dimensions, the folder %d", dim, ini_dim);
+    c.replicas = atoi(get("BuildSSDIndex", "ReplicaCount", "8").c_str());
+    c.k = atoi(get("BuildSSDIndex", "InternalResultNum", "64").c_str());
+    c.rng_factor = strtof(get("BuildSSDIndex", "RNGFactor", "1.0").c_str(), nullptr);
+    int page_limit = atoi(get("BuildSSDIndex", "PostingPageLimit", "3").c_str());
+    const long long vector_limit = atoll(get("BuildSSDIndex", "PostingVectorLimit", "118").c_str());
+    const bool exclude_head = ini_true(get("BuildSSDIndex", "ExcludeHead", "true"));
+    c.rearranged = ini_true(get("BuildSSDIndex", "EnablePostingListRearrange", "false")) ? 1 : 0;
+    const std::string max_check = get("BuildSSDIndex", "MaxCheck", "4096");
+    c.file_num = atoi(get("Base", "SSDIndexFileNum", "1").c_str());
+    if (c.replicas < 1 || c.replicas > kSpannBuildMaxReplicas || c.k < 1 || c.k > 2048 || c.file_num < 1 ||
+        !std::isfinite(c.rng_factor))
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "ReplicaCount %d (1..%d), InternalResultNum %d (1..2048) or SSDIndexFileNum %d",
+                    c.replicas, kSpannBuildMaxReplicas, c.k, c.file_num);
+
+    const std::string head_dir = c.dir + "/" + get("Base", "HeadIndexFolder", "HeadIndex");
+    if (int rc = sptag_b200_load(head_dir.c_str(), device, 0, &st.head)) return rc;
+    sptag_b200_handle h = st.head;
+    if (h->q_type != 0 || h->value_type != c.value_type || h->metric != c.metric)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "the head index's value type or distance does not match the folder's");
+    if (h->dim != dim) return fail(SPTAG_B200_DIMENSION_MISMATCH, "vectors have %d dimensions, the head index %d", dim, h->dim);
+    // SPANNIndex.cpp:901: the head searches with [BuildSSDIndex] MaxCheck
+    if (int rc = sptag_b200_set_param(h, "MaxCheck", max_check.c_str())) return rc;
+    c.num_heads = h->n;
+    // SPANNIndex.cpp:914-925: with ExcludeHead false every head id becomes MaxSize, so that no vector is skipped
+    const std::string id_path = c.dir + "/" + get("Base", "HeadVectorIDs", "SPTAGHeadVectorIDs.bin");
+    if (!exclude_head) {
+        FILE* f = std::fopen(id_path.c_str(), "wb");
+        if (!f) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot write %s", id_path.c_str());
+        const std::vector<uint64_t> ids((size_t)c.num_heads, (uint64_t)INT_MAX);
+        const bool ok = std::fwrite(ids.data(), 8, ids.size(), f) == ids.size();
+        if (std::fclose(f) != 0 || !ok) return fail(SPTAG_B200_FAIL, "writing %s failed", id_path.c_str());
+    }
+    // the head-id set: every uint64 of the file cast to SizeType (ExtraFullGraphSearcher.h:604-616)
+    c.is_head.assign((size_t)num, 0);
+    {
+        std::vector<char> blob;
+        if (!read_file(id_path, blob)) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot read %s", id_path.c_str());
+        for (size_t i = 0; i + 8 <= blob.size(); i += 8) {
+            uint64_t v;
+            memcpy(&v, blob.data() + i, 8);
+            const int32_t id = (int32_t)(uint32_t)v;
+            if (id >= 0 && id < num) c.is_head[(size_t)id] = 1;
+        }
+    }
+    c.searched = 0;
+    for (unsigned char x : c.is_head) c.searched += !x;
+    c.num = num;
+    c.dim = dim;
+    c.normalized = normalized;
+    c.row_bytes = (size_t)dim * value_size(c.value_type);
+    // the posting cut (ExtraFullGraphSearcher.h:722-760): PostingPageLimit is first raised to the pages of
+    // PostingVectorLimit elements; each list keeps its first limit elements
+    const int vis = (int)c.row_bytes + 4;
+    c.limit = INT_MAX;
+    if (page_limit > 0) {
+        page_limit = std::max(page_limit, (int)((vector_limit * vis + 4095) / 4096));
+        c.limit = (long long)page_limit * 4096 / vis;
+    }
+    c.out = c.dir + "/" + get("Base", "SSDIndex", "SPTAGFullList.bin");
+    // SSDIndexFileNum files of ceil(lists / files) lists each (ExtraFullGraphSearcher.h:796-802)
+    const int per_file = (c.num_heads + c.file_num - 1) / c.file_num;
+    if ((long long)(c.file_num - 1) * per_file > c.num_heads)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "SSDIndexFileNum %d leaves a file without lists", c.file_num);
+    return 0;
+}
+
+// Lists [first, first + nl) of posting file i
+void spann_file_lists(const SpannBuildConfig& c, int i, int& first, int& nl) {
+    const int per_file = (c.num_heads + c.file_num - 1) / c.file_num;
+    first = i * per_file;
+    nl = std::min(c.num_heads, first + per_file) - first;
+}
+std::string spann_file_path(const SpannBuildConfig& c, int i) { return i == 0 ? c.out : c.out + "_" + std::to_string(i); }
+
+// The sort's scratch bytes for n edges
+size_t spann_sort_scratch(long long n, int end_bit, cudaStream_t stream) {
+    size_t t = 0;
+    if (spann_sort_edges(nullptr, &t, nullptr, nullptr, nullptr, nullptr, (int)n, end_bit, stream) != cudaSuccess) return SIZE_MAX / 4;
+    return t;
+}
+size_t spann_select_scratch(int n, cudaStream_t stream) {
+    size_t t = 0;
+    if (spann_select_edges(nullptr, &t, nullptr, nullptr, n, 0, 0, nullptr, 0, nullptr, nullptr, nullptr, nullptr, stream) !=
+        cudaSuccess)
+        return SIZE_MAX / 4;
+    return t;
+}
+// SortSelections: node, then distance, then tonode; unfilled edges (node = num_heads) last
+int spann_end_bit(int num_heads) {
+    int end_bit = 32;
+    while (end_bit < 64 && ((unsigned long long)num_heads >> (end_bit - 32)) != 0) ++end_bit;
+    return end_bit;
+}
+
+// The resident path: the rows and every edge in HBM (sptag_b200_spann_build)
+int spann_build_resident(SpannBuildConfig& c, SpannBuildState& st, const void* vectors, int64_t* stats) {
+    sptag_b200_handle h = st.head;
+    const int num = c.num, dim = c.dim, k = c.k, num_heads = c.num_heads;
+    const size_t row_bytes = c.row_bytes, edges = (size_t)num * c.replicas;
+    const std::vector<unsigned char>& is_head = c.is_head;
+    DeviceGuard guard(h->device);
+    CUDA_OK(cudaStreamCreateWithFlags(&st.stream, cudaStreamNonBlocking));
+    for (cudaEvent_t& e : st.ev) CUDA_OK(cudaEventCreate(&e));
+    cudaStream_t stream = st.stream;
+    const int kBatch = 1 << 16;
+    const int batch = std::min(num, kBatch);
+    if (int rc = st.d_rows.ensure((size_t)num * row_bytes)) return rc;
+    for (int i = 0; i < 2; ++i) {
+        if (int rc = st.d_keys[i].ensure(edges * 8)) return rc;
+        if (int rc = st.d_tonode[i].ensure(edges * 4)) return rc;
+    }
+    if (int rc = st.d_head.ensure((size_t)num)) return rc;
+    if (int rc = st.d_list.ensure(((size_t)batch + 1) * 4)) return rc;
+    if (int rc = st.d_ids.ensure((size_t)batch * k * 4)) return rc;
+    if (int rc = st.d_dists.ensure((size_t)batch * k * 4)) return rc;
+    if (int rc = st.d_size.ensure((size_t)num_heads * 4 + 4)) return rc;
+    if (int rc = st.d_counters.ensure(16)) return rc;  // rejections (uint64), the non-finite flag
+    unsigned long long* d_rejected = (unsigned long long*)st.d_counters.ptr;
+    int* d_bad = (int*)((unsigned char*)st.d_counters.ptr + 8);
+    CUDA_OK(cudaMemsetAsync(st.d_counters.ptr, 0, 16, stream));
+    CUDA_OK(cudaMemsetAsync(st.d_size.ptr, 0, (size_t)num_heads * 4, stream));
+    CUDA_OK(cudaMemcpyAsync(st.d_head.ptr, is_head.data(), (size_t)num, cudaMemcpyHostToDevice, stream));
+    ArraySource src;
+    src.ptr = vectors;
+    if (int rc = upload_rows(src, st.d_rows.ptr, (size_t)num, row_bytes, row_bytes, stream)) return rc;
+    unsigned char* rows = (unsigned char*)st.d_rows.ptr;
+    // sort and NaN have no order (std::sort under NaN is undefined): rows must be finite
+    if (c.value_type == SPTAG_B200_VT_FLOAT) {
+        CUDA_OK(launch_spann_nonfinite_check((const float*)rows, (size_t)num * dim, d_bad, stream));
+        int bad = 0;
+        CUDA_OK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        if (bad) return fail(SPTAG_B200_LACK_OF_INPUTS, "a row holds a NaN or an infinity");
+    }
+    // ExtraFullGraphSearcher.h:650: Cosine rows are normalised unless the caller says they are
+    if (c.metric == SPTAG_B200_METRIC_COSINE && !c.normalized) {
+        const int base = value_base(c.value_type);
+        with_elem(h, [&](auto el) {
+            normalize_rows_kernel<typename decltype(el)::type><<<(unsigned)((num + 127) / 128), 128, 0, stream>>>(
+                rows, row_bytes, 0, num, dim, base);
+        });
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+    }
+    // ApproximateRNG in batches of rows: the head search at K = InternalResultNum for the batch's non-head rows (queries
+    // read in place through the query list), then the RNG selection of the whole batch
+    const MetricElem me = metric_elem(h);
+    float ms_search = 0, ms_rng = 0, ms_sort = 0;
+    long long searched = 0;
+    std::vector<unsigned int> list((size_t)batch + 1);
+    SpannRngParams rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.res_ids = (const int*)st.d_ids.ptr;
+    rp.res_dists = (const float*)st.d_dists.ptr;
+    rp.k = k;
+    rp.head = (const unsigned char*)st.d_head.ptr;
+    rp.rows = (const unsigned char*)h->d_vectors.ptr;
+    rp.row_stride = h->row_stride;
+    rp.dim = dim;
+    rp.simd_width = h->simd_width;
+    rp.replicas = c.replicas;
+    rp.num_heads = num_heads;
+    rp.rng_factor = c.rng_factor;
+    rp.keys = (unsigned long long*)st.d_keys[0].ptr;
+    rp.tonode = (int*)st.d_tonode[0].ptr;
+    rp.list_size = (int*)st.d_size.ptr;
+    rp.rejected = d_rejected;
+    rp.bad = d_bad;
+    for (int b0 = 0; b0 < num; b0 += batch) {
+        const int nb = std::min(batch, num - b0);
+        unsigned int cq = 0;
+        for (int i = 0; i < nb; ++i)
+            if (!is_head[(size_t)b0 + i]) list[1 + cq++] = (unsigned int)i;
+        list[0] = cq;
+        searched += cq;
+        CUDA_OK(cudaMemcpyAsync(st.d_list.ptr, list.data(), ((size_t)cq + 1) * 4, cudaMemcpyHostToDevice, stream));
+        CUDA_OK(cudaEventRecord(st.ev[0], stream));
+        if (cq > 0) {
+            CallOpts opts;
+            opts.search_deleted = 0;
+            opts.d_query_list = (const unsigned int*)st.d_list.ptr;
+            std::lock_guard<std::mutex> lock(h->mu);
+            if (int rc = search_device_impl(h, rows + (size_t)b0 * row_bytes, nb, k, (int*)st.d_ids.ptr,
+                                            (float*)st.d_dists.ptr, nullptr, stream, false, opts))
+                return rc;
+        }
+        CUDA_OK(cudaEventRecord(st.ev[1], stream));
+        if (int rc = st.elapsed(ms_search)) return rc;  // also frees `list` for the next batch
+        rp.first = b0;
+        rp.num = nb;
+        CUDA_OK(cudaEventRecord(st.ev[0], stream));
+        CUDA_OK(launch_spann_rng_select(rp, me.cosine, me.elem, stream));
+        g_launches++;
+        CUDA_OK(cudaEventRecord(st.ev[1], stream));
+        if (int rc = st.elapsed(ms_rng)) return rc;
+    }
+    int bad = 0;
+    unsigned long long rejected = 0;
+    CUDA_OK(cudaMemcpy(&bad, d_bad, 4, cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(&rejected, d_rejected, 8, cudaMemcpyDeviceToHost));
+    if (bad) return fail(SPTAG_B200_LACK_OF_INPUTS, "a distance is not finite");
+    const int end_bit = spann_end_bit(num_heads);
+    size_t temp_bytes = 0;
+    CUDA_OK(spann_sort_edges(nullptr, &temp_bytes, nullptr, nullptr, nullptr, nullptr, (int)edges, end_bit, stream));
+    if (int rc = st.d_temp.ensure(std::max<size_t>(temp_bytes, 1))) return rc;
+    CUDA_OK(cudaEventRecord(st.ev[0], stream));
+    CUDA_OK(spann_sort_edges(st.d_temp.ptr, &temp_bytes, (const unsigned long long*)st.d_keys[0].ptr,
+                             (unsigned long long*)st.d_keys[1].ptr, (const int*)st.d_tonode[0].ptr, (int*)st.d_tonode[1].ptr,
+                             (int)edges, end_bit, stream));
+    g_launches++;
+    CUDA_OK(cudaEventRecord(st.ev[1], stream));
+    if (int rc = st.elapsed(ms_sort)) return rc;
+    st.d_keys[0].release();
+    st.d_tonode[0].release();
+    st.d_temp.release();
+    std::vector<int> size((size_t)num_heads);
+    CUDA_OK(cudaMemcpy(size.data(), st.d_size.ptr, (size_t)num_heads * 4, cudaMemcpyDeviceToHost));
+    std::vector<long long> edge_off((size_t)num_heads);
+    std::vector<int> count((size_t)num_heads);
+    long long before = 0, after = 0;
+    for (int l = 0; l < num_heads; ++l) {
+        edge_off[l] = before;
+        before += size[l];
+        count[l] = (int)std::min<long long>(size[l], c.limit);
+        after += count[l];
+    }
+    const auto t0 = std::chrono::steady_clock::now();
+    SpannBuildFile bf;
+    bf.d_tonode = (const int*)st.d_tonode[1].ptr;
+    bf.d_rows = rows;
+    bf.row_bytes = (int)row_bytes;
+    bf.rearranged = c.rearranged;
+    bf.num_vectors = num;
+    bf.dim = dim;
+    bf.edge_off = &edge_off;
+    bf.count = &count;
+    bf.row_off = nullptr;
+    for (int i = 0; i < c.file_num; ++i) {
+        int first, nl;
+        spann_file_lists(c, i, first, nl);
+        if (int rc = write_posting_file(bf, spann_file_path(c, i), first, nl, stream)) return rc;
+    }
+    const double ms_write = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    const int64_t out[8] = {searched, (int64_t)rejected, before, after, (int64_t)(ms_search * 1000.0),
+                            (int64_t)(ms_rng * 1000.0), (int64_t)(ms_sort * 1000.0), (int64_t)(ms_write * 1000.0)};
+    memcpy(stats, out, sizeof(out));
+    return SPTAG_B200_SUCCESS;
+}
+
+// The resident path's device bytes (sptag_b200.h): the rows, 24 B per edge, the sort's scratch, one search batch of
+// results and the 64 MB window
+long long spann_resident_bytes(const SpannBuildConfig& c, cudaStream_t stream) {
+    const long long edges = (long long)c.num * c.replicas;
+    return (long long)c.num * (long long)c.row_bytes + 24 * edges +
+           (long long)spann_sort_scratch(std::min<long long>(edges, INT_MAX), spann_end_bit(c.num_heads), stream) +
+           (long long)std::min(c.num, 1 << 16) * c.k * 8 + SpannFileWriter::kWindow;
+}
+
+// The streamed path's pass 1 for batches of B rows (sptag_b200.h)
+long long spann_pass1_bytes(const SpannBuildConfig& c, long long B, cudaStream_t stream) {
+    const long long per_row = 2 * (long long)c.row_bytes + 1 + 4 + 8ll * c.k + 25ll * c.replicas;
+    return B * per_row + 4 + (long long)spann_select_scratch((int)(B * c.replicas), stream) + 32 + 4ll * c.num_heads + 4;
+}
+
+// The streamed path: the rows stay in the caller's (mapped) buffer, the edges in a pinned host store, and the posting
+// files are written in groups of lists whose edges and rows fit the budget
+int spann_build_streamed(SpannBuildConfig& c, SpannBuildState& st, const void* vectors, long long budget, int64_t* stats) {
+    sptag_b200_handle h = st.head;
+    const int num = c.num, dim = c.dim, k = c.k, num_heads = c.num_heads, R = c.replicas;
+    const size_t row_bytes = c.row_bytes;
+    const std::vector<unsigned char>& is_head = c.is_head;
+    DeviceGuard guard(h->device);
+    CUDA_OK(cudaStreamCreateWithFlags(&st.stream, cudaStreamNonBlocking));
+    CUDA_OK(cudaStreamCreateWithFlags(&st.copy, cudaStreamNonBlocking));
+    for (cudaEvent_t& e : st.ev) CUDA_OK(cudaEventCreate(&e));
+    for (cudaEvent_t& e : st.copied) CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    cudaStream_t stream = st.stream;
+    // pass 1's batch: 65536 rows, halved until its buffers fit
+    long long B = std::min(num, 1 << 16);
+    while (B > 1 && spann_pass1_bytes(c, B, stream) > budget) B = (B + 1) / 2;
+    if (spann_pass1_bytes(c, B, stream) > budget)
+        return fail(SPTAG_B200_MEMORY_OVERFLOW, "a device budget of %lld bytes is below the %lld bytes of a one-row batch",
+                    budget, spann_pass1_bytes(c, 1, stream));
+    // the pinned edge store: every filled edge, 12 B (key, vector id)
+    const long long per_vector = std::min({R, k, num_heads});
+    const long long store_cap = c.searched * per_vector;
+    if (store_cap > 0 && cudaHostAlloc(&st.h_store, (size_t)store_cap * 12, cudaHostAllocDefault) != cudaSuccess) {
+        cudaGetLastError();
+        st.h_store = nullptr;
+        return fail(SPTAG_B200_MEMORY_OVERFLOW, "the pinned edge store (%lld bytes) cannot be allocated", store_cap * 12);
+    }
+    unsigned long long* h_keys = (unsigned long long*)st.h_store;
+    int* h_tonode = (int*)((unsigned char*)st.h_store + (size_t)store_cap * 8);
+    // the caller's rows, mapped; a buffer registered before is used as it is
+    const size_t all_rows = (size_t)num * row_bytes;
+    cudaError_t re = cudaHostRegister((void*)vectors, all_rows, cudaHostRegisterMapped);
+    if (re == cudaSuccess) {
+        st.registered = vectors;
+    } else if (re == cudaErrorHostMemoryAlreadyRegistered) {
+        cudaGetLastError();
+    } else {
+        cudaGetLastError();
+        return fail(SPTAG_B200_FAIL, "cudaHostRegister of the rows failed: %s", cudaGetErrorString(re));
+    }
+    void* d_src = nullptr;
+    CUDA_OK(cudaHostGetDevicePointer(&d_src, (void*)vectors, 0));
+    const unsigned char* src_rows = (const unsigned char*)vectors;
+
+    // pass 1: search, RNG selection and the filled edges appended to the store, batch by batch
+    const long long BR = B * R;
+    for (int i = 0; i < 2; ++i)
+        if (int rc = st.d_brows[i].ensure((size_t)B * row_bytes)) return rc;
+    if (int rc = st.d_head.ensure((size_t)B)) return rc;
+    if (int rc = st.d_list.ensure(((size_t)B + 1) * 4)) return rc;
+    if (int rc = st.d_ids.ensure((size_t)B * k * 4)) return rc;
+    if (int rc = st.d_dists.ensure((size_t)B * k * 4)) return rc;
+    for (int i = 0; i < 2; ++i) {
+        if (int rc = st.d_keys[i].ensure((size_t)BR * 8)) return rc;
+        if (int rc = st.d_tonode[i].ensure((size_t)BR * 4)) return rc;
+    }
+    if (int rc = st.d_flags.ensure((size_t)BR)) return rc;
+    size_t sel_bytes = spann_select_scratch((int)BR, stream);
+    if (int rc = st.d_temp.ensure(std::max<size_t>(sel_bytes, 1))) return rc;
+    if (int rc = st.d_counters.ensure(32)) return rc;  // rejections (uint64), the two non-finite flags, the selected count
+    if (int rc = st.d_size.ensure((size_t)num_heads * 4 + 4)) return rc;
+    unsigned long long* d_rejected = (unsigned long long*)st.d_counters.ptr;
+    int* d_bad = (int*)((unsigned char*)st.d_counters.ptr + 8);
+    int* d_row_bad = d_bad + 1;
+    int* d_nsel = d_bad + 2;
+    CUDA_OK(cudaMemsetAsync(st.d_counters.ptr, 0, 32, stream));
+    CUDA_OK(cudaMemsetAsync(st.d_size.ptr, 0, (size_t)num_heads * 4, stream));
+    const MetricElem me = metric_elem(h);
+    const bool normalize = c.metric == SPTAG_B200_METRIC_COSINE && !c.normalized;
+    const int base = value_base(c.value_type);
+    float ms_search = 0, ms_rng = 0, ms_sort = 0;
+    long long searched = 0, batches = 0, h2d = 0, stored = 0;
+    std::vector<unsigned int> list((size_t)B + 1);
+    SpannRngParams rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.res_ids = (const int*)st.d_ids.ptr;
+    rp.res_dists = (const float*)st.d_dists.ptr;
+    rp.k = k;
+    rp.first = 0;  // batch-local vector ids; the selection adds the batch's first id
+    rp.head = (const unsigned char*)st.d_head.ptr;
+    rp.rows = (const unsigned char*)h->d_vectors.ptr;
+    rp.row_stride = h->row_stride;
+    rp.dim = dim;
+    rp.simd_width = h->simd_width;
+    rp.replicas = R;
+    rp.num_heads = num_heads;
+    rp.rng_factor = c.rng_factor;
+    rp.keys = (unsigned long long*)st.d_keys[0].ptr;
+    rp.tonode = (int*)st.d_tonode[0].ptr;
+    rp.list_size = (int*)st.d_size.ptr;
+    rp.rejected = d_rejected;
+    rp.bad = d_bad;
+    // batch i's rows go to d_brows[i & 1] on the copy stream while batch i - 1 is searched
+    auto copy_batch = [&](int b0) -> int {
+        const int nb = std::min<long long>(B, num - b0);
+        const int slot = (int)((b0 / B) & 1);
+        CUDA_OK(cudaMemcpyAsync(st.d_brows[slot].ptr, src_rows + (size_t)b0 * row_bytes, (size_t)nb * row_bytes,
+                                cudaMemcpyHostToDevice, st.copy));
+        CUDA_OK(cudaEventRecord(st.copied[slot], st.copy));
+        h2d += (long long)nb * (long long)row_bytes;
+        return 0;
+    };
+    if (int rc = copy_batch(0)) return rc;
+    for (int b0 = 0; b0 < num; b0 += (int)B) {
+        const int nb = (int)std::min<long long>(B, num - b0);
+        const int slot = (int)((b0 / B) & 1);
+        unsigned char* rows = (unsigned char*)st.d_brows[slot].ptr;
+        // the other buffer was last read by the previous batch's search, which the host has waited for
+        if (b0 + B < num)
+            if (int rc = copy_batch((int)(b0 + B))) return rc;
+        CUDA_OK(cudaStreamWaitEvent(stream, st.copied[slot], 0));
+        ++batches;
+        if (c.value_type == SPTAG_B200_VT_FLOAT)
+            CUDA_OK(launch_spann_nonfinite_check((const float*)rows, (size_t)nb * dim, d_row_bad, stream));
+        if (normalize) {
+            with_elem(h, [&](auto el) {
+                normalize_rows_kernel<typename decltype(el)::type><<<(unsigned)((nb + 127) / 128), 128, 0, stream>>>(
+                    rows, row_bytes, 0, nb, dim, base);
+            });
+            g_launches++;
+            CUDA_OK(cudaGetLastError());
+        }
+        unsigned int cq = 0;
+        for (int i = 0; i < nb; ++i)
+            if (!is_head[(size_t)b0 + i]) list[1 + cq++] = (unsigned int)i;
+        list[0] = cq;
+        searched += cq;
+        CUDA_OK(cudaMemcpyAsync(st.d_list.ptr, list.data(), ((size_t)cq + 1) * 4, cudaMemcpyHostToDevice, stream));
+        CUDA_OK(cudaMemcpyAsync(st.d_head.ptr, is_head.data() + b0, (size_t)nb, cudaMemcpyHostToDevice, stream));
+        int row_bad = 0;
+        CUDA_OK(cudaMemcpyAsync(&row_bad, d_row_bad, 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        if (row_bad) return fail(SPTAG_B200_LACK_OF_INPUTS, "a row holds a NaN or an infinity");
+        CUDA_OK(cudaEventRecord(st.ev[0], stream));
+        if (cq > 0) {
+            CallOpts opts;
+            opts.search_deleted = 0;
+            opts.d_query_list = (const unsigned int*)st.d_list.ptr;
+            std::lock_guard<std::mutex> lock(h->mu);
+            if (int rc = search_device_impl(h, rows, nb, k, (int*)st.d_ids.ptr, (float*)st.d_dists.ptr, nullptr, stream,
+                                            false, opts))
+                return rc;
+        }
+        CUDA_OK(cudaEventRecord(st.ev[1], stream));
+        if (int rc = st.elapsed(ms_search)) return rc;  // also frees `list` and this batch's rows
+        rp.num = nb;
+        CUDA_OK(cudaEventRecord(st.ev[0], stream));
+        CUDA_OK(launch_spann_rng_select(rp, me.cosine, me.elem, stream));
+        g_launches++;
+        // the filled edges, in vector-id order, with global vector ids
+        CUDA_OK(spann_select_edges(st.d_temp.ptr, &sel_bytes, (const unsigned long long*)st.d_keys[0].ptr,
+                                   (int*)st.d_tonode[0].ptr, (int)(nb * R), b0, num_heads, nullptr, 0,
+                                   (unsigned char*)st.d_flags.ptr, (unsigned long long*)st.d_keys[1].ptr,
+                                   (int*)st.d_tonode[1].ptr, d_nsel, stream));
+        g_launches += 3;
+        CUDA_OK(cudaEventRecord(st.ev[1], stream));
+        if (int rc = st.elapsed(ms_rng)) return rc;
+        int nsel = 0;
+        CUDA_OK(cudaMemcpy(&nsel, d_nsel, 4, cudaMemcpyDeviceToHost));
+        if (stored + nsel > store_cap) return fail(SPTAG_B200_FAIL, "the edge store overflowed");
+        CUDA_OK(cudaMemcpyAsync(h_keys + stored, st.d_keys[1].ptr, (size_t)nsel * 8, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaMemcpyAsync(h_tonode + stored, st.d_tonode[1].ptr, (size_t)nsel * 4, cudaMemcpyDeviceToHost, stream));
+        stored += nsel;
+    }
+    CUDA_OK(cudaStreamSynchronize(stream));
+    int bad = 0;
+    unsigned long long rejected = 0;
+    CUDA_OK(cudaMemcpy(&bad, d_bad, 4, cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(&rejected, d_rejected, 8, cudaMemcpyDeviceToHost));
+    if (bad) return fail(SPTAG_B200_LACK_OF_INPUTS, "a distance is not finite");
+    std::vector<int> size((size_t)num_heads);
+    CUDA_OK(cudaMemcpy(size.data(), st.d_size.ptr, (size_t)num_heads * 4, cudaMemcpyDeviceToHost));
+    for (DeviceBuffer* b : {&st.d_brows[0], &st.d_brows[1], &st.d_head, &st.d_list, &st.d_ids, &st.d_dists, &st.d_keys[0],
+                            &st.d_keys[1], &st.d_tonode[0], &st.d_tonode[1], &st.d_flags, &st.d_temp, &st.d_size})
+        b->release();
+    const auto t0 = std::chrono::steady_clock::now();
+    std::vector<int> count((size_t)num_heads);
+    long long before = 0, after = 0, largest = -1;
+    for (int l = 0; l < num_heads; ++l) {
+        before += size[l];
+        count[l] = (int)std::min<long long>(size[l], c.limit);
+        after += count[l];
+        if (count[l] > 0 && (largest < 0 || size[l] > size[largest])) largest = l;
+    }
+    if (before != stored) return fail(SPTAG_B200_FAIL, "%lld edges stored, %lld counted", stored, before);
+
+    // placement, and the groups: runs of placed lists whose edges, sort buffers and gathered rows fit
+    SpannBuildFile bf;
+    std::vector<long long> edge_off((size_t)num_heads, 0), row_off((size_t)num_heads, 0);
+    bf.d_tonode = nullptr;
+    bf.d_rows = nullptr;
+    bf.row_bytes = (int)row_bytes;
+    bf.rearranged = c.rearranged;
+    bf.num_vectors = num;
+    bf.dim = dim;
+    bf.edge_off = &edge_off;
+    bf.count = &count;
+    bf.row_off = &row_off;
+    std::vector<SpannFileLayout> layouts((size_t)c.file_num);
+    long long max_lists = 0, max_window = 0;
+    for (int i = 0; i < c.file_num; ++i) {
+        int first, nl;
+        spann_file_lists(c, i, first, nl);
+        spann_file_layout(bf, first, nl, layouts[i]);
+        max_lists = std::max<long long>(max_lists, (long long)layouts[i].order.size());
+        max_window = std::max(max_window, SpannFileWriter::window_bytes(layouts[i].area));
+    }
+    const int end_bit = spann_end_bit(num_heads);
+    auto a256 = [](long long x) { return (long long)round_up((size_t)x, 256); };
+    // a group of E edges (before the cut) and C gathered rows: keys and vector ids twice, the sort's scratch, the rows
+    auto group_bytes = [&](long long E, long long C) {
+        return 2 * a256(8 * E) + 2 * a256(4 * E) + a256((long long)spann_sort_scratch(E, end_bit, stream)) +
+               a256(C * (long long)row_bytes);
+    };
+    // pass 2's fixed buffers for chunks of C edges: two chunks of keys and vector ids, their flags, the selection's
+    // scratch and counters, the list-to-group map, one file's per-list arrays and its window
+    auto fixed_bytes = [&](long long C) {
+        return 25 * C + (long long)spann_select_scratch((int)C, stream) + 32 + 4ll * num_heads + 28 * max_lists + max_window;
+    };
+    const long long min_chunk = std::min<long long>(std::max<long long>(stored, 1), 4096);
+    const long long largest_group = largest < 0 ? 0 : group_bytes(size[largest], count[largest]);
+    const long long minimum = std::max(spann_pass1_bytes(c, 1, stream), fixed_bytes(min_chunk) + largest_group);
+    if (budget < minimum)
+        return fail(SPTAG_B200_MEMORY_OVERFLOW, "a device budget of %lld bytes: the streamed build needs at least %lld bytes",
+                    budget, minimum);
+    long long chunk = std::min<long long>(std::max<long long>(stored, 1), 1 << 22);
+    while (chunk > min_chunk && fixed_bytes(chunk) + largest_group > budget) chunk = std::max(min_chunk, (chunk + 1) / 2);
+    const long long cap = budget - fixed_bytes(chunk);
+    struct Group {
+        int file, first, end;  // placed lists [first, end) of the file
+        long long edges, rows, begin, stop;  // the list area's bytes [begin, stop)
+    };
+    std::vector<Group> groups;
+    std::vector<int> group_of((size_t)num_heads, -1);
+    long long max_group = 0;
+    for (int i = 0; i < c.file_num; ++i) {
+        int first, nl;
+        spann_file_lists(c, i, first, nl);
+        const SpannFileLayout& L = layouts[i];
+        const int n_placed = (int)L.order.size();
+        for (int a = 0; a < n_placed;) {
+            long long E = 0, C = 0;
+            int e = a;
+            while (e < n_placed) {
+                const int l = first + L.order[e];
+                const long long E2 = E + size[l], C2 = C + count[l];
+                if (e > a && (E2 > INT_MAX || group_bytes(E2, C2) > cap)) break;
+                E = E2;
+                C = C2;
+                ++e;
+            }
+            Group g{i, a, e, E, C, L.start[a], e < n_placed ? L.start[e] : L.area};
+            // group-local offsets: the sorted edges in list-id order, the gathered rows in placement order
+            std::vector<int> ids;
+            for (int j = a; j < e; ++j) ids.push_back(first + L.order[j]);
+            long long r = 0;
+            for (int l : ids) {
+                row_off[l] = r;
+                r += count[l];
+                group_of[l] = (int)groups.size();
+            }
+            std::sort(ids.begin(), ids.end());
+            long long eo = 0;
+            for (int l : ids) {
+                edge_off[l] = eo;
+                eo += size[l];
+            }
+            max_group = std::max(max_group, group_bytes(E, C));
+            groups.push_back(g);
+            a = e;
+        }
+    }
+
+    // pass 2, per group: the group's edges kept from the store, sorted, their rows gathered, its windows written
+    if (int rc = st.d_group_of.ensure((size_t)num_heads * 4 + 4)) return rc;
+    CUDA_OK(cudaMemcpy(st.d_group_of.ptr, group_of.data(), (size_t)num_heads * 4, cudaMemcpyHostToDevice));
+    for (int i = 0; i < 2; ++i) {
+        if (int rc = st.d_keys[i].ensure((size_t)chunk * 8)) return rc;
+        if (int rc = st.d_tonode[i].ensure((size_t)chunk * 4)) return rc;
+    }
+    if (int rc = st.d_flags.ensure((size_t)chunk)) return rc;
+    sel_bytes = spann_select_scratch((int)chunk, stream);
+    if (int rc = st.d_temp.ensure(std::max<size_t>(sel_bytes, 1))) return rc;
+    if (int rc = st.d_arena.ensure((size_t)std::max<long long>(max_group, 256))) return rc;
+    unsigned char* arena = (unsigned char*)st.d_arena.ptr;
+    const unsigned char* d_src_rows = (const unsigned char*)d_src;
+    long long gathered = 0;
+    for (int i = 0, gi = 0; i < c.file_num; ++i) {
+        int first, nl;
+        spann_file_lists(c, i, first, nl);
+        SpannFileWriter w;
+        if (int rc = w.open(bf, layouts[i], spann_file_path(c, i), first, stream)) return rc;
+        for (; gi < (int)groups.size() && groups[gi].file == i; ++gi) {
+            const Group& g = groups[gi];
+            const long long E = g.edges;
+            unsigned long long* g_keys[2] = {(unsigned long long*)arena, (unsigned long long*)(arena + a256(8 * E))};
+            int* g_ton[2] = {(int*)(arena + 2 * a256(8 * E)), (int*)(arena + 2 * a256(8 * E) + a256(4 * E))};
+            unsigned char* g_temp = arena + 2 * a256(8 * E) + 2 * a256(4 * E);
+            size_t sort_bytes = spann_sort_scratch(E, end_bit, stream);
+            unsigned char* g_rows = g_temp + a256((long long)sort_bytes);
+            // the edge pass: the store through two chunk buffers; the copy of chunk j + 1 overlaps chunk j's selection
+            long long kept = 0;
+            auto copy_chunk = [&](long long c0) -> int {
+                const long long n = std::min(chunk, stored - c0);
+                const int slot = (int)((c0 / chunk) & 1);
+                CUDA_OK(cudaMemcpyAsync(st.d_keys[slot].ptr, h_keys + c0, (size_t)n * 8, cudaMemcpyHostToDevice, st.copy));
+                CUDA_OK(cudaMemcpyAsync(st.d_tonode[slot].ptr, h_tonode + c0, (size_t)n * 4, cudaMemcpyHostToDevice, st.copy));
+                CUDA_OK(cudaEventRecord(st.copied[slot], st.copy));
+                h2d += n * 12;
+                return 0;
+            };
+            if (stored > 0)
+                if (int rc = copy_chunk(0)) return rc;
+            for (long long c0 = 0; c0 < stored; c0 += chunk) {
+                const long long n = std::min(chunk, stored - c0);
+                const int slot = (int)((c0 / chunk) & 1);
+                // the other chunk buffer was last read by the previous chunk's selection, which the host has waited for
+                if (c0 + chunk < stored)
+                    if (int rc = copy_chunk(c0 + chunk)) return rc;
+                CUDA_OK(cudaStreamWaitEvent(stream, st.copied[slot], 0));
+                CUDA_OK(spann_select_edges(st.d_temp.ptr, &sel_bytes, (const unsigned long long*)st.d_keys[slot].ptr,
+                                           (int*)st.d_tonode[slot].ptr, (int)n, 0, num_heads, (const int*)st.d_group_of.ptr,
+                                           gi, (unsigned char*)st.d_flags.ptr, g_keys[0] + kept, g_ton[0] + kept, d_nsel,
+                                           stream));
+                g_launches += 3;
+                int nsel = 0;
+                CUDA_OK(cudaMemcpyAsync(&nsel, d_nsel, 4, cudaMemcpyDeviceToHost, stream));
+                CUDA_OK(cudaStreamSynchronize(stream));
+                kept += nsel;
+            }
+            if (kept != E) return fail(SPTAG_B200_FAIL, "group %d: %lld edges kept, %lld expected", gi, kept, E);
+            // the edges entered in ascending vector id: the stable sort gives EdgeCompare's order
+            CUDA_OK(cudaEventRecord(st.ev[0], stream));
+            CUDA_OK(spann_sort_edges(g_temp, &sort_bytes, g_keys[0], g_keys[1], g_ton[0], g_ton[1], (int)E, end_bit, stream));
+            g_launches++;
+            CUDA_OK(cudaEventRecord(st.ev[1], stream));
+            if (int rc = st.elapsed(ms_sort)) return rc;
+            // the kept edges' rows, from the caller's buffer
+            SpannGatherParams gp;
+            memset(&gp, 0, sizeof(gp));
+            gp.edge_off = (const long long*)w.d_eoff.ptr;
+            gp.row_off = (const long long*)w.d_roff.ptr;
+            gp.count = (const int*)w.d_cnt.ptr;
+            gp.first_list = g.first;
+            gp.num_lists = g.end - g.first;
+            gp.tonode = g_ton[1];
+            gp.src = d_src_rows;
+            gp.row_bytes = (int)row_bytes;
+            gp.dst = g_rows;
+            CUDA_OK(launch_spann_row_gather(gp, stream));
+            g_launches++;
+            gathered += g.rows * (long long)row_bytes;
+            if (normalize && g.rows > 0) {
+                with_elem(h, [&](auto el) {
+                    normalize_rows_kernel<typename decltype(el)::type><<<(unsigned)((g.rows + 127) / 128), 128, 0, stream>>>(
+                        g_rows, row_bytes, 0, (int)g.rows, dim, base);
+                });
+                g_launches++;
+                CUDA_OK(cudaGetLastError());
+            }
+            if (int rc = w.write(g.begin, g.stop, g_ton[1], g_rows)) return rc;
+        }
+        if (layouts[i].area > 0)
+            if (int rc = w.finish()) return rc;
+    }
+    h2d += gathered;
+    const double ms_pass2 = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    const int64_t out[12] = {searched, (int64_t)rejected, before, after, (int64_t)(ms_search * 1000.0),
+                             (int64_t)(ms_rng * 1000.0), (int64_t)(ms_sort * 1000.0),
+                             (int64_t)((ms_pass2 - ms_sort) * 1000.0), 1, batches, (int64_t)groups.size(), h2d};
+    memcpy(stats, out, sizeof(out));
+    return SPTAG_B200_SUCCESS;
+}
 }  // namespace
 
 extern "C" {
@@ -3668,232 +4406,48 @@ int sptag_b200_spann_load_ex(const char* folder, int32_t device, const sptag_b20
 
 int sptag_b200_spann_build(const char* folder, const void* vectors, int32_t num, int32_t dim, int32_t normalized,
                            int32_t device, int64_t* out_stats) {
-    if (!folder || !vectors || num <= 0) return fail(SPTAG_B200_EMPTY_DATA, "no vectors to build from");
-    const std::string dir(folder);
-    IniSections ini;
-    if (!read_ini(dir + "/indexloader.ini", ini)) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot open %s/indexloader.ini", folder);
-    auto get = [&](const char* section, const char* name, const char* def) { return ini_get(ini, section, name, def); };
-    // Refusals: what the device does not reproduce (SPANN/ParameterDefinitionList.h:34, :80-92)
-    if (!get("Base", "QuantizerFilePath", "").empty())
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "posting lists of quantized SPANN indexes are not built on the device");
-    for (const char* key : {"EnableDataCompression", "EnableDeltaEncoding", "OutputEmptyReplicaID"})
-        if (ini_true(get("BuildSSDIndex", key, "false")))
-            return fail(SPTAG_B200_LACK_OF_INPUTS, "%s is not supported by the device build", key);
-    const int value_type = enum_value(kValueTypes, get("Base", "ValueType", "Undefined"));
-    const int metric = enum_value(kDistCalcMethods, get("Base", "DistCalcMethod", "Undefined"));
-    if (value_type < 0 || metric < 0) return fail(SPTAG_B200_LACK_OF_INPUTS, "unsupported ValueType or DistCalcMethod");
-    const int ini_dim = atoi(get("Base", "Dim", "-1").c_str());
-    if (dim <= 0 || (ini_dim != -1 && ini_dim != dim))
-        return fail(SPTAG_B200_DIMENSION_MISMATCH, "vectors have %d dimensions, the folder %d", dim, ini_dim);
-    const int replicas = atoi(get("BuildSSDIndex", "ReplicaCount", "8").c_str());
-    const int k = atoi(get("BuildSSDIndex", "InternalResultNum", "64").c_str());
-    const float rng_factor = strtof(get("BuildSSDIndex", "RNGFactor", "1.0").c_str(), nullptr);
-    int page_limit = atoi(get("BuildSSDIndex", "PostingPageLimit", "3").c_str());
-    const long long vector_limit = atoll(get("BuildSSDIndex", "PostingVectorLimit", "118").c_str());
-    const bool exclude_head = ini_true(get("BuildSSDIndex", "ExcludeHead", "true"));
-    const int rearranged = ini_true(get("BuildSSDIndex", "EnablePostingListRearrange", "false")) ? 1 : 0;
-    const std::string max_check = get("BuildSSDIndex", "MaxCheck", "4096");
-    const int file_num = atoi(get("Base", "SSDIndexFileNum", "1").c_str());
-    if (replicas < 1 || replicas > kSpannBuildMaxReplicas || k < 1 || k > 2048 || file_num < 1 || !std::isfinite(rng_factor))
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "ReplicaCount %d (1..%d), InternalResultNum %d (1..2048) or SSDIndexFileNum %d",
-                    replicas, kSpannBuildMaxReplicas, k, file_num);
-
     SpannBuildState st;
-    const std::string head_dir = dir + "/" + get("Base", "HeadIndexFolder", "HeadIndex");
-    if (int rc = sptag_b200_load(head_dir.c_str(), device, 0, &st.head)) return rc;
-    sptag_b200_handle h = st.head;
-    if (h->q_type != 0 || h->value_type != value_type || h->metric != metric)
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "the head index's value type or distance does not match the folder's");
-    if (h->dim != dim) return fail(SPTAG_B200_DIMENSION_MISMATCH, "vectors have %d dimensions, the head index %d", dim, h->dim);
-    // SPANNIndex.cpp:901: the head searches with [BuildSSDIndex] MaxCheck
-    if (int rc = sptag_b200_set_param(h, "MaxCheck", max_check.c_str())) return rc;
-    const int num_heads = h->n;
-    // SPANNIndex.cpp:914-925: with ExcludeHead false every head id becomes MaxSize, so that no vector is skipped
-    const std::string id_path = dir + "/" + get("Base", "HeadVectorIDs", "SPTAGHeadVectorIDs.bin");
-    if (!exclude_head) {
-        FILE* f = std::fopen(id_path.c_str(), "wb");
-        if (!f) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot write %s", id_path.c_str());
-        const std::vector<uint64_t> ids((size_t)num_heads, (uint64_t)INT_MAX);
-        const bool ok = std::fwrite(ids.data(), 8, ids.size(), f) == ids.size();
-        if (std::fclose(f) != 0 || !ok) return fail(SPTAG_B200_FAIL, "writing %s failed", id_path.c_str());
-    }
-    // the head-id set: every uint64 of the file cast to SizeType (ExtraFullGraphSearcher.h:604-616)
-    std::vector<unsigned char> is_head((size_t)num, 0);
-    {
-        std::vector<char> blob;
-        if (!read_file(id_path, blob)) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot read %s", id_path.c_str());
-        for (size_t i = 0; i + 8 <= blob.size(); i += 8) {
-            uint64_t v;
-            memcpy(&v, blob.data() + i, 8);
-            const int32_t id = (int32_t)(uint32_t)v;
-            if (id >= 0 && id < num) is_head[(size_t)id] = 1;
-        }
-    }
-    const size_t edges = (size_t)num * replicas;
+    SpannBuildConfig c;
+    if (int rc = spann_build_prepare(folder, vectors, num, dim, normalized, device, st, c)) return rc;
+    const size_t edges = (size_t)num * c.replicas;
     if (edges > (size_t)INT_MAX) return fail(SPTAG_B200_MEMORY_OVERFLOW, "%zu edges: more than 2^31 - 1", edges);
-    const size_t row_bytes = (size_t)dim * value_size(value_type);
-    const int vis = (int)row_bytes + 4;
+    int64_t stats[8];
+    if (int rc = spann_build_resident(c, st, vectors, stats)) return rc;
+    if (out_stats) memcpy(out_stats, stats, sizeof(stats));
+    return SPTAG_B200_SUCCESS;
+}
 
-    DeviceGuard guard(h->device);
-    CUDA_OK(cudaStreamCreateWithFlags(&st.stream, cudaStreamNonBlocking));
-    for (cudaEvent_t& e : st.ev) CUDA_OK(cudaEventCreate(&e));
-    cudaStream_t stream = st.stream;
-    const int kBatch = 1 << 16;
-    const int batch = std::min(num, kBatch);
-    if (int rc = st.d_rows.ensure((size_t)num * row_bytes)) return rc;
-    for (int i = 0; i < 2; ++i) {
-        if (int rc = st.d_keys[i].ensure(edges * 8)) return rc;
-        if (int rc = st.d_tonode[i].ensure(edges * 4)) return rc;
+int sptag_b200_spann_build_ex(const char* folder, const void* vectors, int32_t num, int32_t dim, int32_t normalized,
+                              int32_t device, const sptag_b200_spann_build_options* options, int64_t* out_stats) {
+    long long budget = -1;
+    if (options) {
+        if (options->struct_size != (int32_t)sizeof(sptag_b200_spann_build_options))
+            return fail(SPTAG_B200_FAIL, "options size mismatch: %d vs %zu", options->struct_size,
+                        sizeof(sptag_b200_spann_build_options));
+        budget = options->device_budget_bytes;
+        if (budget < -1) return fail(SPTAG_B200_LACK_OF_INPUTS, "device_budget_bytes %lld is below -1", budget);
     }
-    if (int rc = st.d_head.ensure((size_t)num)) return rc;
-    if (int rc = st.d_list.ensure(((size_t)batch + 1) * 4)) return rc;
-    if (int rc = st.d_ids.ensure((size_t)batch * k * 4)) return rc;
-    if (int rc = st.d_dists.ensure((size_t)batch * k * 4)) return rc;
-    if (int rc = st.d_size.ensure((size_t)num_heads * 4 + 4)) return rc;
-    if (int rc = st.d_counters.ensure(16)) return rc;  // rejections (uint64), the non-finite flag
-    unsigned long long* d_rejected = (unsigned long long*)st.d_counters.ptr;
-    int* d_bad = (int*)((unsigned char*)st.d_counters.ptr + 8);
-    CUDA_OK(cudaMemsetAsync(st.d_counters.ptr, 0, 16, stream));
-    CUDA_OK(cudaMemsetAsync(st.d_size.ptr, 0, (size_t)num_heads * 4, stream));
-    CUDA_OK(cudaMemcpyAsync(st.d_head.ptr, is_head.data(), (size_t)num, cudaMemcpyHostToDevice, stream));
-    ArraySource src;
-    src.ptr = vectors;
-    if (int rc = upload_rows(src, st.d_rows.ptr, (size_t)num, row_bytes, row_bytes, stream)) return rc;
-    unsigned char* rows = (unsigned char*)st.d_rows.ptr;
-    // sort and NaN have no order (std::sort under NaN is undefined): rows must be finite
-    if (value_type == SPTAG_B200_VT_FLOAT) {
-        CUDA_OK(launch_spann_nonfinite_check((const float*)rows, (size_t)num * dim, d_bad, stream));
-        int bad = 0;
-        CUDA_OK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, stream));
-        CUDA_OK(cudaStreamSynchronize(stream));
-        if (bad) return fail(SPTAG_B200_LACK_OF_INPUTS, "a row holds a NaN or an infinity");
+    SpannBuildState st;
+    SpannBuildConfig c;
+    if (int rc = spann_build_prepare(folder, vectors, num, dim, normalized, device, st, c)) return rc;
+    DeviceGuard guard(st.head->device);
+    if (budget == -1) {  // AUTO's reserve (sptag_b200_spann_load_ex)
+        size_t free_b = 0, total_b = 0;
+        CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
+        budget = std::max<long long>(0, (long long)free_b - (1ll << 30));
     }
-    // ExtraFullGraphSearcher.h:650: Cosine rows are normalised unless the caller says they are
-    if (metric == SPTAG_B200_METRIC_COSINE && !normalized) {
-        const int base = value_base(value_type);
-        with_elem(h, [&](auto el) {
-            normalize_rows_kernel<typename decltype(el)::type><<<(unsigned)((num + 127) / 128), 128, 0, stream>>>(
-                rows, row_bytes, 0, num, dim, base);
-        });
-        g_launches++;
-        CUDA_OK(cudaGetLastError());
+    const long long edges = (long long)num * c.replicas;
+    int64_t stats[12] = {0};
+    if (edges <= INT_MAX && spann_resident_bytes(c, nullptr) <= budget) {
+        if (int rc = spann_build_resident(c, st, vectors, stats)) return rc;
+        stats[8] = 0;
+        stats[9] = (num + (1 << 16) - 1) >> 16;
+        stats[10] = 1;
+        stats[11] = (long long)num * (long long)c.row_bytes;
+    } else if (int rc = spann_build_streamed(c, st, vectors, budget, stats)) {
+        return rc;
     }
-    // ApproximateRNG in batches of rows: the head search at K = InternalResultNum for the batch's non-head rows (queries
-    // read in place through the query list), then the RNG selection of the whole batch
-    const MetricElem me = metric_elem(h);
-    float ms_search = 0, ms_rng = 0, ms_sort = 0;
-    long long searched = 0;
-    std::vector<unsigned int> list((size_t)batch + 1);
-    SpannRngParams rp;
-    memset(&rp, 0, sizeof(rp));
-    rp.res_ids = (const int*)st.d_ids.ptr;
-    rp.res_dists = (const float*)st.d_dists.ptr;
-    rp.k = k;
-    rp.head = (const unsigned char*)st.d_head.ptr;
-    rp.rows = (const unsigned char*)h->d_vectors.ptr;
-    rp.row_stride = h->row_stride;
-    rp.dim = dim;
-    rp.simd_width = h->simd_width;
-    rp.replicas = replicas;
-    rp.num_heads = num_heads;
-    rp.rng_factor = rng_factor;
-    rp.keys = (unsigned long long*)st.d_keys[0].ptr;
-    rp.tonode = (int*)st.d_tonode[0].ptr;
-    rp.list_size = (int*)st.d_size.ptr;
-    rp.rejected = d_rejected;
-    rp.bad = d_bad;
-    for (int b0 = 0; b0 < num; b0 += batch) {
-        const int nb = std::min(batch, num - b0);
-        unsigned int c = 0;
-        for (int i = 0; i < nb; ++i)
-            if (!is_head[(size_t)b0 + i]) list[1 + c++] = (unsigned int)i;
-        list[0] = c;
-        searched += c;
-        CUDA_OK(cudaMemcpyAsync(st.d_list.ptr, list.data(), ((size_t)c + 1) * 4, cudaMemcpyHostToDevice, stream));
-        CUDA_OK(cudaEventRecord(st.ev[0], stream));
-        if (c > 0) {
-            CallOpts opts;
-            opts.search_deleted = 0;
-            opts.d_query_list = (const unsigned int*)st.d_list.ptr;
-            std::lock_guard<std::mutex> lock(h->mu);
-            if (int rc = search_device_impl(h, rows + (size_t)b0 * row_bytes, nb, k, (int*)st.d_ids.ptr,
-                                            (float*)st.d_dists.ptr, nullptr, stream, false, opts))
-                return rc;
-        }
-        CUDA_OK(cudaEventRecord(st.ev[1], stream));
-        if (int rc = st.elapsed(ms_search)) return rc;  // also frees `list` for the next batch
-        rp.first = b0;
-        rp.num = nb;
-        CUDA_OK(cudaEventRecord(st.ev[0], stream));
-        CUDA_OK(launch_spann_rng_select(rp, me.cosine, me.elem, stream));
-        g_launches++;
-        CUDA_OK(cudaEventRecord(st.ev[1], stream));
-        if (int rc = st.elapsed(ms_rng)) return rc;
-    }
-    int bad = 0;
-    unsigned long long rejected = 0;
-    CUDA_OK(cudaMemcpy(&bad, d_bad, 4, cudaMemcpyDeviceToHost));
-    CUDA_OK(cudaMemcpy(&rejected, d_rejected, 8, cudaMemcpyDeviceToHost));
-    if (bad) return fail(SPTAG_B200_LACK_OF_INPUTS, "a distance is not finite");
-    // SortSelections: node, then distance, then tonode; unfilled edges (node = num_heads) last
-    int end_bit = 32;
-    while (end_bit < 64 && ((unsigned long long)num_heads >> (end_bit - 32)) != 0) ++end_bit;
-    size_t temp_bytes = 0;
-    CUDA_OK(spann_sort_edges(nullptr, &temp_bytes, nullptr, nullptr, nullptr, nullptr, (int)edges, end_bit, stream));
-    if (int rc = st.d_temp.ensure(std::max<size_t>(temp_bytes, 1))) return rc;
-    CUDA_OK(cudaEventRecord(st.ev[0], stream));
-    CUDA_OK(spann_sort_edges(st.d_temp.ptr, &temp_bytes, (const unsigned long long*)st.d_keys[0].ptr,
-                             (unsigned long long*)st.d_keys[1].ptr, (const int*)st.d_tonode[0].ptr, (int*)st.d_tonode[1].ptr,
-                             (int)edges, end_bit, stream));
-    g_launches++;
-    CUDA_OK(cudaEventRecord(st.ev[1], stream));
-    if (int rc = st.elapsed(ms_sort)) return rc;
-    st.d_keys[0].release();
-    st.d_tonode[0].release();
-    st.d_temp.release();
-    // the posting cut (ExtraFullGraphSearcher.h:722-760): PostingPageLimit is first raised to the pages of
-    // PostingVectorLimit elements; each list keeps its first limit elements
-    std::vector<int> size((size_t)num_heads);
-    CUDA_OK(cudaMemcpy(size.data(), st.d_size.ptr, (size_t)num_heads * 4, cudaMemcpyDeviceToHost));
-    long long limit = INT_MAX;
-    if (page_limit > 0) {
-        page_limit = std::max(page_limit, (int)((vector_limit * vis + 4095) / 4096));
-        limit = (long long)page_limit * 4096 / vis;
-    }
-    std::vector<long long> edge_off((size_t)num_heads);
-    std::vector<int> count((size_t)num_heads);
-    long long before = 0, after = 0;
-    for (int l = 0; l < num_heads; ++l) {
-        edge_off[l] = before;
-        before += size[l];
-        count[l] = (int)std::min<long long>(size[l], limit);
-        after += count[l];
-    }
-    // SSDIndexFileNum files of ceil(lists / files) lists each (ExtraFullGraphSearcher.h:796-802)
-    const auto t0 = std::chrono::steady_clock::now();
-    const int per_file = (num_heads + file_num - 1) / file_num;
-    if ((long long)(file_num - 1) * per_file > num_heads)
-        return fail(SPTAG_B200_LACK_OF_INPUTS, "SSDIndexFileNum %d leaves a file without lists", file_num);
-    SpannBuildFile bf;
-    bf.d_tonode = (const int*)st.d_tonode[1].ptr;
-    bf.d_rows = rows;
-    bf.row_bytes = (int)row_bytes;
-    bf.rearranged = rearranged;
-    bf.num_vectors = num;
-    bf.dim = dim;
-    bf.edge_off = &edge_off;
-    bf.count = &count;
-    const std::string out = dir + "/" + get("Base", "SSDIndex", "SPTAGFullList.bin");
-    for (int i = 0; i < file_num; ++i) {
-        const int first = i * per_file, nl = std::min(num_heads, first + per_file) - first;
-        if (int rc = write_posting_file(bf, i == 0 ? out : out + "_" + std::to_string(i), first, nl, stream)) return rc;
-    }
-    const double ms_write = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    if (out_stats) {
-        const int64_t stats[8] = {searched, (int64_t)rejected, before, after, (int64_t)(ms_search * 1000.0),
-                                  (int64_t)(ms_rng * 1000.0), (int64_t)(ms_sort * 1000.0), (int64_t)(ms_write * 1000.0)};
-        memcpy(out_stats, stats, sizeof(stats));
-    }
+    if (out_stats) memcpy(out_stats, stats, sizeof(stats));
     return SPTAG_B200_SUCCESS;
 }
 
