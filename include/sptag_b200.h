@@ -564,6 +564,58 @@ int sptag_b200_spann_cache_warm(sptag_b200_spann_handle s, const void* queries, 
  * MemoryOverFlow when the allocation fails, after which the handle works uncached. */
 int sptag_b200_spann_cache_lists(sptag_b200_spann_handle s, const int32_t* lists, int32_t num_lists);
 
+/* ---- SPANN on several GPUs of one host ----
+ * Replaces: N processes of SPANN::Index<T> on one folder, one per GPU (VectorIndex::LoadIndex, SPANNIndex.cpp:59-140,
+ * SearchIndex, :193-250); the reference has no single call for it.  A group holds one pinned copy of the posting lists
+ * for all its members, and an HBM cache of lists spread over them.
+ *   load:   devices: 1 to 16 CUDA ordinals, one member each (a device may repeat).  The folder's posting files are read
+ *           once, as sptag_b200_spann_load_ex reads them, into one pinned allocation that every device maps
+ *           (cudaHostAlloc, mapped and portable; the HOST placement's layout).  Each member is a HOST-placed handle with
+ *           its own head (sptag_b200_load on its device), translate map, list offsets, counts and page counts, and
+ *           staging sets.  Peer access is enabled both ways between the members' devices where the hardware allows it.
+ *           Codes: sptag_b200_spann_load_ex's refusals with the same codes, LackOfInputs for a null or empty device
+ *           list or more than 16 entries, Fail for a device that does not exist.
+ *   member: member i's handle, borrowed: sptag_b200_spann_search, the iterators, get_param and set_param work on it as
+ *           on any HOST-placed handle; sptag_b200_spann_destroy on it does nothing; sptag_b200_spann_cache_warm and
+ *           sptag_b200_spann_cache_lists on it return LackOfInputs (its peers read its cache).  LackOfInputs for i
+ *           outside [0, members).
+ *   set_param:  sptag_b200_spann_set_param on every member in turn, under the group's lock; the first failure's code.
+ *   search: sptag_b200_spann_search's arguments.  Member i searches queries [i * ceil(Q / n), (i + 1) * ceil(Q / n)) on a
+ *           thread of its own; outputs are written in place, out_stats (HOST [num_queries x 3] int64 or NULL) as
+ *           sptag_b200_spann_search's.  A query's result does not depend on which member runs it, and equals the
+ *           reference's bit for bit.  LackOfInputs when the members differ in SearchInternalResultNum, MaxDistRatio,
+ *           SearchPostingPageLimit or MaxCheck (one was set on its own); otherwise the first failing member's code.
+ *   cache_warm: ranks the lists as sptag_b200_spann_cache_warm does, on member 0's head, then walks the ranking: each
+ *           list goes to the member with the most budget left (the lower index of equals) if its full size, element
+ *           count x (row stride + 4) bytes, fits there, and is skipped otherwise.  budget_bytes_per_member -1: each
+ *           member's free HBM after its cache is released, less 1 GB (members sharing a device each count all of its
+ *           free HBM).  The lists are installed, and written in rank order to out_lists with their members to
+ *           out_owners (HOST, at most capacity; *out_n receives how many were taken).  Codes as
+ *           sptag_b200_spann_cache_warm's.
+ *   cache_lists: caches list lists[i] on member owners[i] (HOST); n = 0 releases every member's cache.  LackOfInputs
+ *           for a list outside the range or given twice, an owner outside [0, members) and a null buffer.
+ * Every list is cached on at most one member.  A member copies a list it does not cache from the pool of the member
+ * that caches it when both are on one device or peer access reaches it (HBM or NVLink), and from the pinned allocation
+ * otherwise; B200.LastGatherBytes and B200.LastGatherRounds count both, over the lists the member does not cache
+ * itself, exactly as on a single handle.  Read-only member parameters: B200.PostingPeerLists (lists the member reads from
+ * a peer's cache) and B200.LastPeerGatherBytes (the part of B200.LastGatherBytes copied from peers; the rest crossed the
+ * host link).  A cache install on any member (these calls, or a stage that grows with B200.PostingStageBytes,
+ * SearchInternalResultNum or the page limit) waits until no search or iterator step runs on any member.
+ *   destroy: destroys every member and frees the pinned allocation. */
+typedef struct sptag_b200_spann_group* sptag_b200_spann_group_handle;
+int sptag_b200_spann_group_load(const char* folder, const int32_t* devices, int32_t num_members,
+                                sptag_b200_spann_group_handle* out);
+int sptag_b200_spann_group_member(sptag_b200_spann_group_handle g, int32_t i, sptag_b200_spann_handle* out);
+int sptag_b200_spann_group_set_param(sptag_b200_spann_group_handle g, const char* name, const char* value);
+int sptag_b200_spann_group_search(sptag_b200_spann_group_handle g, const void* queries, int32_t num_queries, int32_t k,
+                                  int32_t* out_ids, float* out_dists, int64_t* out_stats);
+int sptag_b200_spann_group_cache_warm(sptag_b200_spann_group_handle g, const void* queries, int32_t num_queries,
+                                      int64_t budget_bytes_per_member, int32_t* out_lists, int32_t* out_owners,
+                                      int32_t capacity, int32_t* out_n);
+int sptag_b200_spann_group_cache_lists(sptag_b200_spann_group_handle g, const int32_t* lists, const int32_t* owners,
+                                       int32_t n);
+void sptag_b200_spann_group_destroy(sptag_b200_spann_group_handle g);
+
 /* Replaces: SPANN::Index<T>::GetIterator(p_target) (SPANNIndex.cpp:299-314) and SPANNResultIterator::Next(batch)
  * (SPANNResultIterator.h:37-63, SPANNIndex.cpp:261-296, :416-446, ExtraFullGraphSearcher.h:131-147, :492-525) for every
  * query of a HOST batch, one iterator per query.

@@ -37,7 +37,9 @@ EXPORTS = [
     "sptag_b200_spann_set_param", "sptag_b200_spann_get_param", "sptag_b200_spann_iterator_open",
     "sptag_b200_spann_iterator_next", "sptag_b200_spann_iterator_close", "sptag_b200_multi_scan",
     "sptag_b200_spann_build", "sptag_b200_debug_kernel_for", "sptag_b200_spann_load_ex", "sptag_b200_spann_cache_warm",
-    "sptag_b200_spann_cache_lists", "sptag_b200_spann_build_ex",
+    "sptag_b200_spann_cache_lists", "sptag_b200_spann_build_ex", "sptag_b200_spann_group_load",
+    "sptag_b200_spann_group_member", "sptag_b200_spann_group_set_param", "sptag_b200_spann_group_search",
+    "sptag_b200_spann_group_cache_warm", "sptag_b200_spann_group_cache_lists", "sptag_b200_spann_group_destroy",
 ]
 
 
@@ -146,6 +148,16 @@ def lib():
                                                      C.c_void_p]
         L.sptag_b200_spann_iterator_close.argtypes = [C.c_void_p]
         L.sptag_b200_spann_iterator_close.restype = None
+        L.sptag_b200_spann_group_load.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]
+        L.sptag_b200_spann_group_member.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]
+        L.sptag_b200_spann_group_set_param.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p]
+        L.sptag_b200_spann_group_search.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p]
+        L.sptag_b200_spann_group_cache_warm.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
+                                                        C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]
+        L.sptag_b200_spann_group_cache_lists.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
+        L.sptag_b200_spann_group_destroy.argtypes = [C.c_void_p]
+        L.sptag_b200_spann_group_destroy.restype = None
         L.sptag_b200_multi_scan.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(C.c_void_p), C.c_void_p, C.c_int32,
                                             C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p]
@@ -498,8 +510,9 @@ class B200SpannIndex:
 
     STATS_PER_QUERY = 3  # postings scanned, list elements read, distances computed
 
-    def __init__(self, handle):
+    def __init__(self, handle, group=None):
         self._h = C.c_void_p(handle)
+        self._group = group  # a group member's owner (B200SpannGroup): kept alive, and close() does not destroy
 
     @classmethod
     def load(cls, folder, device=-1, posting_placement=None):
@@ -547,7 +560,8 @@ class B200SpannIndex:
 
     def close(self):
         if self._h:
-            lib().sptag_b200_spann_destroy(self._h)
+            if self._group is None:
+                lib().sptag_b200_spann_destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
@@ -637,6 +651,83 @@ class B200SpannIterators:
             self.close()
         except Exception:
             pass
+
+
+class B200SpannGroup:
+    """A SPANN index on several GPUs of one host (sptag_b200_spann_group_*): one pinned host copy of the posting lists
+    that every member maps, one member handle per device, and an HBM cache spread over the members so that each list is
+    cached at most once; a member gathers a list another member caches from that member's HBM."""
+
+    def __init__(self, handle, n):
+        self._h = C.c_void_p(handle)
+        self.members = []
+        for i in range(n):
+            m = C.c_void_p()
+            _check(lib().sptag_b200_spann_group_member(self._h, i, C.byref(m)))
+            self.members.append(B200SpannIndex(m.value, group=self))
+
+    @classmethod
+    def load(cls, folder, devices):
+        """Loads `folder` once into pinned host memory and opens one member per entry of `devices` (CUDA ordinals; one
+        may repeat)."""
+        devs = np.ascontiguousarray(devices, np.int32)
+        h = C.c_void_p()
+        _check(lib().sptag_b200_spann_group_load(os.fsencode(folder), devs.ctypes.data if len(devs) else None, len(devs),
+                                                 C.byref(h)))
+        return cls(h.value, len(devs))
+
+    def close(self):
+        if self._h:
+            for m in self.members:
+                m._h = C.c_void_p()
+            lib().sptag_b200_spann_group_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_param(self, name, value):
+        """set_param on every member"""
+        _check(lib().sptag_b200_spann_group_set_param(self._h, name.encode(), str(value).encode()))
+
+    def search(self, queries, k, want_stats=False):
+        """B200SpannIndex.search with the batch split into one contiguous slice per member: ids [nq, k], dists [nq, k]
+        (and stats [nq, 3] int64)."""
+        queries = np.ascontiguousarray(queries)
+        nq = queries.shape[0]
+        ids = np.empty((nq, k), np.int32)
+        dists = np.empty((nq, k), np.float32)
+        stats = np.zeros((nq, B200SpannIndex.STATS_PER_QUERY), np.int64) if want_stats else None
+        _check(lib().sptag_b200_spann_group_search(self._h, queries.ctypes.data, nq, k, ids.ctypes.data,
+                                                   dists.ctypes.data, stats.ctypes.data if want_stats else None))
+        return (ids, dists, stats) if want_stats else (ids, dists)
+
+    def cache_warm(self, queries, budget_bytes=-1):
+        """Ranks the lists as B200SpannIndex.cache_warm does and gives each, in rank order, to the member with the most
+        budget left that holds it whole (budget_bytes per member; -1: each member's free HBM less 1 GB); installs them and
+        returns (lists, owners), int32, in rank order."""
+        queries = np.ascontiguousarray(queries)
+        nq = queries.shape[0]
+        cap = max(nq * max(int(self.members[0].get_param("SearchInternalResultNum")), 1), 1)
+        lists = np.empty(cap, np.int32)
+        owners = np.empty(cap, np.int32)
+        n = C.c_int32()
+        _check(lib().sptag_b200_spann_group_cache_warm(self._h, queries.ctypes.data, nq, int(budget_bytes),
+                                                       lists.ctypes.data, owners.ctypes.data, cap, C.byref(n)))
+        if n.value > cap:  # SearchInternalResultNum was raised during the call
+            raise RuntimeError("cache_warm installed %d lists, but only the first %d were returned" % (n.value, cap))
+        return lists[:n.value].copy(), owners[:n.value].copy()
+
+    def cache_lists(self, lists, owners):
+        """Caches list lists[i] on member owners[i] (empty: releases every member's cache)."""
+        lists = np.ascontiguousarray(lists, np.int32)
+        owners = np.ascontiguousarray(owners, np.int32)
+        if lists.shape != owners.shape:
+            raise ValueError("one owner per list")
+        _check(lib().sptag_b200_spann_group_cache_lists(self._h, lists.ctypes.data, owners.ctypes.data, len(lists)))
 
 
 def multi_scan(indexes, queries, k, *, term_cond, search_limit, weights=None, want_stats=False):

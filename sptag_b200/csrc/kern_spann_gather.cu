@@ -91,16 +91,31 @@ __global__ void spann_union_len_kernel(const PostingGather g) {
 }
 
 // One CTA per union list at a time: its rows as 16-byte words (row_stride is a multiple of 16), kUnroll loads in flight
-// per thread before their stores, then its ids
+// per thread before their stores, then its ids.  PEERS: a list g.peers.first places in a peer's pool is read from
+// there (HBM of the same device, or over NVLink), the others from mapped host memory.
 constexpr int kGatherThreads = 256;
 constexpr int kUnroll = 8;
+template <bool PEERS>
 __global__ void __launch_bounds__(kGatherThreads) spann_gather_kernel(const PostingGather g) {
     const int n = *g.nlists;
     const long long words_per_row = (long long)(g.host.row_stride / 16);
     for (int u = blockIdx.x; u < n; u += gridDim.x) {
         const int l = g.lists[u];
-        const long long from = g.host.off[l], to = g.stage_off[l], c = g.len[l];
-        const uint4* src = reinterpret_cast<const uint4*>(g.host.rows) + from * words_per_row;
+        long long from = g.host.off[l];
+        const long long to = g.stage_off[l], c = g.len[l];
+        const unsigned char* rows = g.host.rows;
+        const int* ids = g.host.ids;
+        if (PEERS) {
+            const long long first = g.peers.first[l];
+            if (first >= 0) {
+                const int o = g.peers.owner[l];
+                from = first;
+                rows = g.peers.rows[o];
+                ids = g.peers.ids[o];
+                if (threadIdx.x == 0) atomicAdd(g.peers.elems, (unsigned long long)c);
+            }
+        }
+        const uint4* src = reinterpret_cast<const uint4*>(rows) + from * words_per_row;
         uint4* dst = reinterpret_cast<uint4*>(g.stage_rows) + to * words_per_row;
         const long long words = c * words_per_row;
         for (long long w0 = threadIdx.x; w0 < words; w0 += (long long)kUnroll * kGatherThreads) {
@@ -116,7 +131,7 @@ __global__ void __launch_bounds__(kGatherThreads) spann_gather_kernel(const Post
                 if (w < words) dst[w] = v[j];
             }
         }
-        for (long long i = threadIdx.x; i < c; i += kGatherThreads) g.stage_ids[to + i] = g.host.ids[from + i];
+        for (long long i = threadIdx.x; i < c; i += kGatherThreads) g.stage_ids[to + i] = ids[from + i];
     }
 }
 
@@ -190,7 +205,10 @@ cudaError_t launch_spann_count(const int* chosen, const int* nchosen, int stride
 }
 
 cudaError_t launch_spann_gather(const PostingGather& g, int grid, cudaStream_t stream) {
-    spann_gather_kernel<<<grid, kGatherThreads, 0, stream>>>(g);
+    if (g.peers.first)
+        spann_gather_kernel<true><<<grid, kGatherThreads, 0, stream>>>(g);
+    else
+        spann_gather_kernel<false><<<grid, kGatherThreads, 0, stream>>>(g);
     return cudaGetLastError();
 }
 

@@ -135,6 +135,17 @@ int spann_iter_step_blocks_per_sm(bool cosine, int elem, int cap);
 // share one allocation and one element space: `resident` holds a cached list's first element there (-1: not cached),
 // the union takes the other lists only, the stage starts at element stage_base (stage_rows / stage_ids point there), and
 // the kernels read a view of the whole allocation with off = view_off.
+// A member of a SPANN group (sptag_b200_spann_group_load) also has `peers`: a union list that another member caches
+// (same device, or one peer access reaches) is copied from that member's pool instead of from host memory.
+constexpr int kMaxSpannPeers = 16;
+struct PostingPeers {
+    const long long* first;  // [num_lists] the list's first element in its owner's pool, -1: read from host memory
+                             // (nullptr: no list is, and the host-only gather runs)
+    const int* owner;        // [num_lists] the member that caches it
+    const unsigned char* rows[kMaxSpannPeers];  // per member, its pool's rows and ids (element space of its cache)
+    const int* ids[kMaxSpannPeers];
+    unsigned long long* elems;  // += the elements copied from peers
+};
 struct PostingGather {
     PostingLists host;
     int num_lists;
@@ -151,6 +162,7 @@ struct PostingGather {
     const long long* resident;  // [num_lists], or nullptr without a cache
     long long stage_base;
     long long* view_off;        // [num_lists] with a cache: resident[l], or stage_base + stage_off[l]
+    PostingPeers peers;
 };
 size_t spann_union_temp_bytes(int num_lists);
 // chosen[q * stride ...] / nchosen[q]: the lists query q of a search reads (choose_postings), for every query of p
@@ -164,8 +176,8 @@ cudaError_t launch_spann_iter_chosen(const SpannIterParams& p, int b, int e, int
 // g.nlists (and with a cache g.view_off).  g.stage_off[g.num_lists] is the union's element count.
 cudaError_t launch_spann_union(const PostingGather& g, const int* chosen, const int* nchosen, int stride, int n,
                                cudaStream_t stream);
-// Copies g.len[l] elements of every list l of g.lists (the union: its searched prefix) from host memory to element
-// g.stage_off[l] of the stage
+// Copies g.len[l] elements of every list l of g.lists (the union: its searched prefix) from host memory, or with
+// g.peers.first from the peer that caches it, to element g.stage_off[l] of the stage
 cudaError_t launch_spann_gather(const PostingGather& g, int grid, cudaStream_t stream);
 // counts[l] += the items (chosen / nchosen as above) that read list l
 cudaError_t launch_spann_count(const int* chosen, const int* nchosen, int stride, int n, int* counts, cudaStream_t stream);

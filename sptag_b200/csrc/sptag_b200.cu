@@ -35,6 +35,7 @@
 #include <sys/stat.h>
 #include <sstream>
 #include <string>
+#include <thread>
 #include <type_traits>
 #include <utility>
 #include <vector>
@@ -686,7 +687,10 @@ int lay_out(const sptag_b200_index* h, int nq, SearchLaunch& L) {
         L.kern = pick_kernel(h, p.mres_cap, want_slots, sketch);
         if (!L.kern)
             return fail(SPTAG_B200_LACK_OF_INPUTS, "max(MaxCheck/16, K) = %d exceeds what this index type supports (2048; quantized: 1024)", p.mres_cap);
-        CUDA_OK(cudaFuncSetAttribute((const void*)L.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
+        // the opt-in maximum, one value for every call: handles that share an instantiation (a SPANN group's heads)
+        // plan their launches on several threads, and a smaller value set between another thread's plan and its launch
+        // would fail that launch
+        CUDA_OK(cudaFuncSetAttribute((const void*)L.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
         // resident single-warp CTAs per SM allowed by registers + shared memory for this instantiation
         int fit = 0;
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, (const void*)L.kern, 32, L.smem));
@@ -2901,9 +2905,29 @@ struct sptag_b200_spann {
         // host placement: the chosen lists per item, the union (PostingGather), an iterator launch's sub-list, the stage
         DeviceBuffer d_chosen, d_nchosen, d_flags, d_len, d_stage_off, d_union, d_nunion, d_cub, d_sub, d_stage;
         DeviceBuffer d_view_off;  // with a cache: the view's list offsets
+        DeviceBuffer d_peer_elems;  // a group member's: the elements a call copied from peers
     };
     StagingPool<StagingBuffers> staging;
     std::mutex mu;  // the search parameters
+    // A member of a SPANN group (sptag_b200_spann_group_load): the group owns the handle and the pinned allocation
+    // (h_postings stays null here).  Its peer table (spann_group_peer_tables, rebuilt with every member's staging sets
+    // held, so that a call holding one set sees a fixed table): per list the member that caches it and its first element
+    // there, per member the pool's rows and ids; peers.first is null when no reachable peer caches a list.
+    sptag_b200_spann_group* group = nullptr;
+    DeviceBuffer d_peer_first, d_peer_owner;
+    PostingPeers peers = {};
+    long peer_lists = 0;
+    long last_peer_gather_bytes = 0;
+};
+
+// A SPANN group: members on one or more devices that share one pinned copy of the posting lists, and whose HBM caches
+// hold each list at most once.  reach[i][o]: member i reads member o's pool (the same device, or peer access enabled).
+struct sptag_b200_spann_group {
+    std::vector<sptag_b200_spann*> members;
+    std::vector<std::vector<char>> reach;
+    void* h_postings = nullptr;
+    std::mutex install;  // taken by every install on a member, before every member's staging sets (GroupSets)
+    std::mutex params;   // sptag_b200_spann_group_set_param
 };
 
 namespace {
@@ -2963,10 +2987,10 @@ long long stage_elems(const sptag_b200_spann* s, const SpannSnapshot& sp) {
 // the next round starts from the same m.  choose(b, e, chosen, nchosen) points chosen / nchosen at the lists items
 // [b, e) read (stride apart), enqueued on stream; run(b, e, view) runs items [b, e) on the staged view.  The stage holds
 // the larger of B200.PostingStageBytes and one query's worst case.  Adds the bytes gathered and the rounds to bytes and
-// rounds.
+// rounds, and the part of those bytes a group member copied from peers' pools to peer_bytes.
 template <typename Buffers, typename Choose, typename Run>
 int gather_rounds(sptag_b200_spann* s, Buffers& sb, const SpannSnapshot& sp, int n, int stride, cudaStream_t stream,
-                  Choose&& choose, Run&& run, long& bytes, long& rounds) {
+                  Choose&& choose, Run&& run, long& bytes, long& rounds, long& peer_bytes) {
     const PostingLists host = posting_lists(s, sp.page_limit);
     const long long elem_bytes = (long long)host.row_stride + 4;
     const long long cap_elems = stage_elems(s, sp);
@@ -3020,6 +3044,13 @@ int gather_rounds(sptag_b200_spann* s, Buffers& sb, const SpannSnapshot& sp, int
         view.ids = ids;
         view.rows = rows;
     }
+    // the peer table is rebuilt only while every staging set of every member is held, so it is fixed during the call
+    if (s->peers.first) {
+        if (int rc = sb.d_peer_elems.ensure(8)) return rc;
+        g.peers = s->peers;
+        g.peers.elems = (unsigned long long*)sb.d_peer_elems.ptr;
+        CUDA_OK(cudaMemsetAsync(g.peers.elems, 0, 8, stream));
+    }
     const int grid = s->head->num_sms * 4;
     for (int b = 0, m = n; b < n; b += m) {
         m = std::min(m, n - b);
@@ -3041,6 +3072,12 @@ int gather_rounds(sptag_b200_spann* s, Buffers& sb, const SpannSnapshot& sp, int
         if (int rc = run(b, b + m, view)) return rc;
         bytes += (long)(elems * elem_bytes);
         ++rounds;
+    }
+    if (g.peers.first) {
+        unsigned long long from_peers = 0;
+        CUDA_OK(cudaMemcpyAsync(&from_peers, g.peers.elems, 8, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        peer_bytes += (long)((long long)from_peers * elem_bytes);
     }
     return 0;
 }
@@ -3133,27 +3170,105 @@ int spann_cache_install(sptag_b200_spann* s, const std::vector<int>& lists, long
     return rc;
 }
 
+// Every member's two staging sets, in member order then set order, under the group's install mutex: what an install on
+// a group member holds, since its peers read its pool.  A search or iterator step holds one set of one member at a
+// time and takes no other lock while it does, so this order cannot deadlock.
+struct GroupSets {
+    std::unique_lock<std::mutex> install;
+    std::vector<std::unique_lock<std::mutex>> sets;
+    explicit GroupSets(sptag_b200_spann_group* g) : install(g->install) {
+        for (sptag_b200_spann* m : g->members)
+            for (auto& set : m->staging.sets) sets.emplace_back(set.mu);
+    }
+};
+
+// Rebuilds every member's peer table from the members' caches (spann_cache_copy's pool layout: the lists whole, in
+// cache_lists order).  A member whose table cannot be uploaded reads every list it does not cache from host memory.
+// Caller holds GroupSets.
+int spann_group_peer_tables(sptag_b200_spann_group* g) {
+    const size_t n = g->members.size(), nl = (size_t)g->members[0]->num_lists;
+    std::vector<int> owner(nl, -1);
+    std::vector<long long> first(nl, -1);
+    PostingPeers pools = {};
+    for (size_t o = 0; o < n; ++o) {
+        const sptag_b200_spann* m = g->members[o];
+        if (!m->d_cache.ptr) continue;
+        long long pos = 0;
+        for (int l : m->cache_lists) {
+            owner[l] = (int)o;
+            first[l] = pos;
+            pos += m->cnt[l];
+        }
+        pools.rows[o] = (const unsigned char*)m->d_cache.ptr;
+        pools.ids[o] = (const int*)(pools.rows[o] + (size_t)(m->cache_pool + 2 * m->cache_stage) * m->head->row_stride);
+    }
+    int rc = 0;
+    for (size_t i = 0; i < n; ++i) {
+        sptag_b200_spann* s = g->members[i];
+        std::vector<long long> from(nl, -1);
+        std::vector<int> by(nl, 0);
+        long count = 0;
+        for (size_t l = 0; l < nl; ++l) {
+            if (owner[l] < 0 || owner[l] == (int)i || !g->reach[i][(size_t)owner[l]]) continue;
+            from[l] = first[l];
+            by[l] = owner[l];
+            ++count;
+        }
+        PostingPeers p = pools;
+        p.first = nullptr;
+        p.owner = nullptr;
+        int r = 0;
+        if (count > 0) {
+            DeviceGuard guard(s->head->device);
+            if (!(r = s->d_peer_first.ensure(nl * 8)) && !(r = s->d_peer_owner.ensure(nl * 4))) {
+                cudaError_t e = cudaMemcpy(s->d_peer_first.ptr, from.data(), nl * 8, cudaMemcpyHostToDevice);
+                if (e == cudaSuccess) e = cudaMemcpy(s->d_peer_owner.ptr, by.data(), nl * 4, cudaMemcpyHostToDevice);
+                if (e != cudaSuccess) r = fail(SPTAG_B200_FAIL, "peer table upload failed: %s", cudaGetErrorString(e));
+            }
+            if (!r) {
+                p.first = (const long long*)s->d_peer_first.ptr;
+                p.owner = (const int*)s->d_peer_owner.ptr;
+            }
+        }
+        if (r && !rc) rc = r;
+        std::lock_guard<std::mutex> lock(s->mu);
+        s->peers = p;
+        s->peer_lists = p.first ? count : 0;
+    }
+    return rc;
+}
+
 // Before a host-placed call takes its staging set: a cache whose stages are smaller than the call's (the stage
-// parameters grew since the install) is re-installed with the call's
+// parameters grew since the install) is re-installed with the call's.  Locks: the handle's two staging sets; on a group
+// member the group's install mutex and every member's sets (GroupSets), and every peer table is rebuilt before they
+// are released, since the member's pool moved.
 int spann_cache_fit(sptag_b200_spann* s, const SpannSnapshot& sp) {
     const long long need = stage_elems(s, sp);
     {
         std::lock_guard<std::mutex> lock(s->mu);
         if (s->cache_lists.empty() || s->cache_stage >= need) return 0;
     }
-    BothSets both(s);
+    std::unique_ptr<GroupSets> all;
+    std::unique_ptr<BothSets> both;
+    if (s->group)
+        all.reset(new GroupSets(s->group));
+    else
+        both.reset(new BothSets(s));
     std::vector<int> lists;
     {
         std::lock_guard<std::mutex> lock(s->mu);
         if (s->cache_lists.empty() || s->cache_stage >= need) return 0;
         lists = s->cache_lists;
     }
-    return spann_cache_install(s, lists, need);
+    const int rc = spann_cache_install(s, lists, need);
+    if (!s->group) return rc;
+    const int prc = spann_group_peer_tables(s->group);
+    return rc ? rc : prc;
 }
 
 // A host-placed call's staging set, with a cache (if any) whose stages hold the call's stage: the cache is fitted, the
 // set taken, and both again if an install from smaller stage parameters came in between (a cache's stage only grows,
-// so the second fit holds)
+// so the second fit holds).  The fit takes its locks (spann_cache_fit) and releases them before the set is taken.
 template <typename Set>
 int spann_acquire_fitted(sptag_b200_spann* s, const SpannSnapshot& sp, std::unique_lock<std::mutex>& slock, Set*& set) {
     for (;;) {
@@ -3192,6 +3307,10 @@ const Param<Spann> kSpannParams[] = {
     // the HBM cache of lists (sptag_b200_spann_cache_lists): its lists and the pool's bytes
     {"B200.PostingCacheLists", [](Spann* s, char* o, size_t n) { return put(o, n, "%zu", s->cache_lists.size()); }},
     {"B200.PostingCacheBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%lld", s->cache_bytes); }},
+    // a group member's (sptag_b200_spann_group_load): lists it reads from a peer's cache, and the part of
+    // B200.LastGatherBytes its last search or iterator step copied from peers
+    {"B200.PostingPeerLists", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->peer_lists); }},
+    {"B200.LastPeerGatherBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_peer_gather_bytes); }},
     {"B200.LastIteratorRounds", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_iter_rounds); }},
     {"B200.LastIteratorDedupBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_iter_dedup_bytes); }},
     {"B200.LastPostingKernel", [](Spann* s, char* o, size_t n) { return put(o, n, "%s", kernel_name(s->last_posting_kernel).c_str()); }},
@@ -3237,10 +3356,16 @@ int read_posting_header(FILE* f, PostingFile& pf, const char* name) {
 }
 
 
+// spann_fill's placement for a group's first member: HOST, in an allocation every device maps (cudaHostAllocPortable)
+constexpr int kPostingsPortable = -1;
+
 // Everything sptag_b200_spann_load reads after the head: the head's [BuildHead] parameters, the search parameters, the
-// translate map and the posting files, with the lists' rows and ids placed as `placement` says (SPTAG_B200_POSTINGS_*).
-// The caller destroys s on failure.
-int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& ini, int placement) {
+// translate map and the posting files, with the lists' rows and ids placed as `placement` says (SPTAG_B200_POSTINGS_*,
+// or kPostingsPortable).  With `shared` (a group's later members: the portable allocation of shared_bytes its first
+// member filled from the same folder) the lists' bodies are not read again: the handle maps that allocation, which it
+// does not own.  The caller destroys s on failure.
+int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& ini, int placement, void* shared = nullptr,
+               size_t shared_bytes = 0) {
     auto get = [&](const char* section, const char* name, const char* def) { return ini_get(ini, section, name, def); };
     sptag_b200_handle head = s->head;
     // SPANN::Index::LoadConfig hands every [BuildHead] entry to the head (SPANNIndex.cpp:59-71, :1033-1038)
@@ -3308,18 +3433,22 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
     }
     unsigned char* rows_base = nullptr;
     int32_t* ids_base = nullptr;
-    if (placement == SPTAG_B200_POSTINGS_HOST) {
+    if (shared && shared_bytes != rows_bytes + ids_bytes)
+        return fail(SPTAG_B200_FAIL, "the posting lists take %zu bytes, the group's first member loaded %zu",
+                    rows_bytes + ids_bytes, shared_bytes);
+    if (placement == SPTAG_B200_POSTINGS_HOST || placement == kPostingsPortable) {
         // the rows, then the ids (rows_bytes is a multiple of 16), in the layout they have in HBM
-        if (cudaHostAlloc(&s->h_postings, rows_bytes + ids_bytes, cudaHostAllocMapped) != cudaSuccess) {
+        const unsigned flags = placement == kPostingsPortable ? cudaHostAllocMapped | cudaHostAllocPortable : cudaHostAllocMapped;
+        if (!shared && cudaHostAlloc(&s->h_postings, rows_bytes + ids_bytes, flags) != cudaSuccess) {
             s->h_postings = nullptr;
             cudaGetLastError();
             return fail(SPTAG_B200_MEMORY_OVERFLOW, "cudaHostAlloc(%zu) of the posting lists failed", rows_bytes + ids_bytes);
         }
         s->host_postings = true;
         s->h_posting_bytes = rows_bytes + ids_bytes;
-        memset(s->h_postings, 0, rows_bytes);
+        if (!shared) memset(s->h_postings, 0, rows_bytes);
         void* dev = nullptr;
-        CUDA_OK(cudaHostGetDevicePointer(&dev, s->h_postings, 0));
+        CUDA_OK(cudaHostGetDevicePointer(&dev, shared ? shared : s->h_postings, 0));
         rows_base = (unsigned char*)dev;
         ids_base = (int32_t*)(rows_base + rows_bytes);
         s->h_rows = rows_base;
@@ -3335,6 +3464,11 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
     CUDA_OK(cudaMemcpy(s->d_off.ptr, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(s->d_cnt.ptr, s->cnt.data(), off.size() * 4, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(s->d_pages.ptr, s->pages.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    if (shared) {
+        std::lock_guard<std::mutex> lock(s->mu);
+        spann_update_shape(s);
+        return 0;
+    }
     // The lists of a file are read in file order, in runs of consecutive lists of at most kRun bytes (a longer list is a
     // run of its own), each run streamed through upload_rows' pinned chunks into one device staging buffer and split
     // there: ParsePostingList lays an element out as int32 id + row, ParsePostingListRearrange as every row of the list,
@@ -4308,42 +4442,11 @@ int spann_build_streamed(SpannBuildConfig& c, SpannBuildState& st, const void* v
     memcpy(stats, out, sizeof(out));
     return SPTAG_B200_SUCCESS;
 }
-}  // namespace
 
-extern "C" {
-
-void sptag_b200_spann_destroy(sptag_b200_spann_handle s) {
-    if (!s) return;
-    {
-        DeviceGuard guard(s->head ? s->head->device : 0);
-        cudaDeviceSynchronize();
-        sptag_b200_handle head = s->head;
-        if (s->h_postings) cudaFreeHost(s->h_postings);
-        delete s;  // frees the device buffers, with the index's device current
-        sptag_b200_destroy(head);
-    }
-}
-
-int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_handle* out) {
-    sptag_b200_spann_load_options o;
-    o.struct_size = (int32_t)sizeof(o);
-    o.posting_placement = SPTAG_B200_POSTINGS_DEVICE;
-    return sptag_b200_spann_load_ex(folder, device, &o, out);
-}
-
-int sptag_b200_spann_load_ex(const char* folder, int32_t device, const sptag_b200_spann_load_options* options,
-                             sptag_b200_spann_handle* out) {
-    if (!folder || !out) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
-    int placement = SPTAG_B200_POSTINGS_AUTO;
-    if (options) {
-        if (options->struct_size != (int32_t)sizeof(sptag_b200_spann_load_options))
-            return fail(SPTAG_B200_FAIL, "options size mismatch: %d vs %zu", options->struct_size,
-                        sizeof(sptag_b200_spann_load_options));
-        placement = options->posting_placement;
-        if (placement != SPTAG_B200_POSTINGS_AUTO && placement != SPTAG_B200_POSTINGS_DEVICE &&
-            placement != SPTAG_B200_POSTINGS_HOST)
-            return fail(SPTAG_B200_LACK_OF_INPUTS, "unknown posting placement %d", placement);
-    }
+// sptag_b200_spann_load_ex after its options: the folder's refusals, the head and spann_fill (shared, shared_bytes: a
+// group member's, as spann_fill takes them)
+int spann_open(const char* folder, int32_t device, int placement, void* shared, size_t shared_bytes,
+               sptag_b200_spann_handle* out) {
     *out = nullptr;
     const std::string dir(folder);
     IniSections ini;
@@ -4396,12 +4499,134 @@ int sptag_b200_spann_load_ex(const char* folder, int32_t device, const sptag_b20
         sptag_b200_spann_destroy(s);
         return fail(SPTAG_B200_LACK_OF_INPUTS, "head index value type %d does not match ValueType %s", head->value_type, vt.c_str());
     }
-    if (int rc = spann_fill(s, dir, ini, placement)) {
+    if (int rc = spann_fill(s, dir, ini, placement, shared, shared_bytes)) {
         sptag_b200_spann_destroy(s);
         return rc;
     }
     *out = s;
     return SPTAG_B200_SUCCESS;
+}
+
+// cache_warm's ranking (sptag_b200_spann_cache_warm): for each sample query the head search and posting choice of a
+// search with K <= SearchInternalResultNum, on staging set 0 of s, the lists counted on the device; order receives the
+// lists some query chose, by count, descending, then list id.  Caller holds both of s's staging sets and checked that
+// SearchInternalResultNum <= 2048.
+int spann_warm_order(sptag_b200_spann* s, const SpannSnapshot& sp, const void* queries, int32_t num_queries,
+                     std::vector<int>& order) {
+    sptag_b200_handle h = s->head;
+    const size_t nl = (size_t)s->num_lists, nq = (size_t)num_queries;
+    // a search's head search and posting choice at K <= SearchInternalResultNum, on staging set 0's buffers
+    const int w = std::max(sp.internal, 1);
+    std::vector<int> counts(nl, 0);
+    DeviceGuard guard(h->device);
+    auto& st = s->staging.sets[0];
+    cudaStream_t stream = st.stream;
+    if (nq > 0) {
+        DeviceBuffer d_counts;
+        if (int rc = st.d_q.ensure(nq * query_bytes(h))) return rc;
+        if (int rc = st.d_hids.ensure(nq * w * 4)) return rc;
+        if (int rc = st.d_hdists.ensure(nq * w * 4)) return rc;
+        if (int rc = st.d_chosen.ensure(nq * w * 4)) return rc;
+        if (int rc = st.d_nchosen.ensure(nq * 4)) return rc;
+        if (int rc = d_counts.ensure(nl * 4)) return rc;
+        CUDA_OK(cudaMemcpyAsync(st.d_q.ptr, queries, nq * query_bytes(h), cudaMemcpyHostToDevice, stream));
+        {
+            std::lock_guard<std::mutex> lock(h->mu);
+            if (int rc = search_device_impl(h, st.d_q.ptr, num_queries, w, (int*)st.d_hids.ptr, (float*)st.d_hdists.ptr,
+                                            nullptr, stream)) {
+                cudaStreamSynchronize(stream);
+                return rc;
+            }
+        }
+        SpannScanParams p;
+        memset(&p, 0, sizeof(p));
+        p.head_ids = (const int*)st.d_hids.ptr;
+        p.head_dists = (const float*)st.d_hdists.ptr;
+        p.nq = num_queries;
+        p.w = w;
+        p.k = w;
+        p.translate = (const int*)s->d_translate.ptr;
+        p.lists = posting_lists(s, sp.page_limit);
+        p.internal = sp.internal;
+        p.max_dist_ratio = sp.max_dist_ratio;
+        CUDA_OK(cudaMemsetAsync(d_counts.ptr, 0, nl * 4, stream));
+        CUDA_OK(launch_spann_choose(p, (int*)st.d_chosen.ptr, (int*)st.d_nchosen.ptr, w, stream));
+        CUDA_OK(launch_spann_count((const int*)st.d_chosen.ptr, (const int*)st.d_nchosen.ptr, w, num_queries,
+                                   (int*)d_counts.ptr, stream));
+        g_launches += 2;
+        CUDA_OK(cudaMemcpyAsync(counts.data(), d_counts.ptr, nl * 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+    }
+    order.clear();
+    for (size_t l = 0; l < nl; ++l)
+        if (counts[l] > 0) order.push_back((int)l);
+    std::sort(order.begin(), order.end(), [&](int a, int b) { return counts[a] != counts[b] ? counts[a] > counts[b] : a < b; });
+    return 0;
+}
+
+// cache_warm's budget: budget_bytes, or for -1 cudaMemGetInfo's free bytes on s's device less kPostingReserve
+int spann_warm_budget(const sptag_b200_spann* s, long long budget_bytes, long long& budget) {
+    budget = budget_bytes;
+    if (budget != -1) return 0;
+    DeviceGuard guard(s->head->device);
+    size_t free_bytes = 0, total_bytes = 0;
+    CUDA_OK(cudaMemGetInfo(&free_bytes, &total_bytes));
+    budget = std::max(0ll, (long long)free_bytes - kPostingReserve);
+    return 0;
+}
+
+// Installs lists[i] on member i of g (spann_cache_install, each with its own stage parameters), then rebuilds every
+// peer table.  Returns the first failure; the members installed before it keep their caches.  Caller holds GroupSets.
+int spann_group_install(sptag_b200_spann_group* g, const std::vector<std::vector<int>>& lists) {
+    int rc = 0;
+    for (size_t i = 0; i < g->members.size(); ++i) {
+        sptag_b200_spann* m = g->members[i];
+        SpannSnapshot sp;
+        spann_snapshot(m, sp);  // fills sp whether or not the page limit would refuse a search
+        const int r = spann_cache_install(m, lists[i], stage_elems(m, sp));
+        if (r && !rc) rc = r;
+    }
+    const int r = spann_group_peer_tables(g);
+    return rc ? rc : r;
+}
+
+}  // namespace
+
+extern "C" {
+
+void sptag_b200_spann_destroy(sptag_b200_spann_handle s) {
+    if (!s || s->group) return;  // a group member: the group owns it
+    {
+        DeviceGuard guard(s->head ? s->head->device : 0);
+        cudaDeviceSynchronize();
+        sptag_b200_handle head = s->head;
+        if (s->h_postings) cudaFreeHost(s->h_postings);
+        delete s;  // frees the device buffers, with the index's device current
+        sptag_b200_destroy(head);
+    }
+}
+
+int sptag_b200_spann_load(const char* folder, int32_t device, sptag_b200_spann_handle* out) {
+    sptag_b200_spann_load_options o;
+    o.struct_size = (int32_t)sizeof(o);
+    o.posting_placement = SPTAG_B200_POSTINGS_DEVICE;
+    return sptag_b200_spann_load_ex(folder, device, &o, out);
+}
+
+int sptag_b200_spann_load_ex(const char* folder, int32_t device, const sptag_b200_spann_load_options* options,
+                             sptag_b200_spann_handle* out) {
+    if (!folder || !out) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
+    int placement = SPTAG_B200_POSTINGS_AUTO;
+    if (options) {
+        if (options->struct_size != (int32_t)sizeof(sptag_b200_spann_load_options))
+            return fail(SPTAG_B200_FAIL, "options size mismatch: %d vs %zu", options->struct_size,
+                        sizeof(sptag_b200_spann_load_options));
+        placement = options->posting_placement;
+        if (placement != SPTAG_B200_POSTINGS_AUTO && placement != SPTAG_B200_POSTINGS_DEVICE &&
+            placement != SPTAG_B200_POSTINGS_HOST)
+            return fail(SPTAG_B200_LACK_OF_INPUTS, "unknown posting placement %d", placement);
+    }
+    return spann_open(folder, device, placement, nullptr, 0, out);
 }
 
 int sptag_b200_spann_build(const char* folder, const void* vectors, int32_t num, int32_t dim, int32_t normalized,
@@ -4558,7 +4783,7 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     if (s->host_postings) {
         // the queries' chosen lists, once; then the rounds, each a scan over its queries on the staged lists
         const int stride = std::max(p.internal, 1);
-        long bytes = 0, rounds = 0;
+        long bytes = 0, rounds = 0, peer_bytes = 0;
         int rc = 0;
         if (!(rc = st->d_chosen.ensure(nq * stride * 4)) && !(rc = st->d_nchosen.ensure(nq * 4))) {
             const cudaError_t e = launch_spann_choose(p, (int*)st->d_chosen.ptr, (int*)st->d_nchosen.ptr, stride, stream);
@@ -4589,7 +4814,7 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
             if (err != cudaSuccess) return fail(SPTAG_B200_FAIL, "posting scan launch failed: %s", cudaGetErrorString(err));
             return 0;
         };
-        if (!rc) rc = gather_rounds(s, *st, sp, num_queries, stride, stream, choose, run, bytes, rounds);
+        if (!rc) rc = gather_rounds(s, *st, sp, num_queries, stride, stream, choose, run, bytes, rounds, peer_bytes);
         if (rc) {
             cudaStreamSynchronize(stream);
             return rc;
@@ -4597,6 +4822,7 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
         std::lock_guard<std::mutex> lock(s->mu);
         s->last_gather_bytes = bytes;
         s->last_gather_rounds = rounds;
+        s->last_peer_gather_bytes = peer_bytes;
     } else {
         cudaError_t e = s->quantized ? launch_spann_pq_scan(pq, grid, stream, &kern)
                                      : launch_spann_scan(p, me.cosine, me.elem, grid, stream, &kern);
@@ -4637,71 +4863,25 @@ int sptag_b200_spann_cache_warm(sptag_b200_spann_handle s, const void* queries, 
                                 int32_t* out_lists, int32_t capacity, int32_t* out_num_lists) {
     if (!s) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
     if (!s->host_postings) return fail(SPTAG_B200_LACK_OF_INPUTS, "the HBM cache of posting lists needs the host placement");
+    if (s->group)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "a group member's cache is set by sptag_b200_spann_group_cache_warm / "
+                                               "_cache_lists: its peers read its pool");
     if (num_queries < 0 || (num_queries > 0 && !queries) || !out_num_lists || capacity < 0 || (capacity > 0 && !out_lists))
         return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
     if (budget_bytes < -1) return fail(SPTAG_B200_LACK_OF_INPUTS, "budget %lld below -1", (long long)budget_bytes);
     *out_num_lists = 0;
     SpannSnapshot sp;
     if (int rc = spann_snapshot(s, sp)) return rc;
-    sptag_b200_handle h = s->head;
-    const size_t nl = (size_t)s->num_lists, nq = (size_t)num_queries;
-    // a search's head search and posting choice at K <= SearchInternalResultNum, on staging set 0's buffers
-    const int w = std::max(sp.internal, 1);
-    if (w > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchInternalResultNum %d exceeds 2048", sp.internal);
-    std::vector<int> counts(nl, 0);
+    if (sp.internal > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchInternalResultNum %d exceeds 2048", sp.internal);
     BothSets both(s);
-    DeviceGuard guard(h->device);
-    auto& st = s->staging.sets[0];
-    cudaStream_t stream = st.stream;
-    if (nq > 0) {
-        DeviceBuffer d_counts;
-        if (int rc = st.d_q.ensure(nq * query_bytes(h))) return rc;
-        if (int rc = st.d_hids.ensure(nq * w * 4)) return rc;
-        if (int rc = st.d_hdists.ensure(nq * w * 4)) return rc;
-        if (int rc = st.d_chosen.ensure(nq * w * 4)) return rc;
-        if (int rc = st.d_nchosen.ensure(nq * 4)) return rc;
-        if (int rc = d_counts.ensure(nl * 4)) return rc;
-        CUDA_OK(cudaMemcpyAsync(st.d_q.ptr, queries, nq * query_bytes(h), cudaMemcpyHostToDevice, stream));
-        {
-            std::lock_guard<std::mutex> lock(h->mu);
-            if (int rc = search_device_impl(h, st.d_q.ptr, num_queries, w, (int*)st.d_hids.ptr, (float*)st.d_hdists.ptr,
-                                            nullptr, stream)) {
-                cudaStreamSynchronize(stream);
-                return rc;
-            }
-        }
-        SpannScanParams p;
-        memset(&p, 0, sizeof(p));
-        p.head_ids = (const int*)st.d_hids.ptr;
-        p.head_dists = (const float*)st.d_hdists.ptr;
-        p.nq = num_queries;
-        p.w = w;
-        p.k = w;
-        p.translate = (const int*)s->d_translate.ptr;
-        p.lists = posting_lists(s, sp.page_limit);
-        p.internal = sp.internal;
-        p.max_dist_ratio = sp.max_dist_ratio;
-        CUDA_OK(cudaMemsetAsync(d_counts.ptr, 0, nl * 4, stream));
-        CUDA_OK(launch_spann_choose(p, (int*)st.d_chosen.ptr, (int*)st.d_nchosen.ptr, w, stream));
-        CUDA_OK(launch_spann_count((const int*)st.d_chosen.ptr, (const int*)st.d_nchosen.ptr, w, num_queries,
-                                   (int*)d_counts.ptr, stream));
-        g_launches += 2;
-        CUDA_OK(cudaMemcpyAsync(counts.data(), d_counts.ptr, nl * 4, cudaMemcpyDeviceToHost, stream));
-        CUDA_OK(cudaStreamSynchronize(stream));
-    }
-    spann_cache_release(s);
-    long long budget = budget_bytes;
-    if (budget == -1) {
-        size_t free_bytes = 0, total_bytes = 0;
-        CUDA_OK(cudaMemGetInfo(&free_bytes, &total_bytes));
-        budget = std::max(0ll, (long long)free_bytes - kPostingReserve);
-    }
-    // by count, descending, then list id; each list that fits what is left of the budget, whole
+    DeviceGuard guard(s->head->device);
     std::vector<int> order;
-    for (size_t l = 0; l < nl; ++l)
-        if (counts[l] > 0) order.push_back((int)l);
-    std::sort(order.begin(), order.end(), [&](int a, int b) { return counts[a] != counts[b] ? counts[a] > counts[b] : a < b; });
-    const long long elem_bytes = (long long)h->row_stride + 4;
+    if (int rc = spann_warm_order(s, sp, queries, num_queries, order)) return rc;
+    spann_cache_release(s);
+    long long budget = 0;
+    if (int rc = spann_warm_budget(s, budget_bytes, budget)) return rc;
+    // in rank order, each list that fits what is left of the budget, whole
+    const long long elem_bytes = (long long)s->head->row_stride + 4;
     std::vector<int> taken;
     for (int l : order) {
         const long long bytes = (long long)s->cnt[l] * elem_bytes;
@@ -4718,6 +4898,9 @@ int sptag_b200_spann_cache_warm(sptag_b200_spann_handle s, const void* queries, 
 int sptag_b200_spann_cache_lists(sptag_b200_spann_handle s, const int32_t* lists, int32_t num_lists) {
     if (!s) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
     if (!s->host_postings) return fail(SPTAG_B200_LACK_OF_INPUTS, "the HBM cache of posting lists needs the host placement");
+    if (s->group)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "a group member's cache is set by sptag_b200_spann_group_cache_lists: its "
+                                               "peers read its pool");
     if (num_lists < 0 || (num_lists > 0 && !lists)) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
     std::vector<char> seen((size_t)s->num_lists, 0);
     for (int32_t i = 0; i < num_lists; ++i) {
@@ -4730,6 +4913,196 @@ int sptag_b200_spann_cache_lists(sptag_b200_spann_handle s, const int32_t* lists
     spann_snapshot(s, sp);  // fills sp whether or not the page limit would refuse a search
     BothSets both(s);
     return spann_cache_install(s, std::vector<int>(lists, lists + num_lists), stage_elems(s, sp));
+}
+
+void sptag_b200_spann_group_destroy(sptag_b200_spann_group_handle g) {
+    if (!g) return;
+    for (sptag_b200_spann* m : g->members) {
+        m->group = nullptr;
+        sptag_b200_spann_destroy(m);
+    }
+    if (g->h_postings) cudaFreeHost(g->h_postings);
+    delete g;
+}
+
+int sptag_b200_spann_group_load(const char* folder, const int32_t* devices, int32_t num_members,
+                                sptag_b200_spann_group_handle* out) {
+    if (!folder || !out) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
+    *out = nullptr;
+    if (num_members < 1 || num_members > kMaxSpannPeers)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "%d members outside [1, %d]", num_members, kMaxSpannPeers);
+    if (!devices) return fail(SPTAG_B200_LACK_OF_INPUTS, "null device list");
+    int count = 0;
+    if (cudaGetDeviceCount(&count) != cudaSuccess) {
+        cudaGetLastError();
+        count = 0;
+    }
+    for (int i = 0; i < num_members; ++i)
+        if (devices[i] < 0 || devices[i] >= count)
+            return fail(SPTAG_B200_FAIL, "member %d: device %d, %d devices visible", i, devices[i], count);
+    auto* g = new sptag_b200_spann_group();
+    for (int i = 0; i < num_members; ++i) {
+        // the first member reads the lists into a portable pinned allocation, which the group takes; the others map it
+        sptag_b200_spann_handle m = nullptr;
+        const size_t bytes = i ? g->members[0]->h_posting_bytes : 0;
+        if (int rc = spann_open(folder, devices[i], kPostingsPortable, g->h_postings, bytes, &m)) {
+            sptag_b200_spann_group_destroy(g);
+            return rc;
+        }
+        if (i == 0) g->h_postings = std::exchange(m->h_postings, nullptr);
+        m->group = g;
+        g->members.push_back(m);
+    }
+    // peer access both ways between the members' devices where the hardware allows it, as sptag_b200_group_create
+    // enables it; a member reads the pools of the members it reaches
+    const size_t n = g->members.size();
+    g->reach.assign(n, std::vector<char>(n, 0));
+    for (size_t i = 0; i < n; ++i) {
+        for (size_t o = 0; o < n; ++o) {
+            const int a = devices[i], b = devices[o];
+            int can = a == b;
+            if (!can && cudaDeviceCanAccessPeer(&can, a, b) == cudaSuccess && can) {
+                DeviceGuard guard(a);
+                const cudaError_t e = cudaDeviceEnablePeerAccess(b, 0);
+                can = e == cudaSuccess || e == cudaErrorPeerAccessAlreadyEnabled;
+            }
+            cudaGetLastError();
+            g->reach[i][o] = (char)(can ? 1 : 0);
+        }
+    }
+    *out = g;
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_spann_group_member(sptag_b200_spann_group_handle g, int32_t i, sptag_b200_spann_handle* out) {
+    if (!g) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (!out) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
+    if (i < 0 || i >= (int32_t)g->members.size())
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "member %d outside [0, %zu)", i, g->members.size());
+    *out = g->members[(size_t)i];
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_spann_group_set_param(sptag_b200_spann_group_handle g, const char* name, const char* value) {
+    if (!g) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (!name || !value) return fail(SPTAG_B200_LACK_OF_INPUTS, "null argument");
+    std::lock_guard<std::mutex> lock(g->params);
+    for (sptag_b200_spann* m : g->members)
+        if (int rc = sptag_b200_spann_set_param(m, name, value)) return rc;
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_spann_group_search(sptag_b200_spann_group_handle g, const void* queries, int32_t num_queries, int32_t k,
+                                  int32_t* out_ids, float* out_dists, int64_t* out_stats) {
+    if (!g) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (num_queries < 0 || (num_queries > 0 && (!queries || !out_ids || !out_dists)))
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    if (k < 1 || k > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "k = %d outside the supported range [1, 2048]", k);
+    // the members search with the same parameters, so that a query's result does not depend on which one runs it
+    for (const char* name : {"SearchInternalResultNum", "MaxDistRatio", "SearchPostingPageLimit", "MaxCheck"}) {
+        char first[64], other[64];
+        if (int rc = sptag_b200_spann_get_param(g->members[0], name, first, sizeof(first))) return rc;
+        for (size_t i = 1; i < g->members.size(); ++i) {
+            if (int rc = sptag_b200_spann_get_param(g->members[i], name, other, sizeof(other))) return rc;
+            if (strcmp(first, other) != 0)
+                return fail(SPTAG_B200_LACK_OF_INPUTS, "members 0 and %zu differ in %s: %s, %s", i, name, first, other);
+        }
+    }
+    if (num_queries == 0) return SPTAG_B200_SUCCESS;
+    // member i: queries [i * per, (i + 1) * per), on a thread of its own (a search blocks once per gather round)
+    const size_t n = g->members.size(), nq = (size_t)num_queries, per = (nq + n - 1) / n;
+    const size_t qrow = query_bytes(g->members[0]->head);
+    std::vector<int> rcs(n, 0);
+    std::vector<std::string> errors(n);
+    std::vector<std::thread> threads;
+    for (size_t i = 0; i < n && i * per < nq; ++i) {
+        threads.emplace_back([&, i] {
+            const size_t b = i * per, e = std::min(nq, b + per);
+            std::vector<int32_t> stats(out_stats ? (e - b) * 3 : 0);
+            rcs[i] = sptag_b200_spann_search(g->members[i], (const unsigned char*)queries + b * qrow, (int32_t)(e - b), k,
+                                             out_ids + b * k, out_dists + b * k, out_stats ? stats.data() : nullptr);
+            if (rcs[i]) {
+                errors[i] = g_last_error;
+                return;
+            }
+            for (size_t j = 0; j < stats.size(); ++j) out_stats[b * 3 + j] = stats[j];
+        });
+    }
+    for (std::thread& t : threads) t.join();
+    for (size_t i = 0; i < n; ++i)
+        if (rcs[i]) return fail(rcs[i], "member %zu: %s", i, errors[i].c_str());
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_spann_group_cache_warm(sptag_b200_spann_group_handle g, const void* queries, int32_t num_queries,
+                                      int64_t budget_bytes_per_member, int32_t* out_lists, int32_t* out_owners,
+                                      int32_t capacity, int32_t* out_n) {
+    if (!g) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (num_queries < 0 || (num_queries > 0 && !queries) || !out_n || capacity < 0 ||
+        (capacity > 0 && (!out_lists || !out_owners)))
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    if (budget_bytes_per_member < -1)
+        return fail(SPTAG_B200_LACK_OF_INPUTS, "budget %lld below -1", (long long)budget_bytes_per_member);
+    *out_n = 0;
+    sptag_b200_spann* m0 = g->members[0];
+    SpannSnapshot sp;
+    if (int rc = spann_snapshot(m0, sp)) return rc;
+    if (sp.internal > 2048) return fail(SPTAG_B200_LACK_OF_INPUTS, "SearchInternalResultNum %d exceeds 2048", sp.internal);
+    GroupSets all(g);
+    std::vector<int> order;
+    if (int rc = spann_warm_order(m0, sp, queries, num_queries, order)) return rc;
+    const size_t n = g->members.size();
+    std::vector<long long> left(n, 0);
+    for (size_t i = 0; i < n; ++i) {
+        {
+            DeviceGuard guard(g->members[i]->head->device);
+            spann_cache_release(g->members[i]);
+        }
+        if (int rc = spann_warm_budget(g->members[i], budget_bytes_per_member, left[i])) {
+            spann_group_peer_tables(g);
+            return rc;
+        }
+    }
+    // in rank order, each list to the member with the most budget left (the lower index of equals), if it fits there
+    const long long elem_bytes = (long long)m0->head->row_stride + 4;
+    std::vector<std::vector<int>> mine(n);
+    std::vector<int> lists, owners;
+    for (int l : order) {
+        size_t o = 0;
+        for (size_t i = 1; i < n; ++i)
+            if (left[i] > left[o]) o = i;
+        const long long bytes = (long long)m0->cnt[l] * elem_bytes;
+        if (bytes > left[o]) continue;
+        left[o] -= bytes;
+        mine[o].push_back(l);
+        lists.push_back(l);
+        owners.push_back((int)o);
+    }
+    if (int rc = spann_group_install(g, mine)) return rc;
+    *out_n = (int32_t)lists.size();
+    const size_t c = std::min<size_t>(lists.size(), (size_t)capacity);
+    std::copy_n(lists.begin(), c, out_lists);
+    std::copy_n(owners.begin(), c, out_owners);
+    return SPTAG_B200_SUCCESS;
+}
+
+int sptag_b200_spann_group_cache_lists(sptag_b200_spann_group_handle g, const int32_t* lists, const int32_t* owners,
+                                       int32_t n) {
+    if (!g) return fail(SPTAG_B200_EMPTY_INDEX, "null handle");
+    if (n < 0 || (n > 0 && (!lists || !owners))) return fail(SPTAG_B200_LACK_OF_INPUTS, "null buffer");
+    const int nl = g->members[0]->num_lists, members = (int)g->members.size();
+    std::vector<char> seen((size_t)nl, 0);
+    std::vector<std::vector<int>> mine((size_t)members);
+    for (int32_t i = 0; i < n; ++i) {
+        const int l = lists[i], o = owners[i];
+        if (l < 0 || l >= nl) return fail(SPTAG_B200_LACK_OF_INPUTS, "list %d outside [0, %d)", l, nl);
+        if (o < 0 || o >= members) return fail(SPTAG_B200_LACK_OF_INPUTS, "owner %d outside [0, %d)", o, members);
+        if (seen[l]) return fail(SPTAG_B200_LACK_OF_INPUTS, "list %d given twice", l);
+        seen[l] = 1;
+        mine[(size_t)o].push_back(l);
+    }
+    GroupSets all(g);
+    return spann_group_install(g, mine);
 }
 
 }  // extern "C"
@@ -4894,7 +5267,7 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     decltype(s->staging.acquire(slock)) gs = nullptr;
     if (s->host_postings)
         if (int rc = spann_acquire_fitted(s, sp, slock, gs)) return rc;
-    long gather_bytes = 0, gather_rounds_n = 0;
+    long gather_bytes = 0, gather_rounds_n = 0, gather_peer_bytes = 0;
     if (gs) {
         if (int rc = gs->d_chosen.ensure(nq * it->hb * 4)) return rc;
         if (int rc = gs->d_nchosen.ensure(nq * 4)) return rc;
@@ -4917,7 +5290,8 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
             r.lists = view;
             return step(r, e - b);
         };
-        return gather_rounds(s, *gs, sp, (int)n, it->hb, stream, choose, run, gather_bytes, gather_rounds_n);
+        return gather_rounds(s, *gs, sp, (int)n, it->hb, stream, choose, run, gather_bytes, gather_rounds_n,
+                             gather_peer_bytes);
     };
     // Rounds: the posting step over the queries of the round; queries whose tables must grow run again (same round);
     // then the head's FromNeareast(false) for the queries whose postings ran out, and the posting step over those.
@@ -4958,6 +5332,7 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     if (gs) {
         s->last_gather_bytes = gather_bytes;
         s->last_gather_rounds = gather_rounds_n;
+        s->last_peer_gather_bytes = gather_peer_bytes;
     }
     return SPTAG_B200_SUCCESS;
 }
