@@ -409,11 +409,29 @@ void sptag_b200_spann_destroy(sptag_b200_spann_handle s);
  *           case, SearchInternalResultNum x the longest searched list x (row stride + 4) bytes.  MemoryOverFlow when the
  *           pinned allocation fails.  sptag_b200_spann_cache_warm / sptag_b200_spann_cache_lists keep some lists, whole,
  *           in HBM as well: those are read in place and never copied, and a batch's union and its rounds count the
- *           other lists only. */
+ *           other lists only.
+ *   FILE:   the lists stay in their posting files, as the reference keeps them on SSD (ExtraFullGraphSearcher::
+ *           SearchIndex reads each chosen list's pages at search time).  The load reads the ini, the head, the translate
+ *           map and each posting file's header, and none of the lists' bodies; it keeps one descriptor per posting file
+ *           open for the handle's life, and each list's offset, count and page count in HBM.  It returns Fail when a
+ *           list's full extent runs past the end of its file.  Searches, iterator steps and cache installs run as on a
+ *           HOST handle, with the same stages, rounds and results, but read each round's union from the files: a pool
+ *           of min(16, hardware threads) threads preads it, a piece of at most 64 MB (or the largest list) at a time,
+ *           into one of two pinned, mapped windows per staging set, and a kernel cuts each piece's records into the
+ *           stage while the next piece is read.  A round reads each list's searched prefix (plain layout) or the whole
+ *           list (rearranged layout): element count x (dim x sizeof(T) + 4) bytes; lists cached in HBM are never read.
+ *           Each call first checks that every posting file is still the file loaded at its path (same device and
+ *           inode).  A posting file moved away or replaced, or a read that fails or ends early (a file truncated after
+ *           the load), fails the call with Fail, whose message names the file (and the list and offset of a read); the
+ *           handle keeps working, and the next call reads again.  Pinned host memory: 2 x 2 x (64 MB, or the largest
+ *           list's bytes, + 64 KB) windows, allocated on a staging set's first read; HBM: the lists' offsets, counts and
+ *           pages, the stages and the cache.  Compressed and delta-encoded lists are refused as on every placement, and
+ *           SPANN groups (sptag_b200_spann_group_load) keep the HOST layout. */
 enum {
     SPTAG_B200_POSTINGS_AUTO = 0,
     SPTAG_B200_POSTINGS_DEVICE = 1,
-    SPTAG_B200_POSTINGS_HOST = 2
+    SPTAG_B200_POSTINGS_HOST = 2,
+    SPTAG_B200_POSTINGS_FILE = 3
 };
 typedef struct {
     int32_t struct_size;        /* sizeof(sptag_b200_spann_load_options) */
@@ -422,7 +440,7 @@ typedef struct {
 
 /* sptag_b200_spann_load with a choice of where the posting lists live (options NULL: AUTO).  LackOfInputs for an unknown
  * placement, Fail for a struct_size other than sizeof(sptag_b200_spann_load_options).  The handle's B200.PostingPlacement
- * reads "device" or "host". */
+ * reads "device", "host" or "file". */
 int sptag_b200_spann_load_ex(const char* folder, int32_t device, const sptag_b200_spann_load_options* options,
                              sptag_b200_spann_handle* out);
 
@@ -523,13 +541,16 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
  * are the head handle's (sptag_b200_set_param): they choose the visited sets of the head iterators SPANN iterators open.
  * B200.SpannDedupEntries: the first dedup table size of an iterator's queries, 0 (default: room for one head batch of
  * the longest list, at most 2^14) or a power of two >= 64; tables double as they fill.  B200.PostingStageBytes (host
- * placement, sptag_b200_spann_load_ex): the HBM stage of each of the two staging sets, default 268435456 (256 MB), in
+ * or file placement, sptag_b200_spann_load_ex): the HBM stage of each of the two staging sets, default 268435456 (256 MB), in
  * [0, 2^31 - 1]; 0 leaves one query's worst case.  The stage grows when a call needs more and never shrinks.
- * Read-only: PostingBytes (device bytes of the posting lists and the translate map; with host placement the lists'
- * offsets, counts and page counts only), B200.PostingPlacement ("device" or "host"), B200.PostingHostBytes (pinned
- * host bytes of the lists' rows and ids, 0 with device placement), B200.LastGatherBytes and B200.LastGatherRounds (host
- * placement: the bytes copied from host memory and the gather rounds of the last search or iterator step on this
- * handle), B200.LastIteratorRounds (head refill rounds of the last sptag_b200_spann_iterator_next on this handle) and
+ * Read-only: PostingBytes (device bytes of the posting lists and the translate map; with host or file placement the
+ * lists' offsets, counts and page counts only), B200.PostingPlacement ("device", "host" or "file"),
+ * B200.PostingHostBytes (pinned host bytes of the lists' rows and ids, 0 with device or file placement),
+ * B200.LastGatherBytes and B200.LastGatherRounds (host or file placement: the staged elements x (row stride + 4) bytes
+ * and the rounds of the last search or iterator step on this handle; a FILE handle's equal a HOST handle's for the same
+ * calls), B200.LastReadBytes (file placement: the posting-file bytes the last search, iterator step or cache install on
+ * this handle read, the sum of element count x (dim x sizeof(T) + 4) over the lists read; 0 otherwise),
+ * B200.LastIteratorRounds (head refill rounds of the last sptag_b200_spann_iterator_next on this handle) and
  * B200.LastIteratorDedupBytes (that iterator's dedup table bytes), and B200.LastPostingKernel (the demangled name of the
  * last posting-scan or posting-step kernel instantiation a search or iterator step on this handle launched, e.g.
  * "sptag_b200::(anonymous namespace)::spann_scan_kernel<true, 2>"; empty before the first).
@@ -537,7 +558,8 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
 int sptag_b200_spann_set_param(sptag_b200_spann_handle s, const char* name, const char* value);
 int sptag_b200_spann_get_param(sptag_b200_spann_handle s, const char* name, char* value_out, int32_t capacity);
 
-/* An HBM cache of posting lists on a handle loaded with the HOST placement.  Ranks the posting lists by how many of
+/* An HBM cache of posting lists on a handle loaded with the HOST or FILE placement (on FILE, the cached lists are read
+ * from their files once, by the install, and never again).  Ranks the posting lists by how many of
  * num_queries sample queries choose them, and caches the top of that order in HBM.  Each query runs the head search and
  * the posting choice of a search with K <= SearchInternalResultNum (W = SearchInternalResultNum), with the search
  * parameters in force; the lists are counted on the device, ranked by count, descending, then list id, ascending, and
@@ -553,7 +575,8 @@ int sptag_b200_spann_cache_warm(sptag_b200_spann_handle s, const void* queries, 
 /* Caches exactly the given lists in HBM (num_lists = 0 releases the cache), e.g. a set an earlier
  * sptag_b200_spann_cache_warm returned.  lists: HOST, distinct ids in [0, number of lists).  The call waits until no
  * search or iterator step runs on the handle (it takes both staging sets), releases the old cache and copies every
- * element of each list, whatever SearchPostingPageLimit is, from the pinned host allocation into one HBM allocation that
+ * element of each list, whatever SearchPostingPageLimit is, from the pinned host allocation (FILE: from the posting
+ * files, through staging set 0's windows) into one HBM allocation that
  * also holds the stage of each staging set.  Searches and iterator steps that start after it returns read the cached
  * lists in place; iterators opened earlier keep working, with unchanged results.  Results equal the device placement's
  * bit for bit with any cache.  B200.LastGatherBytes and B200.LastGatherRounds count only what is still copied from host
@@ -561,7 +584,8 @@ int sptag_b200_spann_cache_warm(sptag_b200_spann_handle s, const void* queries, 
  * raised) re-installs the same lists.  Read-only parameters: B200.PostingCacheLists (lists cached) and
  * B200.PostingCacheBytes (the HBM their rows and ids take).  Device memory: those bytes plus both stages.
  * Codes: LackOfInputs for a DEVICE-placed handle, an id outside the range, an id given twice and a null buffer;
- * MemoryOverFlow when the allocation fails, after which the handle works uncached. */
+ * MemoryOverFlow when the allocation fails, and on a FILE handle Fail when a read fails, after either of which the
+ * handle works uncached. */
 int sptag_b200_spann_cache_lists(sptag_b200_spann_handle s, const int32_t* lists, int32_t num_lists);
 
 /* ---- SPANN on several GPUs of one host ----

@@ -66,7 +66,7 @@ class SpannBuildOptions(C.Structure):
 
 
 # sptag_b200_spann_load_ex's posting_placement (SPTAG_B200_POSTINGS_*)
-POSTING_PLACEMENTS = {"auto": 0, "device": 1, "host": 2}
+POSTING_PLACEMENTS = {"auto": 0, "device": 1, "host": 2, "file": 3}
 
 
 class SptagB200Error(RuntimeError):
@@ -505,8 +505,9 @@ def debug_kernel_for(*, value_type, metric, algo, dim, simd_width=16, enable_bfs
 
 
 class B200SpannIndex:
-    """Handle to a SPANN index whose head lives in HBM and whose posting lists live in HBM or, loaded with
-    posting_placement="host", in pinned host memory (SPANN::Index<T>: LoadIndex, SearchIndex)."""
+    """Handle to a SPANN index whose head lives in HBM and whose posting lists live in HBM, in pinned host memory
+    (posting_placement="host") or in their posting files (posting_placement="file") (SPANN::Index<T>: LoadIndex,
+    SearchIndex)."""
 
     STATS_PER_QUERY = 3  # postings scanned, list elements read, distances computed
 
@@ -517,8 +518,10 @@ class B200SpannIndex:
     @classmethod
     def load(cls, folder, device=-1, posting_placement=None):
         """VectorIndex::LoadIndex(folder) for a SPANN folder.  posting_placement: None (the posting lists in HBM, as
-        sptag_b200_spann_load), or "auto", "device" or "host" (sptag_b200_spann_load_ex: "host" keeps them in pinned host
-        memory and gathers each batch's lists into HBM; "auto" picks HBM when they fit)."""
+        sptag_b200_spann_load), or "auto", "device", "host" or "file" (sptag_b200_spann_load_ex: "host" keeps them in
+        pinned host memory and gathers each batch's lists into HBM; "file" leaves them in the posting files and reads
+        each batch's lists from there into HBM, with the same stages, rounds and results as "host" (B200.LastReadBytes:
+        the file bytes the last call read); "auto" picks HBM when they fit)."""
         h = C.c_void_p()
         if posting_placement is None:
             _check(lib().sptag_b200_spann_load(os.fsencode(folder), device, C.byref(h)))
@@ -596,9 +599,10 @@ class B200SpannIndex:
         return B200SpannIterators(self, queries)
 
     def cache_warm(self, queries, budget_bytes=-1):
-        """On a posting_placement="host" handle: caches in HBM the lists the sample HOST queries choose most often, as
-        many as fit budget_bytes (-1: free HBM less 1 GB), and returns them as int32 list ids in rank order
-        (sptag_b200_spann_cache_warm).  cache_lists(ids) installs the same set again later."""
+        """On a posting_placement="host" or "file" handle: caches in HBM the lists the sample HOST queries choose most
+        often, as many as fit budget_bytes (-1: free HBM less 1 GB), and returns them as int32 list ids in rank order
+        (sptag_b200_spann_cache_warm; a "file" handle reads the taken lists from the posting files here, once).
+        cache_lists(ids) installs the same set again later."""
         queries = np.ascontiguousarray(queries)
         nq = queries.shape[0]
         # a query chooses at most SearchInternalResultNum lists, so that many per query bound the taken set
@@ -613,7 +617,7 @@ class B200SpannIndex:
         return out[:n.value].copy()
 
     def cache_lists(self, lists):
-        """On a posting_placement="host" handle: caches exactly these list ids in HBM (empty: releases the cache;
+        """On a posting_placement="host" or "file" handle: caches exactly these list ids in HBM (empty: releases the cache;
         sptag_b200_spann_cache_lists)."""
         lists = np.ascontiguousarray(lists, np.int32)
         _check(lib().sptag_b200_spann_cache_lists(self._h, lists.ctypes.data, len(lists)))

@@ -135,6 +135,92 @@ __global__ void __launch_bounds__(kGatherThreads) spann_gather_kernel(const Post
     }
 }
 
+// The file placement's unpack: one CTA per list of a piece.  The list's raw bytes (16-byte aligned in the window) come
+// into shared memory as aligned 16-byte words, a chunk of whole records at a time; each record is then cut out at its
+// byte offset, which need not be a multiple of 4 (vis 21, 37, ...).
+constexpr int kUnpackThreads = 256;
+constexpr int kUnpackChunk = 32 << 10;  // shared bytes of one chunk, unless one record needs more
+constexpr int kUnpackSlack = 32;        // readable bytes past a chunk: unpack_word reads up to 20 bytes past its offset
+
+// Loads bytes [a, b) of the list at src into sm as the aligned 16-byte words that cover them; returns where byte a is
+__device__ __forceinline__ int unpack_load(const uint4* src, long long a, long long b, uint4* sm) {
+    const long long w0 = a >> 4;
+    const int words = (int)(((b + 15) >> 4) - w0);  // at most a chunk's
+    src += w0;
+    for (int i = threadIdx.x; i < words; i += kUnpackThreads) sm[i] = src[i];
+    return (int)(a & 15);
+}
+
+__device__ __forceinline__ unsigned unpack_u32(const unsigned char* sm, int o) {
+    const unsigned* w = reinterpret_cast<const unsigned*>(sm + (o & ~3));
+    return __funnelshift_r(w[0], w[1], (o & 3) * 8);
+}
+
+// The 16 bytes at offset o of sm, the bytes from `valid` on zeroed (a row's padding)
+__device__ __forceinline__ uint4 unpack_word(const unsigned char* sm, int o, int valid) {
+    const unsigned* w = reinterpret_cast<const unsigned*>(sm + (o & ~3));
+    const int sh = (o & 3) * 8;
+    unsigned v[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const unsigned x = __funnelshift_r(w[k], w[k + 1], sh);
+        const int keep = valid - 4 * k;
+        v[k] = keep >= 4 ? x : keep <= 0 ? 0u : x & ((1u << (8 * keep)) - 1u);
+    }
+    return make_uint4(v[0], v[1], v[2], v[3]);
+}
+
+// n rows of row_bytes, row i at offset base + i * step of sm, to dst at wpr 16-byte words per row
+__device__ __forceinline__ void unpack_rows(const unsigned char* sm, int base, int step, int n, int row_bytes, int wpr,
+                                            uint4* dst) {
+    for (int t = threadIdx.x; t < n * wpr; t += kUnpackThreads) {
+        const int i = t / wpr, j = t - i * wpr, valid = row_bytes - 16 * j;
+        dst[(long long)i * wpr + j] = valid > 0 ? unpack_word(sm, base + i * step + 16 * j, valid) : make_uint4(0, 0, 0, 0);
+    }
+}
+
+template <bool REARRANGED>
+__global__ void __launch_bounds__(kUnpackThreads) spann_file_unpack_kernel(const PostingGather g,
+                                                                          const FilePieceList* table,
+                                                                          const unsigned char* window, int chunk) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    uint4* sm = reinterpret_cast<uint4*>(smem);
+    const FilePieceList pl = table[blockIdx.x];
+    const int l = pl.list;
+    const long long len = g.len[l], to = g.stage_off[l];
+    const int vis = g.host.vector_info_size, rb = vis - 4, wpr = (int)(g.host.row_stride / 16);
+    const uint4* src = reinterpret_cast<const uint4*>(window + pl.window_off);
+    uint4* rows = reinterpret_cast<uint4*>(g.stage_rows) + to * wpr;
+    int* ids = g.stage_ids + to;
+    if (!REARRANGED) {  // element i: [id | row] at i * vis
+        const int per = (chunk - 16) / vis;
+        for (long long e0 = 0; e0 < len; e0 += per) {
+            const int n = (int)min((long long)per, len - e0);
+            __syncthreads();  // the last chunk is consumed
+            const int base = unpack_load(src, e0 * vis, (e0 + n) * vis, sm);
+            __syncthreads();
+            unpack_rows(smem, base + 4, vis, n, rb, wpr, rows + e0 * wpr);
+            for (int i = threadIdx.x; i < n; i += kUnpackThreads) ids[e0 + i] = (int)unpack_u32(smem, base + i * vis);
+        }
+    } else {  // every row (rb bytes each), then every id, of the whole list (ExtraFullGraphSearcher.h:1186-1195)
+        const long long cnt = g.host.cnt[l], per = (chunk - 16) / rb, per_id = (chunk - 16) / 4;
+        for (long long e0 = 0; e0 < len; e0 += per) {
+            const int n = (int)min(per, len - e0);
+            __syncthreads();
+            const int base = unpack_load(src, e0 * rb, (e0 + n) * rb, sm);
+            __syncthreads();
+            unpack_rows(smem, base, rb, n, rb, wpr, rows + e0 * wpr);
+        }
+        for (long long e0 = 0; e0 < len; e0 += per_id) {
+            const int n = (int)min(per_id, len - e0);
+            __syncthreads();
+            const int base = unpack_load(src, rb * cnt + 4 * e0, rb * cnt + 4 * (e0 + n), sm);
+            __syncthreads();
+            for (int i = threadIdx.x; i < n; i += kUnpackThreads) ids[e0 + i] = (int)unpack_u32(smem, base + 4 * i);
+        }
+    }
+}
+
 // The stage offsets (exclusive sum of g.len) and the compacted union (the flagged list numbers); with temp null, the
 // scratch bytes the two need
 cudaError_t union_cub(const PostingGather& g, void* temp, size_t& bytes, cudaStream_t stream) {
@@ -209,6 +295,25 @@ cudaError_t launch_spann_gather(const PostingGather& g, int grid, cudaStream_t s
         spann_gather_kernel<true><<<grid, kGatherThreads, 0, stream>>>(g);
     else
         spann_gather_kernel<false><<<grid, kGatherThreads, 0, stream>>>(g);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_spann_file_unpack(const PostingGather& g, const FilePieceList* table, int n, const unsigned char* window,
+                                     bool rearranged, cudaStream_t stream) {
+    if (n <= 0) return cudaSuccess;
+    const int record = rearranged ? g.host.vector_info_size - 4 : g.host.vector_info_size;
+    const int chunk = std::max(kUnpackChunk, (record + 15) / 16 * 16 + 16);  // at least one record per chunk
+    const size_t smem = (size_t)chunk + kUnpackSlack;
+    auto kernel = rearranged ? spann_file_unpack_kernel<true> : spann_file_unpack_kernel<false>;
+    if (smem > (48u << 10)) {  // records over 32 KB: the opt-in maximum, one value for every caller
+        int dev = 0, optin = 0;
+        cudaError_t e = cudaGetDevice(&dev);
+        if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+        if (e == cudaSuccess && smem > (size_t)optin) e = cudaErrorInvalidValue;
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+        if (e != cudaSuccess) return e;
+    }
+    kernel<<<n, kUnpackThreads, smem, stream>>>(g, table, window, chunk);
     return cudaGetLastError();
 }
 

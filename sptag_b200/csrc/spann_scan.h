@@ -179,6 +179,18 @@ cudaError_t launch_spann_union(const PostingGather& g, const int* chosen, const 
 // Copies g.len[l] elements of every list l of g.lists (the union: its searched prefix) from host memory, or with
 // g.peers.first from the peer that caches it, to element g.stage_off[l] of the stage
 cudaError_t launch_spann_gather(const PostingGather& g, int grid, cudaStream_t stream);
+// Posting lists left in their files (the FILE placement): a union's raw records are read from the posting files into a
+// mapped host window, a piece of lists at a time, each list at a 16-byte-aligned window_off.  The unpack cuts each
+// list's records into the stage as the gather does: g.len[l] rows at g.host.row_stride, padding bytes zero, and ids,
+// from element g.stage_off[l].  Plain layout: element i is [int32 id | row] at i * vis; rearranged: row i at i * (vis -
+// 4), id i at (vis - 4) * cnt + 4 * i (the whole list is in the window).  table: [n] in device memory.
+struct FilePieceList {
+    long long window_off;
+    int list;
+    int pad;
+};
+cudaError_t launch_spann_file_unpack(const PostingGather& g, const FilePieceList* table, int n, const unsigned char* window,
+                                     bool rearranged, cudaStream_t stream);
 // counts[l] += the items (chosen / nchosen as above) that read list l
 cudaError_t launch_spann_count(const int* chosen, const int* nchosen, int stride, int n, int* counts, cudaStream_t stream);
 

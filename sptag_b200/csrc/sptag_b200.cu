@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cctype>
+#include <cerrno>
 #include <cfloat>
 #include <chrono>
 #include <climits>
@@ -24,9 +25,13 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <condition_variable>
 #include <cxxabi.h>
+#include <deque>
 #include <dlfcn.h>
+#include <fcntl.h>
 #include <fstream>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -37,6 +42,7 @@
 #include <string>
 #include <thread>
 #include <type_traits>
+#include <unistd.h>
 #include <utility>
 #include <vector>
 
@@ -2858,6 +2864,92 @@ int32_t sptag_b200_num_deleted(sptag_b200_handle h) {
 // posting scan kernel (kern_spann.cu; kern_spann_pq.cu on a quantized index, whose head and lists hold M-byte code
 // rows: ExtraFullGraphSearcher<std::uint8_t>, SPANNIndex.cpp:93-99).
 // ---------------------------------------------------------------------------------------------------------------
+namespace {
+
+// The threads a FILE-placed handle reads its posting files on.  run(n, fn) calls fn(0) .. fn(n - 1) on them and returns
+// when every call has returned; two callers' batches share the threads, in turn.  The destructor joins them.
+class ReadPool {
+  public:
+    explicit ReadPool(unsigned threads) {
+        for (unsigned i = 0; i < threads; ++i) workers_.emplace_back([this] { work(); });
+    }
+    ~ReadPool() {
+        {
+            std::lock_guard<std::mutex> lock(mu_);
+            stop_ = true;
+        }
+        more_.notify_all();
+        for (std::thread& t : workers_) t.join();
+    }
+    void run(size_t n, const std::function<void(size_t)>& fn) {
+        if (n == 0) return;
+        Batch b{&fn, n};
+        std::unique_lock<std::mutex> lock(mu_);
+        queue_.push_back(&b);
+        more_.notify_all();
+        done_.wait(lock, [&] { return b.done == n; });
+    }
+
+  private:
+    struct Batch {
+        const std::function<void(size_t)>* fn;
+        size_t n, next = 0, done = 0;
+    };
+    void work() {
+        std::unique_lock<std::mutex> lock(mu_);
+        for (;;) {
+            more_.wait(lock, [&] { return stop_ || !queue_.empty(); });
+            if (queue_.empty()) return;  // stop_: no caller is waiting (the handle is being destroyed)
+            Batch* b = queue_.front();
+            const size_t i = b->next++;
+            if (b->next == b->n) queue_.pop_front();
+            lock.unlock();
+            (*b->fn)(i);
+            lock.lock();
+            if (++b->done == b->n) done_.notify_all();
+        }
+    }
+    std::mutex mu_;
+    std::condition_variable more_, done_;
+    std::deque<Batch*> queue_;
+    bool stop_ = false;
+    std::vector<std::thread> workers_;
+};
+
+// A FILE-placed handle's posting files: each one's path and descriptor (O_RDONLY, open for the handle's life)
+struct PostingFileSet {
+    std::vector<std::string> paths;
+    std::vector<int> fds;
+    ~PostingFileSet() {
+        for (int fd : fds) close(fd);
+    }
+};
+
+// A staging set's windows for the FILE placement: two pinned, mapped windows of `bytes` the posting files are read into,
+// each followed by its piece table, and per window the event recorded behind the last unpack kernel that read it
+constexpr size_t kFileWindow = 64ull << 20;
+constexpr int kPieceLists = 4096;
+struct FileWindows {
+    unsigned char* host = nullptr;  // 2 x (bytes + kPieceLists FilePieceLists)
+    unsigned char* dev = nullptr;   // its device (mapped) address
+    size_t bytes = 0;
+    cudaEvent_t read[2] = {nullptr, nullptr};
+    DeviceBuffer d_tables;  // 2 x kPieceLists FilePieceLists
+    FileWindows() = default;
+    FileWindows(const FileWindows&) = delete;
+    FileWindows& operator=(const FileWindows&) = delete;
+    ~FileWindows() {
+        if (host) cudaFreeHost(host);
+        for (cudaEvent_t e : read)
+            if (e) cudaEventDestroy(e);
+    }
+    size_t span() const { return bytes + kPieceLists * sizeof(FilePieceList); }
+    unsigned char* window(int w) const { return host + w * span(); }
+    FilePieceList* table(int w) const { return reinterpret_cast<FilePieceList*>(window(w) + bytes); }
+};
+
+}  // namespace
+
 struct sptag_b200_spann {
     sptag_b200_index* head = nullptr;
     bool quantized = false;  // [Base] QuantizerFilePath: the head's quantizer scores the postings too
@@ -2897,6 +2989,15 @@ struct sptag_b200_spann {
     DeviceBuffer d_cache, d_resident;
     std::vector<int> cache_lists;
     long long cache_pool = 0, cache_stage = 0, cache_bytes = 0;
+    // File placement (host_postings is set too: the lists are staged as the host placement's are): the lists stay in
+    // their posting files and each call reads its union from there (spann_stage); per list its file and first byte.
+    // last_read_bytes: the file bytes the last search, iterator step or cache install on this handle read.
+    bool file_postings = false;
+    PostingFileSet post_files;
+    std::vector<int> list_file;
+    std::vector<long long> list_start;
+    std::unique_ptr<ReadPool> readers;
+    long last_read_bytes = 0;
     // Host-buffer calls run on one of two staging sets, each with its own stream, head results, dedup tables and outputs,
     // so that two callers overlap; the head search kernels are ordered by the head handle (search_device_impl)
     struct StagingBuffers {
@@ -2906,6 +3007,7 @@ struct sptag_b200_spann {
         DeviceBuffer d_chosen, d_nchosen, d_flags, d_len, d_stage_off, d_union, d_nunion, d_cub, d_sub, d_stage;
         DeviceBuffer d_view_off;  // with a cache: the view's list offsets
         DeviceBuffer d_peer_elems;  // a group member's: the elements a call copied from peers
+        FileWindows windows;        // file placement
     };
     StagingPool<StagingBuffers> staging;
     std::mutex mu;  // the search parameters
@@ -2981,16 +3083,165 @@ long long stage_elems(const sptag_b200_spann* s, const SpannSnapshot& sp) {
     return cap / elem_bytes;
 }
 
+// File placement: the window of a staging set, grown to `bytes` (its events and tables made on first use).  Caller holds
+// the set; the set's earlier unpack kernels have completed or are waited for here.
+int spann_file_windows(FileWindows& fw, size_t bytes) {
+    for (cudaEvent_t& e : fw.read)
+        if (!e) CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    if (int rc = fw.d_tables.ensure(2 * kPieceLists * sizeof(FilePieceList))) return rc;
+    if (fw.bytes >= bytes) return 0;
+    for (cudaEvent_t e : fw.read) CUDA_OK(cudaEventSynchronize(e));
+    if (fw.host) cudaFreeHost(fw.host);
+    fw.host = fw.dev = nullptr;
+    fw.bytes = bytes;
+    if (cudaHostAlloc((void**)&fw.host, 2 * fw.span(), cudaHostAllocMapped) != cudaSuccess) {
+        fw.host = nullptr;
+        fw.bytes = 0;
+        cudaGetLastError();
+        return fail(SPTAG_B200_MEMORY_OVERFLOW, "cudaHostAlloc(%zu) of the posting-file windows failed",
+                    2 * (bytes + kPieceLists * sizeof(FilePieceList)));
+    }
+    CUDA_OK(cudaHostGetDevicePointer((void**)&fw.dev, fw.host, 0));
+    return 0;
+}
+
+// File placement: every posting file is still the one the handle opened at its path (a file moved away or replaced
+// since the load fails the call, which would otherwise read the old file's bytes)
+int spann_files_in_place(const sptag_b200_spann* s) {
+    const PostingFileSet& pf = s->post_files;
+    for (size_t i = 0; i < pf.fds.size(); ++i) {
+        struct stat at, open_st;
+        if (stat(pf.paths[i].c_str(), &at) != 0 || fstat(pf.fds[i], &open_st) != 0 || at.st_dev != open_st.st_dev ||
+            at.st_ino != open_st.st_ino)
+            return fail(SPTAG_B200_FAIL, "posting file %s is no longer the file the index loaded (moved or replaced)",
+                        pf.paths[i].c_str());
+    }
+    return 0;
+}
+
+// Where a union's lists come from, for the gather rounds and the cache installs: copies g.len[l] elements of every list
+// l of g.lists (*g.nlists of them) to element g.stage_off[l] of g's stage.  whole: g.len holds every element of each
+// list (a cache install), else the searched prefix at g.host.page_limit.
+//   HOST (and a group member): from mapped host memory or a peer's pool, with the gather kernel.
+//   FILE: the union, in order, is cut into pieces that fit a window of kFileWindow bytes (or of the largest list's raw
+//   bytes), each list's raw bytes at a 16-byte-aligned offset: plain, its len x vis searched bytes; rearranged, the
+//   whole list.  The read pool preads piece p into one of the set's two windows while the unpack kernel of piece p - 1
+//   cuts the other into the stage; a window is refilled once the event behind its last kernel has completed.
+//   read_bytes += the file bytes read.  A failed or short read fails the call, naming the file, the list and the
+//   offset, with the stream synchronised.
+int spann_stage(sptag_b200_spann* s, sptag_b200_spann::StagingBuffers& set, const PostingGather& g, bool whole,
+                cudaStream_t stream, long& read_bytes) {
+    if (!s->file_postings) {
+        CUDA_OK(launch_spann_gather(g, s->head->num_sms * 4, stream));
+        g_launches++;
+        return 0;
+    }
+    if (int rc = spann_files_in_place(s)) return rc;
+    int n = 0;
+    CUDA_OK(cudaMemcpyAsync(&n, g.nlists, 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    std::vector<int> lists((size_t)n);
+    if (n > 0) {
+        CUDA_OK(cudaMemcpyAsync(lists.data(), g.lists, (size_t)n * 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+    }
+    // each list's raw bytes: the host's own count of what g.len holds
+    std::vector<long long> raw((size_t)n);
+    long long largest = 0, total = 0;
+    for (int u = 0; u < n; ++u) {
+        const int l = lists[u];
+        const long long len = whole ? s->cnt[l] : posting_searched(s->cnt[l], s->pages[l], g.host.page_limit, s->vis);
+        raw[u] = len == 0 ? 0 : (s->rearranged ? (long long)s->cnt[l] : len) * s->vis;
+        largest = std::max(largest, raw[u]);
+        total += raw[u];
+    }
+    FileWindows& fw = set.windows;
+    if (int rc = spann_file_windows(fw, std::max<size_t>(kFileWindow, round_up((size_t)largest, 16)))) return rc;
+    // a piece's reads, split into jobs of about kReadJob bytes so that a large list keeps several threads busy
+    constexpr long long kReadJob = 1ll << 20;
+    struct Read {
+        int file, list;
+        long long offset, bytes;
+        unsigned char* dst;
+    };
+    std::vector<Read> reads;
+    std::vector<size_t> jobs;  // the first read of each job, then reads.size()
+    std::mutex err_mu;
+    std::string err;
+    auto do_job = [&](size_t j) {
+        for (size_t r = jobs[j]; r < jobs[j + 1]; ++r) {
+            const Read& rd = reads[r];
+            long long got = 0;
+            while (got < rd.bytes) {
+                const ssize_t k = pread(s->post_files.fds[rd.file], rd.dst + got, (size_t)(rd.bytes - got), rd.offset + got);
+                if (k < 0 && errno == EINTR) continue;
+                if (k <= 0) {
+                    char msg[512];
+                    snprintf(msg, sizeof(msg), "posting file %s: list %d: read at offset %lld %s",
+                             s->post_files.paths[rd.file].c_str(), rd.list, rd.offset + got,
+                             k < 0 ? strerror(errno) : "ends before the list does");
+                    std::lock_guard<std::mutex> lock(err_mu);
+                    if (err.empty()) err = msg;
+                    return;
+                }
+                got += k;
+            }
+        }
+    };
+    const std::function<void(size_t)> job_fn = do_job;
+    int piece = 0;
+    for (int u0 = 0; u0 < n; ++piece) {
+        const int w = piece & 1;
+        CUDA_OK(cudaEventSynchronize(fw.read[w]));  // the kernel that last read this window
+        unsigned char* win = fw.window(w);
+        FilePieceList* table = fw.table(w);
+        reads.clear();
+        jobs.assign(1, 0);
+        long long at = 0, job_bytes = 0;
+        int u = u0;
+        for (; u < n && u - u0 < kPieceLists; ++u) {
+            const long long off = (long long)round_up((size_t)at, 16);
+            if (u > u0 && off + raw[u] > (long long)fw.bytes) break;
+            const int l = lists[u];
+            table[u - u0] = {off, l, 0};
+            for (long long b = 0; b < raw[u]; b += kReadJob) {
+                reads.push_back({s->list_file[l], l, s->list_start[l] + b, std::min(kReadJob, raw[u] - b), win + off + b});
+                job_bytes += reads.back().bytes;
+                if (job_bytes >= kReadJob) {
+                    jobs.push_back(reads.size());
+                    job_bytes = 0;
+                }
+            }
+            at = off + raw[u];
+        }
+        if (jobs.back() != reads.size()) jobs.push_back(reads.size());
+        s->readers->run(jobs.size() - 1, job_fn);
+        if (!err.empty()) {
+            cudaStreamSynchronize(stream);
+            return fail(SPTAG_B200_FAIL, "%s", err.c_str());
+        }
+        FilePieceList* d_table = (FilePieceList*)fw.d_tables.ptr + w * kPieceLists;
+        CUDA_OK(cudaMemcpyAsync(d_table, table, (size_t)(u - u0) * sizeof(FilePieceList), cudaMemcpyHostToDevice, stream));
+        CUDA_OK(launch_spann_file_unpack(g, d_table, u - u0, fw.dev + (win - fw.host), s->rearranged != 0, stream));
+        g_launches++;
+        CUDA_OK(cudaEventRecord(fw.read[w], stream));
+        u0 = u;
+    }
+    read_bytes += (long)total;
+    return 0;
+}
+
 // Host placement: runs the n items of a call (the queries of a search, or of an iterator's posting-step launch) in
 // gather rounds on staging set sb.  A round takes the next m items, m starting at n and halved (rounded up) until the
 // union of their lists fits the stage (never below one item), gathers that union into the stage and runs them on it;
 // the next round starts from the same m.  choose(b, e, chosen, nchosen) points chosen / nchosen at the lists items
 // [b, e) read (stride apart), enqueued on stream; run(b, e, view) runs items [b, e) on the staged view.  The stage holds
 // the larger of B200.PostingStageBytes and one query's worst case.  Adds the bytes gathered and the rounds to bytes and
-// rounds, and the part of those bytes a group member copied from peers' pools to peer_bytes.
+// rounds, the part of those bytes a group member copied from peers' pools to peer_bytes, and the file bytes a
+// FILE-placed handle read to read_bytes.
 template <typename Buffers, typename Choose, typename Run>
 int gather_rounds(sptag_b200_spann* s, Buffers& sb, const SpannSnapshot& sp, int n, int stride, cudaStream_t stream,
-                  Choose&& choose, Run&& run, long& bytes, long& rounds, long& peer_bytes) {
+                  Choose&& choose, Run&& run, long& bytes, long& rounds, long& peer_bytes, long& read_bytes) {
     const PostingLists host = posting_lists(s, sp.page_limit);
     const long long elem_bytes = (long long)host.row_stride + 4;
     const long long cap_elems = stage_elems(s, sp);
@@ -3051,7 +3302,6 @@ int gather_rounds(sptag_b200_spann* s, Buffers& sb, const SpannSnapshot& sp, int
         g.peers.elems = (unsigned long long*)sb.d_peer_elems.ptr;
         CUDA_OK(cudaMemsetAsync(g.peers.elems, 0, 8, stream));
     }
-    const int grid = s->head->num_sms * 4;
     for (int b = 0, m = n; b < n; b += m) {
         m = std::min(m, n - b);
         long long elems = 0;
@@ -3067,8 +3317,7 @@ int gather_rounds(sptag_b200_spann* s, Buffers& sb, const SpannSnapshot& sp, int
         }
         if (elems > cap_elems)  // one query reads at most SearchInternalResultNum lists of at most `longest` elements
             return fail(SPTAG_B200_FAIL, "one query's %lld posting elements exceed the stage's %lld", elems, cap_elems);
-        CUDA_OK(launch_spann_gather(g, grid, stream));
-        g_launches++;
+        if (int rc = spann_stage(s, sb, g, false, stream, read_bytes)) return rc;
         if (int rc = run(b, b + m, view)) return rc;
         bytes += (long)(elems * elem_bytes);
         ++rounds;
@@ -3111,7 +3360,7 @@ void spann_cache_release(sptag_b200_spann* s) {
     s->cache_pool = s->cache_bytes = 0;
 }
 
-// The copy of spann_cache_install, on the handle's device
+// The copy of spann_cache_install, on the handle's device (the lists' source: spann_stage, on staging set 0)
 int spann_cache_copy(sptag_b200_spann* s, const std::vector<int>& lists, long long stage) {
     const size_t nl = (size_t)s->num_lists, rs = s->head->row_stride;
     stage = std::max({stage, s->cache_stage, 1ll});
@@ -3147,10 +3396,11 @@ int spann_cache_copy(sptag_b200_spann* s, const std::vector<int>& lists, long lo
     g.stage_rows = (unsigned char*)s->d_cache.ptr;
     g.stage_ids = (int*)(g.stage_rows + (size_t)all * rs);
     cudaStream_t stream = s->staging.sets[0].stream;
-    CUDA_OK(launch_spann_gather(g, s->head->num_sms * 4, stream));
-    g_launches++;
+    long read_bytes = 0;
+    if (int rc = spann_stage(s, s->staging.sets[0], g, true, stream, read_bytes)) return rc;
     CUDA_OK(cudaStreamSynchronize(stream));
     std::lock_guard<std::mutex> lock(s->mu);
+    s->last_read_bytes = read_bytes;
     s->cache_lists = lists;
     s->cache_pool = pool;
     s->cache_stage = stage;
@@ -3300,10 +3550,14 @@ const Param<Spann> kSpannParams[] = {
      }},
     // host placement (sptag_b200_spann_load_ex): the HBM stage per staging set, and what the placement holds and gathered
     {"B200.PostingStageBytes", &Spann::stage_bytes, 0, 0, INT_MAX},
-    {"B200.PostingPlacement", [](Spann* s, char* o, size_t n) { return put(o, n, "%s", s->host_postings ? "host" : "device"); }},
+    {"B200.PostingPlacement", [](Spann* s, char* o, size_t n) {
+         return put(o, n, "%s", s->file_postings ? "file" : s->host_postings ? "host" : "device");
+     }},
     {"B200.PostingHostBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%zu", s->h_posting_bytes); }},
     {"B200.LastGatherBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_gather_bytes); }},
     {"B200.LastGatherRounds", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_gather_rounds); }},
+    // file placement: the posting-file bytes the last search, iterator step or cache install read
+    {"B200.LastReadBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%ld", s->last_read_bytes); }},
     // the HBM cache of lists (sptag_b200_spann_cache_lists): its lists and the pool's bytes
     {"B200.PostingCacheLists", [](Spann* s, char* o, size_t n) { return put(o, n, "%zu", s->cache_lists.size()); }},
     {"B200.PostingCacheBytes", [](Spann* s, char* o, size_t n) { return put(o, n, "%lld", s->cache_bytes); }},
@@ -3361,7 +3615,7 @@ constexpr int kPostingsPortable = -1;
 
 // Everything sptag_b200_spann_load reads after the head: the head's [BuildHead] parameters, the search parameters, the
 // translate map and the posting files, with the lists' rows and ids placed as `placement` says (SPTAG_B200_POSTINGS_*,
-// or kPostingsPortable).  With `shared` (a group's later members: the portable allocation of shared_bytes its first
+// or kPostingsPortable; FILE reads only the files' headers).  With `shared` (a group's later members: the portable allocation of shared_bytes its first
 // member filled from the same folder) the lists' bodies are not read again: the handle maps that allocation, which it
 // does not own.  The caller destroys s on failure.
 int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& ini, int placement, void* shared = nullptr,
@@ -3398,11 +3652,13 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
     // the posting files: SSDIndex, SSDIndex_1, ... while they exist (ExtraFullGraphSearcher.h:165-206)
     FileCloser fc;
     std::vector<PostingFile> files;
+    std::vector<std::string> paths;
     const std::string base = dir + "/" + get("BuildSSDIndex", "SSDIndex", get("Base", "SSDIndex", "SPTAGFullList.bin").c_str());
     for (std::string cur = base;; cur = base + "_" + std::to_string(files.size())) {
         FILE* f = fc.open(cur);
         if (!f) break;
         files.emplace_back();
+        paths.push_back(cur);
         if (int rc = read_posting_header(f, files.back(), cur.c_str())) return rc;
         if (files.back().dim != head->dim)
             return fail(SPTAG_B200_DIMENSION_MISMATCH, "%s: dimension %d, head index %d", cur.c_str(), files.back().dim, head->dim);
@@ -3453,7 +3709,7 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
         ids_base = (int32_t*)(rows_base + rows_bytes);
         s->h_rows = rows_base;
         s->h_ids = ids_base;
-    } else {
+    } else if (placement != SPTAG_B200_POSTINGS_FILE) {
         if (int rc = s->d_ids.ensure(ids_bytes)) return rc;
         if (int rc = s->d_rows.ensure(rows_bytes)) return rc;
         CUDA_OK(cudaMemset(s->d_rows.ptr, 0, s->d_rows.bytes));
@@ -3464,7 +3720,30 @@ int spann_fill(sptag_b200_spann* s, const std::string& dir, const IniSections& i
     CUDA_OK(cudaMemcpy(s->d_off.ptr, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(s->d_cnt.ptr, s->cnt.data(), off.size() * 4, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(s->d_pages.ptr, s->pages.data(), off.size() * 4, cudaMemcpyHostToDevice));
-    if (shared) {
+    if (placement == SPTAG_B200_POSTINGS_FILE) {
+        // The lists stay in their files, whose descriptors the handle keeps (dups of the ones the headers were read
+        // from).  Nothing is read before the first search, so every list's extent is checked here.
+        size_t first_list = 0;
+        for (size_t fi = 0; fi < files.size(); ++fi) {
+            const PostingFile& pf = files[fi];
+            const long long fsz = file_size(pf.f);
+            for (int i = 0; i < pf.lists; ++i) {
+                if (pf.cnt[i] > 0 && pf.start[i] + (long long)pf.cnt[i] * s->vis > fsz)
+                    return fail(SPTAG_B200_FAIL, "posting list %zu runs past the end of its file %s", first_list + i,
+                                paths[fi].c_str());
+                s->list_file.push_back((int)fi);
+                s->list_start.push_back(pf.start[i]);
+            }
+            first_list += (size_t)pf.lists;
+            const int fd = fcntl(fileno(pf.f), F_DUPFD_CLOEXEC, 0);
+            if (fd < 0) return fail(SPTAG_B200_FAILED_OPEN_FILE, "cannot keep %s open: %s", paths[fi].c_str(), strerror(errno));
+            s->post_files.fds.push_back(fd);
+            s->post_files.paths.push_back(paths[fi]);
+        }
+        s->host_postings = s->file_postings = true;
+        s->readers.reset(new ReadPool(std::min(16u, std::max(1u, std::thread::hardware_concurrency()))));
+    }
+    if (shared || s->file_postings) {
         std::lock_guard<std::mutex> lock(s->mu);
         spann_update_shape(s);
         return 0;
@@ -4623,7 +4902,7 @@ int sptag_b200_spann_load_ex(const char* folder, int32_t device, const sptag_b20
                         sizeof(sptag_b200_spann_load_options));
         placement = options->posting_placement;
         if (placement != SPTAG_B200_POSTINGS_AUTO && placement != SPTAG_B200_POSTINGS_DEVICE &&
-            placement != SPTAG_B200_POSTINGS_HOST)
+            placement != SPTAG_B200_POSTINGS_HOST && placement != SPTAG_B200_POSTINGS_FILE)
             return fail(SPTAG_B200_LACK_OF_INPUTS, "unknown posting placement %d", placement);
     }
     return spann_open(folder, device, placement, nullptr, 0, out);
@@ -4783,7 +5062,7 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
     if (s->host_postings) {
         // the queries' chosen lists, once; then the rounds, each a scan over its queries on the staged lists
         const int stride = std::max(p.internal, 1);
-        long bytes = 0, rounds = 0, peer_bytes = 0;
+        long bytes = 0, rounds = 0, peer_bytes = 0, read_bytes = 0;
         int rc = 0;
         if (!(rc = st->d_chosen.ensure(nq * stride * 4)) && !(rc = st->d_nchosen.ensure(nq * 4))) {
             const cudaError_t e = launch_spann_choose(p, (int*)st->d_chosen.ptr, (int*)st->d_nchosen.ptr, stride, stream);
@@ -4814,7 +5093,8 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
             if (err != cudaSuccess) return fail(SPTAG_B200_FAIL, "posting scan launch failed: %s", cudaGetErrorString(err));
             return 0;
         };
-        if (!rc) rc = gather_rounds(s, *st, sp, num_queries, stride, stream, choose, run, bytes, rounds, peer_bytes);
+        if (!rc)
+            rc = gather_rounds(s, *st, sp, num_queries, stride, stream, choose, run, bytes, rounds, peer_bytes, read_bytes);
         if (rc) {
             cudaStreamSynchronize(stream);
             return rc;
@@ -4823,6 +5103,7 @@ int sptag_b200_spann_search(sptag_b200_spann_handle s, const void* queries, int3
         s->last_gather_bytes = bytes;
         s->last_gather_rounds = rounds;
         s->last_peer_gather_bytes = peer_bytes;
+        s->last_read_bytes = read_bytes;
     } else {
         cudaError_t e = s->quantized ? launch_spann_pq_scan(pq, grid, stream, &kern)
                                      : launch_spann_scan(p, me.cosine, me.elem, grid, stream, &kern);
@@ -5267,7 +5548,7 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
     decltype(s->staging.acquire(slock)) gs = nullptr;
     if (s->host_postings)
         if (int rc = spann_acquire_fitted(s, sp, slock, gs)) return rc;
-    long gather_bytes = 0, gather_rounds_n = 0, gather_peer_bytes = 0;
+    long gather_bytes = 0, gather_rounds_n = 0, gather_peer_bytes = 0, read_bytes = 0;
     if (gs) {
         if (int rc = gs->d_chosen.ensure(nq * it->hb * 4)) return rc;
         if (int rc = gs->d_nchosen.ensure(nq * 4)) return rc;
@@ -5291,7 +5572,7 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
             return step(r, e - b);
         };
         return gather_rounds(s, *gs, sp, (int)n, it->hb, stream, choose, run, gather_bytes, gather_rounds_n,
-                             gather_peer_bytes);
+                             gather_peer_bytes, read_bytes);
     };
     // Rounds: the posting step over the queries of the round; queries whose tables must grow run again (same round);
     // then the head's FromNeareast(false) for the queries whose postings ran out, and the posting step over those.
@@ -5333,6 +5614,7 @@ int sptag_b200_spann_iterator_next(sptag_b200_spann_iter it, int32_t batch, int3
         s->last_gather_bytes = gather_bytes;
         s->last_gather_rounds = gather_rounds_n;
         s->last_peer_gather_bytes = gather_peer_bytes;
+        s->last_read_bytes = read_bytes;
     }
     return SPTAG_B200_SUCCESS;
 }
